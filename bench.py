@@ -2,8 +2,9 @@
 """bench.py -- the measurement contract (one JSON line on stdout from rank 0).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME] [--no-secondary]
+                    [--dump-outputs DIR]
 
-N > 1 is launched by the driver as
+N > 1 is launched as
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 one rank per GPU; the batch (independent sequences) is sharded across ranks with no data-path
 collective; one NCCL all_gather of per-rank result checksums per step replaces the reference's
@@ -13,6 +14,10 @@ events), max over ranks, barrier + synchronize on both sides.
 The main line is BASELINE cfg 3 (benchmarks/workloads.py::InterleavedCfg3) through the reference surface
 ``MMInterleaved.forward``; the other BASELINE configurations that fit one GPU (cfg 2, cfg 4, cfg 5) are timed
 afterwards with the same procedure at a few steps each and attached as ``"secondary": {name: {...}}`` objects.
+
+``--dump-outputs DIR`` writes what the main workload's last timed step returned (``DIR/<name>.npy``: integer arrays as
+float64, floating ones as float32; an array of more than DUMP_SAMPLE elements is replaced by a fixed seeded sample of
+that many, so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -39,6 +44,8 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the cfg 2 / cfg 4 / cfg 5 secondary measurements")
     ap.add_argument("--secondary", default="", help="comma-separated subset of secondary workloads to run")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's outputs of the main workload as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -91,7 +98,30 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def measure(wl, steps, warmup, dist, rank, world, local_rank, cpu_baseline):
+DUMP_SAMPLE = 1 << 22             # elements kept per dumped array (16 MiB as float32)
+DUMP_LIMIT = 64 * 1024 * 1024     # bytes over all dumped arrays
+
+
+def dump_outputs(outputs, out_dir):
+    """Write {name: tensor} as out_dir/<name>.npy (float64 for integer tensors, float32 otherwise)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, t in outputs.items():
+        t = t.detach().reshape(-1)
+        if t.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randint(0, t.numel(), (DUMP_SAMPLE,), generator=g).sort().values
+            t = t[idx.to(t.device)]
+        a = t.to("cpu", torch.float32 if t.is_floating_point() else torch.float64).numpy()
+        total += a.nbytes
+        if total > DUMP_LIMIT:
+            raise SystemExit(f"--dump-outputs: more than {DUMP_LIMIT} bytes at {name}")
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
+def measure(wl, steps, warmup, dist, rank, world, local_rank, cpu_baseline, dump_dir=""):
     """The timing procedure of the contract for one workload; returns its result object."""
     import torch
 
@@ -123,6 +153,8 @@ def measure(wl, steps, warmup, dist, rank, world, local_rank, cpu_baseline):
         ev[i][1].record()
     barrier()
     t_wall1 = time.time()
+    if dump_dir and rank == 0:
+        dump_outputs(wl.outputs(), dump_dir)
     step_ms = [a.elapsed_time(b) for a, b in ev]
     total_ms = torch.tensor([sum(step_ms)], dtype=torch.float64, device="cuda")
     if dist is not None:
@@ -199,7 +231,8 @@ def main():
 
     wl = workloads.make(args.workload, rank=rank, world=world, local_batch=args.local_batch)
     wl.setup()
-    line = measure(wl, args.steps, args.warmup, dist, rank, world, local_rank, cpu_baseline=not args.no_cpu_baseline)
+    line = measure(wl, args.steps, args.warmup, dist, rank, world, local_rank, cpu_baseline=not args.no_cpu_baseline,
+                   dump_dir=args.dump_outputs)
     wl.teardown()
 
     main_name = workloads.AUTO if args.workload == "auto" else args.workload

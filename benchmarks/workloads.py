@@ -19,27 +19,19 @@ import time
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+FLUSH_MIB = 128                                 # written between timed steps: well over the H100's 50 MB L2
 SOI_ID, IMG_ID, BOS_ID = 32000, 32001, 1       # mm_interleaved.py:33-39 / wds_utils.py:203
 
 
 def measured_peaks():
-    """Roofline denominators: the driver-written MEASURED_PEAKS.json, else the profiling guide's
-    stated fallback (6.65 TB/s, 1.59 PFLOP/s)."""
+    """Roofline denominators: MEASURED_PEAKS.json when present, else NVIDIA's H100 SXM data-sheet figures
+    (3.35 TB/s HBM3, 989 TFLOP/s dense BF16 at up to 700 W)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d["bf16_tflops"]),
                 "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
-
-
-def ncu_traffic(kernel_key):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch from the committed ``ncu --set full`` capture named in
-    profiles/traffic.json ({key: {"bytes_per_launch": ..., "batch": ..., "source": "profiles/<file>"}}); None if absent."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if not os.path.exists(p):
-        return None
-    return json.load(open(p)).get(kernel_key)
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 def msda_algorithmic_bytes(N, S, M, D, L, Lq, P, elem_size):
@@ -138,7 +130,7 @@ class Workload:
     # -- shared helpers -----------------------------------------------------------------
     def flush_l2(self):
         if self._flush is None:
-            self._flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+            self._flush = torch.empty(FLUSH_MIB * 1024 * 1024, dtype=torch.uint8, device="cuda")
         self._flush.zero_()
 
     def reset_counters(self):
@@ -172,6 +164,11 @@ class Workload:
 
     def teardown(self):
         pass
+
+    def outputs(self):
+        """{name: tensor} of what the last device step returned to its caller."""
+        last = self.last if isinstance(self.last, (tuple, list)) else (self.last,)
+        return {f"out{i}": t for i, t in enumerate(last)}
 
 
 def _timed(events_list, fn, count=None):
@@ -290,7 +287,7 @@ class MsdaCfg3(Workload):
                             f"{self.B} sequences/GPU (L=12,S=5376,Lq=2048,M=16,D=64,P=8)",
                 "step_unit": f"the 10 sampler launches of {self.B} sequences", "sequences_per_step": self.B,
                 "global_batch": self.B * self.world, "seq_len": 2048, "images_per_seq": 4,
-                "parallelism": f"dp{self.world}", "l2": "192 MiB buffer written between timed steps (L2 flush)"}
+                "parallelism": f"dp{self.world}", "l2": f"{FLUSH_MIB} MiB buffer written between timed steps (L2 flush)"}
 
     def roofline(self, kernel):
         peaks = measured_peaks()
@@ -426,6 +423,7 @@ class InterleavedCfg3(Workload):
         with torch.no_grad():
             out = self.model(text_ids=ids, image_tensors=images, num_image_per_seq=nimg, attention_mask=None,
                              max_num_image=self.N_IMG, return_loss=False)
+            self.last_logits = out["text_logits"]
             return out["text_logits"].argmax(-1)
 
     def step_device(self):
@@ -443,6 +441,9 @@ class InterleavedCfg3(Workload):
 
     def result_checksum(self):
         return self.last.sum().reshape(1).float()
+
+    def outputs(self):
+        return {"text_ids": self.last, "text_logits": self.last_logits}
 
     def h2d_bytes(self):
         return sum(t.numel() * t.element_size() for t in self.host)
@@ -467,7 +468,7 @@ class InterleavedCfg3(Workload):
                 "parallelism": f"dp{self.world}",
                 "params": "13B Llama + 10 MMFS layers + 0.45B visual tokenizer (+ 1.3B image decoder resident, unused here), random init, bf16",
                 "inputs": f"{self.N_SETS} distinct image/token sets rotated step by step (no cross-step reuse of image-side work)",
-                "l2": "192 MiB buffer written between timed steps (L2 flush); weights (27 GB) exceed L2 anyway",
+                "l2": f"{FLUSH_MIB} MiB buffer written between timed steps (L2 flush); weights (27 GB) exceed L2 anyway",
                 "cuda_graph": "visual tokenizer captured once per image-batch shape inside MMInterleaved and replayed; decoder eager"}
 
     def roofline(self, kernel):
@@ -481,16 +482,14 @@ class InterleavedCfg3(Workload):
         achieved = ab / t / 1e9 if t else None
         flops = 4.0 * self.B * self.T * self.T * 5120 / 2                     # causal QK^T + PV per layer
         ta = kernel["attn_avg_ms"] * 1e-3 if kernel.get("attn_avg_ms") else None
-        tr = ncu_traffic(f"mmfs_sampler_{self.label}")
         return {"kernel": "mmfs_sampler_v2_kernel<bf16,3 levels> (fused MMFS deform-attn sampler)", "bound": "hbm",
                 "achieved": achieved, "peak": peaks["hbm_gbs"], "peak_source": peaks["source"], "unit": "GB/s",
                 "frac": achieved / peaks["hbm_gbs"] if achieved else None,
                 "algorithmic_bytes_per_launch": ab, "fused_kernel_bytes_per_launch": fused,
                 "achieved_fused_bytes_GBs": fused / t / 1e9 if t else None,
                 "avg_launch_us": t * 1e6 if t else None, "launches_timed": kernel["launches"],
-                "traffic": tr["bytes_per_launch"] * self.B / tr["batch"] if tr else None,
-                "traffic_source": tr["source"] if tr else None,
-                "attention": {"kernel": "attn_fwd_kernel<bf16,128> (tcgen05)", "bound": "tensor",
+                "traffic": None,                          # DRAM bytes need a profiler capture; none is run here
+                "attention": {"kernel": "attn_fwd_kernel<bf16,128> (wgmma)", "bound": "tensor",
                               "achieved": flops / ta / 1e12 if ta else None, "peak": peaks["bf16_tflops_sustained"],
                               "unit": "TFLOP/s", "frac": flops / ta / 1e12 / peaks["bf16_tflops_sustained"] if ta else None,
                               "flops_per_launch": flops, "avg_launch_us": ta * 1e6 if ta else None,
@@ -567,7 +566,7 @@ class InterleavedCfg3(Workload):
 
 
 class InterleavedCfg2(InterleavedCfg3):
-    """BASELINE cfg 2: CLIP ViT-L/14 encode + Llama-13B prefill, 1-image context, seq_len 512, bf16, one B200
+    """BASELINE cfg 2: CLIP ViT-L/14 encode + Llama-13B prefill, 1-image context, seq_len 512, bf16, one GPU
     (the same ``MMInterleaved.forward`` call as cfg 3 on shorter single-image sequences)."""
 
     name = "interleaved_cfg2"
@@ -665,6 +664,9 @@ class SdCfg4(Workload):
     def result_checksum(self):
         return self.last.float().sum().reshape(1)
 
+    def outputs(self):
+        return {"latents": self.last}
+
     def h2d_bytes(self):
         return sum(t.numel() * t.element_size() for t in self.host)
 
@@ -691,14 +693,14 @@ class SdCfg4(Workload):
     def config(self):
         return {"workload": f"BASELINE cfg4: SD-2.1-base UNet (866 M params, random init) {self.STEPS}-step CFG denoise through "
                             f"StableDiffusion.generate_images, latents ({2 * self.B},4,64,64), ctx (77,1024), MMFSNet (13 blocks) on 1 "
-                            "context image, DDPM scheduler (sd.py:48-50); 3x3/1x1 convs (tcgen05 implicit GEMM), GroupNorm+SiLU, GEGLU, "
+                            "context image, DDPM scheduler (sd.py:48-50); 3x3/1x1 convs (wgmma implicit GEMM), GroupNorm+SiLU, GEGLU, "
                             "attention, LayerNorm, MMFS = this repo's kernels; conv_in/conv_out + Linear GEMMs = cuDNN/cuBLAS; VAE not run",
                 "step_unit": f"one {self.STEPS}-step denoise of the rank-local batch of {self.B} images (2B UNet rows for CFG)",
                 "images_per_step": self.B, "global_batch": self.B * self.world, "parallelism": f"dp{self.world}",
                 "cuda_graph": "UNet evaluation captured once per shape and kept across generate_images calls "
                               "(StableDiffusion.enable_cuda_graphs); per call the context, mask and MMFS image-side state are "
                               "refreshed in place; scheduler steps eager; roofline kernels timed in separate eager evaluations",
-                "l2": "192 MiB buffer written between timed steps"}
+                "l2": f"{FLUSH_MIB} MiB buffer written between timed steps"}
 
     def roofline(self, kernel):
         peaks = measured_peaks()
@@ -707,12 +709,12 @@ class SdCfg4(Workload):
         tc = kernel["avg_ms"] * 1e-3 if kernel["avg_ms"] else None
         flops = 4.0 * (2 * self.B) * 4096 * 4096 * 320                   # self-attn at T=4096, C=320 (5 x 64)
         t = kernel["attn_avg_ms"] * 1e-3 if kernel.get("attn_avg_ms") else None
-        return {"kernel": f"conv_igemm_kernel<bf16> (tcgen05 implicit GEMM), {cin}->{cout} {side}x{side} {ks}x{ks}, batch {2 * self.B}",
+        return {"kernel": f"conv_igemm_kernel<bf16> (wgmma implicit GEMM), {cin}->{cout} {side}x{side} {ks}x{ks}, batch {2 * self.B}",
                 "bound": "tensor", "achieved": cflops / tc / 1e12 if tc else None, "peak": peaks["bf16_tflops_sustained"],
                 "unit": "TFLOP/s", "frac": cflops / tc / 1e12 / peaks["bf16_tflops_sustained"] if tc else None,
                 "flops_per_launch": cflops, "avg_launch_us": tc * 1e6 if tc else None, "launches_timed": kernel["launches"],
                 "traffic": None,
-                "attention": {"kernel": "attn_fwd_kernel<bf16,64> (tcgen05), UNet self-attention at T=4096 (5 heads x 64)",
+                "attention": {"kernel": "attn_fwd_kernel<bf16,64> (wgmma), UNet self-attention at T=4096 (5 heads x 64)",
                               "bound": "tensor", "achieved": flops / t / 1e12 if t else None,
                               "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s",
                               "frac": flops / t / 1e12 / peaks["bf16_tflops_sustained"] if t else None,
@@ -811,6 +813,9 @@ class GenerateCfg5(Workload):
     def result_checksum(self):
         return (self.last[0].sum().float() + self.last[1].float().sum()).reshape(1)
 
+    def outputs(self):
+        return {"text_ids": self.last[0], "image_latents": self.last[1]}
+
     def h2d_bytes(self):
         return sum(t.numel() * t.element_size() for t in self.host)
 
@@ -828,7 +833,7 @@ class GenerateCfg5(Workload):
                 "global_batch": self.world, "seq_len": self.T, "images_per_seq": self.N_IMG, "parallelism": f"dp{self.world}",
                 "cuda_graph": "visual tokenizer graph + one decode-step graph replayed per generated token (enable_decode_graphs) + "
                               "the UNet evaluation graph kept across calls",
-                "l2": "192 MiB buffer written between timed steps"}
+                "l2": f"{FLUSH_MIB} MiB buffer written between timed steps"}
 
     def roofline(self, kernel):
         peaks = measured_peaks()

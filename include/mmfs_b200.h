@@ -1,5 +1,5 @@
 /*
- * include/mmfs_b200.h -- C ABI of libmmfs_b200.so (hand-written sm_100a kernels for
+ * include/mmfs_b200.h -- C ABI of libmmfs_b200.so (hand-written sm_90a kernels for
  * the MM-Interleaved interleaved image-text forward hot path).
  *
  * Plain pointers and sizes only: no torch / ATen types cross this boundary.  Every
@@ -41,13 +41,13 @@ extern "C" {
                                reference multiplies them in, which only matters when
                                `value` holds inf/nan); default skips those fetches */
 #define MMFS_MSDA_W16    2u /* 16-bit element types only: round each tap weight (lerp * attention weight) to the
-                               element type and accumulate with the mixed-precision FMA (fma.rn.f32.bf16/f16,
-                               SASS FHFMA) -- fewer instructions per fetch; the reference keeps fp32 weights, so
+                               element type and accumulate value x weight with one fp32 FMA of the widened 16-bit
+                               operands -- fewer instructions per fetch; the reference keeps fp32 weights, so
                                this is opt-in (error << one storage ulp of the result) */
 
 /* flags for mmfs_sampler_forward (in addition to MMFS_MSDA_STRICT) */
 #define MMFS_SAMPLER_EXACT_WEIGHTS 4u /* keep fp32 tap weights in the specialised 16-bit kernel (default there: weights
-                                         rounded to the element type, FHFMA accumulate; bound in mmfs_sampler_v2_sm100.cu) */
+                                         rounded to the element type, mixed-precision FMA accumulate; bound in mmfs_sampler_v2_sm100.cu) */
 #define MMFS_SAMPLER_GENERIC       8u /* force the generic kernel (A/B runs, tests) */
 
 int mmfs_abi_version(void);
@@ -133,7 +133,7 @@ void mmfs_release_scratch(void);
  * plain tile order instead of the per-SM swizzle. */
 int mmfs_msda_set_tuning(int rows_per_warp, int mapping);
 /* Same for the specialised fused sampler: rows per warp per tile (0 = automatic); wmode 1 = 16-bit tap weights +
- * FHFMA (default), 0 = fp32 tap weights everywhere. */
+ * mixed-precision FMA (default), 0 = fp32 tap weights everywhere. */
 int mmfs_sampler_set_tuning(int rows_per_warp, int wmode);
 
 /*
@@ -247,7 +247,7 @@ int mmfs_attn_decode(const void *q, const void *k, const void *v, void *out, con
                      float scale, int causal, int past, int dtype, void *stream);
 
 /*
- * softmax(q k^T * scale + mask) v on the tensor cores (tcgen05.mma, TMEM accumulators, TMA tiles):
+ * softmax(q k^T * scale + mask) v on the tensor cores (wgmma, register accumulators, TMA tiles):
  * the prefill path.  Same argument meaning as mmfs_attn_generic; requires hd in {64, 128}, dtype
  * bf16 / f16, 16-byte aligned pointers and strides (MMFS_EUNSUPPORTED otherwise -- callers route
  * those cases to mmfs_attn_generic).  Replaces LlamaAttention.forward's eager attention
@@ -259,9 +259,9 @@ int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, co
                       long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
                       float scale, int causal, int past, int dtype, void *stream);
 
-/* The same op as a PERSISTENT kernel: 2 CTAs per SM walk the (batch, query tile, head) items handed out by an atomic
- * counter, with barriers / TMEM / tensor maps set up once and the next item's loads and first MMA overlapping the
- * current item's O read-out.  Taken when there are more items than resident CTAs (else the call runs the kernel above).
+/* The same op as a PERSISTENT kernel: the resident CTAs (1 per SM at hd 128, 2 at hd 64) walk the (batch, query tile,
+ * head) items handed out by an atomic counter, with barriers and tensor maps set up once and the K / V ring running on
+ * across items.  Taken when there are more items than resident CTAs (else the call runs the kernel above).
  * work_counter: one device uint32 that is ZERO when the kernel starts and private to the call until it completes. */
 int mmfs_attn_forward_persistent(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
                                  int B, int H, int Tq, int Tkv, int hd,
@@ -269,7 +269,7 @@ int mmfs_attn_forward_persistent(const void *q, const void *k, const void *v, vo
                                  float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream);
 
 /*
- * 2-D convolution as an implicit GEMM on the tensor cores (tcgen05, TMA-shifted input boxes, no im2col buffer).
+ * 2-D convolution as an implicit GEMM on the tensor cores (wgmma, TMA-shifted input boxes, no im2col buffer).
  * Replaces the cuDNN convolutions diffusers' UNet issues in the denoise step (called from
  * utils/monkey_patch/sd_unet_forward_monkey_patch.py:235-366; 3x3 stride 1/2 and 1x1, NHWC).
  *   x (B,H,W,Cin) NHWC; w (Cout,KH,KW,Cin); out (B,Ho,Wo,Cout) NHWC; optional fused epilogue terms: bias (Cout),

@@ -1,4 +1,4 @@
-"""mm_interleaved_b200 -- B200-native (sm_100a) kernels for MM-Interleaved's interleaved
+"""mm_interleaved_b200 -- H100-native (sm_90a) kernels for MM-Interleaved's interleaved
 image-text forward hot path, behind the reference's own operator / module API.
 
 Import name ``mm_interleaved_b200`` (via the shim ``mm_interleaved_b200.py`` at the repo

@@ -1,5 +1,5 @@
-"""CUDA-graph replay of launch-bound sub-graphs (SURVEY.md 8 f3): the visual tokenizer is ~2400 kernels of 5-50 us per
-16 images and one decode step is ~1000 small kernels -- issued eagerly, the host cannot keep the GPU busy.
+"""CUDA-graph replay of launch-bound sub-graphs (SURVEY.md 8 f3): the visual tokenizer is ~2400 small kernels per 16
+images and one decode step is ~1000 small kernels -- issued eagerly, the host cannot keep the GPU busy.
 
 ``GraphedCallable`` captures ``fn(*tensors)`` once per input signature (shapes, dtypes, device) over private static
 input buffers and replays it on later calls after copying the new inputs in.  The returned tensors live in the

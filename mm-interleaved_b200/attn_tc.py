@@ -1,4 +1,4 @@
-"""Dispatch to the tcgen05 flash-attention kernel (csrc/attn_fwd_sm100.cu)."""
+"""Dispatch to the wgmma flash-attention kernel (csrc/attn_fwd_sm100.cu)."""
 from __future__ import annotations
 
 import os
@@ -27,7 +27,9 @@ def forward(q, k, v, out, key_mask, causal, past, scale):
     sms = _SMS.get(q.device.index)
     if sms is None:
         sms = _SMS[q.device.index] = torch.cuda.get_device_properties(q.device).multi_processor_count
-    if PERSISTENT and B * H * ((Tq + 127) // 128) > 2 * sms:
+    # resident CTAs per SM: 1 at hd 128, 2 at hd 64 (attn_ctas_per_sm in csrc/attn_fwd_sm100.cu); the persistent
+    # kernel only pays off with more items than resident CTAs
+    if PERSISTENT and B * H * ((Tq + 127) // 128) > (2 if hd == 64 else 1) * sms:
         # one zeroed word per call (a fill kernel; inside a CUDA graph it is re-zeroed on every replay): the kernel's
         # work counter must be private to the launch
         counter = torch.zeros((1,), dtype=torch.int32, device=q.device)
@@ -37,7 +39,7 @@ def forward(q, k, v, out, key_mask, causal, past, scale):
                 B, H, Tq, k.shape[1], hd, q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1),
                 out.stride(0), out.stride(1), float(scale), 1 if causal else 0, int(past), _DTYPE_CODE[q.dtype],
                 counter.data_ptr(), torch.cuda.current_stream().cuda_stream)
-        _lib.check(rc, "attention (tcgen05, persistent)")
+        _lib.check(rc, "attention (wgmma, persistent)")
         return
     with torch.cuda.device(q.device):
         rc = _lib.lib().mmfs_attn_forward(
@@ -45,4 +47,4 @@ def forward(q, k, v, out, key_mask, causal, past, scale):
             B, H, Tq, k.shape[1], hd, q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1),
             out.stride(0), out.stride(1), float(scale), 1 if causal else 0, int(past), _DTYPE_CODE[q.dtype],
             torch.cuda.current_stream().cuda_stream)
-    _lib.check(rc, "attention (tcgen05)")
+    _lib.check(rc, "attention (wgmma)")

@@ -1,9 +1,9 @@
-"""Build libmmfs_b200.so in-tree with nvcc for sm_100a (no torch headers involved).
+"""Build libmmfs_b200.so in-tree with nvcc for sm_90a (no torch headers involved).
 
     python mm-interleaved_b200/build.py [--force]
 
-The library lands next to this file so that it travels with the repository snapshot to
-the GPU box; it is git-ignored (built artefact).
+The library lands next to this file, so the package imports from the repository tree;
+it is git-ignored (built artefact).
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmmfs_b200.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
 ]
 
@@ -53,7 +53,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     for src, p in procs:
         if p.wait() != 0:
             raise RuntimeError(f"nvcc failed on {src}")
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB, *objs, "-lcudart"])
+    subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB, *objs, "-lcudart"])
     return LIB
 
 

@@ -1,4 +1,4 @@
-// attn_common.cuh -- parameter block and register-level helpers of the tcgen05 attention kernel (attn_fwd_sm100.cu).
+// attn_common.cuh -- parameter block and register-level helpers of the wgmma attention kernel (attn_fwd_sm100.cu).
 #pragma once
 #include <stdlib.h>
 
@@ -6,19 +6,12 @@
 
 namespace mmfs {
 
-constexpr float kRescaleThreshold = 8.f;   // lazy O rescale: only when the running max grows by > 2^8 (exact)
-
-template <typename T> struct AttnFmt;
-template <> struct AttnFmt<__nv_bfloat16> { static constexpr int code = 1; };
-template <> struct AttnFmt<__half> { static constexpr int code = 0; };
-
 struct AttnParams {
     void *out;                 // (B, Tq, H, hd), strides o_bs / o_ts elements
     const uint8_t *key_mask;   // (B, Tkv) or null
     int B, H, Tq, Tkv, causal, past;
     long o_bs, o_ts;
     float scale_log2e;         // scale * log2(e)
-    int debug;                 // timing experiments only (env MMFS_ATTN_DEBUG): 1 = no softmax math, 2 = no MMAs; results are garbage
 };
 
 template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b);
@@ -35,44 +28,5 @@ __device__ __forceinline__ float fast_exp2(float x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// packed fp32 pairs (Blackwell fma.rn.f32x2 / add.rn.f32x2: two lanes per issue slot)
-__device__ __forceinline__ uint64_t pack_f32x2(float a, float b) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t v, float &a, float &b) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-}
-__device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-// two back-to-back 32-column TMEM loads, one wait
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, float (&v)[64]) {
-    uint32_t r[64];
-#pragma unroll
-    for (int hlf = 0; hlf < 2; ++hlf) {
-        uint32_t *q = r + 32 * hlf;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-            : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]), "=r"(q[8]), "=r"(q[9]),
-              "=r"(q[10]), "=r"(q[11]), "=r"(q[12]), "=r"(q[13]), "=r"(q[14]), "=r"(q[15]), "=r"(q[16]), "=r"(q[17]), "=r"(q[18]),
-              "=r"(q[19]), "=r"(q[20]), "=r"(q[21]), "=r"(q[22]), "=r"(q[23]), "=r"(q[24]), "=r"(q[25]), "=r"(q[26]), "=r"(q[27]),
-              "=r"(q[28]), "=r"(q[29]), "=r"(q[30]), "=r"(q[31])
-            : "r"(taddr + 32u * hlf));
-    }
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 64; ++i) v[i] = __uint_as_float(r[i]);
-}
-
 
 }  // namespace mmfs

@@ -1,4 +1,4 @@
-// attn_fwd_sm100.cu -- softmax(Q K^T * scale + mask) V on the 5th-generation tensor cores.
+// attn_fwd_sm100.cu -- softmax(Q K^T * scale + mask) V on the Hopper tensor cores (wgmma).
 //
 // Replaces, for prefill-sized problems,
 //   LlamaAttention.forward's eager path      decoders/modeling_llama_mmfs.py:246-264
@@ -7,351 +7,60 @@
 //       memory_efficient_attention, non-causal, T = 257, 16 x 64)
 //   the SD-UNet self-/cross-attention        decoders/sd.py:64-65 (xformers)
 //
-// B200-first design (hand-written PTX, no CUTLASS):
-//   * one CTA per (128 query rows, head, batch entry); Q / K / V tiles arrive by TMA
-//     (cp.async.bulk.tensor.4d, SWIZZLE_128B) straight from the projection GEMM's (B, T, H, hd)
-//     layout -- no transposes, K and V double-buffered;
-//   * S = Q K^T and O += P V are tcgen05.mma (cta_group::1, kind::f16, M = 128) issued by ONE
-//     thread; accumulators live in TMEM: two S buffers (2 x 128 columns) so that S_{j+1} is
-//     computed while the softmax of S_j runs, plus the O accumulator (hd columns);
-//   * 4 softmax warps own one TMEM lane (= one query row) per thread: tcgen05.ld the scores, online
-//     softmax in fp32 (packed fma/add.f32x2, MUFU exp2), P written back as 16-bit pairs into the first
-//     32 columns of the SAME S buffer (tcgen05.st) and consumed by the second MMA as a TMEM A operand
-//     -- no shared-memory P tile, no proxy fence, no wait on the previous P V; O is rescaled in TMEM
-//     lazily.  (Measured alternatives that lost: 8 softmax warps with two threads per row, -15 %;
-//     one-lane-per-warp mbarrier arrive/wait, no change.)
-//   * V is consumed as an MN-major B operand exactly as TMA delivers it (no transpose);
-//   * causal tiles above the diagonal are never loaded; causal / key-padding / tail masks are
-//     applied on the scores in registers; the (B,1,T,T) additive mask is never built.
-// Roofline: tensor pipe (2 * 2 * 128*128*hd flop per KV tile); the MUFU exp2 of the softmax is the
-// co-limiter (128*128 exps per tile at 16/clk/SM), see DESIGN.md.
+// Design (hand-written PTX, no CUTLASS):
+//   * one work item = (128 query rows, head, batch entry); Q / K / V tiles arrive by TMA (cp.async.bulk.tensor.4d,
+//     SWIZZLE_128B) straight from the projection GEMM's (B, T, H, hd) layout -- no transposes, K and V double-buffered;
+//   * warps 0-3 and 4-7 are two consumer warpgroups of 64 query rows each, warp 8 is the TMA producer;
+//   * S = Q K^T is wgmma m64n64k16 with both operands in shared memory; the online softmax runs on the fp32
+//     accumulator fragment in registers (row max / sum over the 4 lanes of a quad), P is packed to 16 bit in
+//     registers and fed to O += P V as the register A operand (wgmma m64n{hd}k16, V MN-major exactly as TMA
+//     delivers it); O stays in registers for the whole item;
+//   * causal tiles above the diagonal are never loaded; causal / key-padding / tail masks are applied on the
+//     scores in registers; the (B,1,T,T) additive mask is never built.
+// One CTA per SM at hd 128 (139 registers per thread), two at hd 64.  With more items than resident CTAs the kernel
+// is persistent: the producer hands out items through an atomic counter (longest causal query tile first, heads
+// fastest inside a batch entry, so that the resident CTAs share one batch entry's K / V in L2), and every
+// barrier phase runs on a global tile counter, so the K / V ring continues across items without a drain.
 #include "attn_common.cuh"
 
 namespace mmfs {
 
-constexpr int kBM = 128, kBN = 64;  // 64-key tiles: 99 KB of shared memory (hd 128) and 256 TMEM columns per CTA -> 2 CTAs / SM
-constexpr int kAttnThreads = 192;   // warp 0: TMA, warp 1: MMA + TMEM alloc, warps 2-5: softmax / epilogue
-constexpr uint32_t kTmemCols = 256; // S0 (64) | S1 (64) | O (<= 128)
+constexpr int kBM = 128, kBN = 64;
+constexpr int kAttnThreads = 288;   // warpgroups 0, 1: softmax + MMA; warp 8: TMA producer
+constexpr int kConsumers = 256;
 
 // Shared memory (dynamic, 1024-byte aligned):
-//   Q [HD/64 boxes][128 rows][128 B] | K [2 stages][HD/64][64][128 B] | V [2][HD/64][64][128 B] |
-//   barriers | tmem base | key-mask bytes [2][64]
+//   Q [HD/64 boxes][128 rows][128 B] | K [2 stages][HD/64][64][128 B] | V [2][HD/64][64][128 B] | barriers | items [2]
+template <int HD> constexpr int attn_ctas_per_sm() { return HD == 64 ? 2 : 1; }
+
 template <typename T, int HD>
-__global__ void __launch_bounds__(kAttnThreads, 2)
+__global__ void __launch_bounds__(kAttnThreads, attn_ctas_per_sm<HD>())
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                const __grid_constant__ CUtensorMap map_v, const AttnParams p) {
-    constexpr int NBOX = HD / 64;
-    constexpr uint32_t QBOX_BYTES = kBM * 128;           // 128 rows x 128 B
-    constexpr uint32_t KBOX_BYTES = kBN * 128;           // 64 rows x 128 B
-    constexpr uint32_t Q_BYTES = NBOX * QBOX_BYTES;
-    constexpr uint32_t KV_BYTES = NBOX * KBOX_BYTES;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // SWIZZLE_128B tiles need 1024-byte alignment; the dynamic window starts at offset 0 of the CTA's shared
-    // memory (no static __shared__ in this kernel), which the __align__ above requests.  No slack is added on
-    // purpose: 2 CTAs must fit in 227 KB.
-    if ((s_addr(smem_raw) & 1023u) != 0u) { asm volatile("trap;"); }
-    uint8_t *sQ = smem_raw;
-    uint8_t *sK = sQ + Q_BYTES;
-    uint8_t *sV = sK + 2 * KV_BYTES;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sV + 2 * KV_BYTES);
-    uint64_t *q_full = bars + 0, *k_full = bars + 1 /*[2]*/, *v_full = bars + 3 /*[2]*/, *k_empty = bars + 5 /*[2]*/,
-             *v_empty = bars + 7 /*[2]*/, *s_full = bars + 9 /*[2]*/, *p_full = bars + 11, *o_ready = bars + 12;
-    uint32_t *tmem_base_smem = reinterpret_cast<uint32_t *>(bars + 13);
-    float *s_kadd = reinterpret_cast<float *>(bars + 14);        // [2][64]: 0 for a visible key, -inf for a padded one
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // grid = (heads, query tiles, batch), x fastest.  Causal: the CTA scheduler hands blocks out in linear order, so within
-    // one batch entry every head's LONGEST query tile (most visible keys) is issued first and the shortest last —
-    // longest-processing-time-first over the whole batch entry instead of per head (a list-scheduling model of the
-    // cfg-3 grid on 296 slots: 1.13x the ideal makespan per head, 1.01x per batch entry), while the K/V working set of
-    // the resident CTAs stays one batch entry's heads (40 MB at cfg 3, inside L2)
-    const int h = blockIdx.x, b = blockIdx.z;
-    const int m_tile = p.causal ? (int)(gridDim.y - 1 - blockIdx.y) : (int)blockIdx.y;
-    const int q0 = m_tile * kBM;
-    // keys this query tile can see: causal -> j <= past + q; never beyond Tkv
-    int kv_end = p.Tkv;
-    if (p.causal) kv_end = min(p.Tkv, p.past + min(q0 + kBM, p.Tq));
-    const int n_tiles = (kv_end + kBN - 1) / kBN;
-
-    if (threadIdx.x == 0) {
-        bar_init(q_full, 1);
-        for (int i = 0; i < 2; ++i) { bar_init(k_full + i, 1); bar_init(v_full + i, 1); bar_init(k_empty + i, 1); bar_init(v_empty + i, 1); bar_init(s_full + i, 1); }
-        bar_init(p_full, 128);
-        bar_init(o_ready, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {   // TMEM allocation is a warp-wide operation; the same warp frees it at the end
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_addr(tmem_base_smem)), "r"(kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_smem;
-    const uint32_t tmem_s0 = tmem_base, tmem_o = tmem_base + 2 * kBN;
-
-    if (warp == 0) {
-        // ============================== TMA producer ==============================
-        if (lane == 0) {
-            bar_expect_tx(q_full, Q_BYTES);
-#pragma unroll
-            for (int bx = 0; bx < NBOX; ++bx) tma_load_4d(sQ + bx * QBOX_BYTES, &map_q, q_full, bx * 64, h, q0, b);
-            for (int j = 0; j < n_tiles; ++j) {
-                const int s = j & 1;
-                const uint32_t ph = (j >> 1) & 1;
-                bar_wait(k_empty + s, ph ^ 1);
-                bar_expect_tx(k_full + s, KV_BYTES);
-#pragma unroll
-                for (int bx = 0; bx < NBOX; ++bx)
-                    tma_load_4d(sK + s * KV_BYTES + bx * KBOX_BYTES, &map_k, k_full + s, bx * 64, h, j * kBN, b);
-                bar_wait(v_empty + s, ph ^ 1);
-                bar_expect_tx(v_full + s, KV_BYTES);
-#pragma unroll
-                for (int bx = 0; bx < NBOX; ++bx)
-                    tma_load_4d(sV + s * KV_BYTES + bx * KBOX_BYTES, &map_v, v_full + s, bx * 64, h, j * kBN, b);
-            }
-        }
-    } else if (warp == 1) {
-        // ============================== MMA issuer (one thread) ==============================
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = instr_desc(AttnFmt<T>::code, 0, kBM, kBN);   // S = Q K^T : both K-major
-            constexpr uint32_t idesc_o = instr_desc(AttnFmt<T>::code, 1, kBM, HD);    // O = P V   : V is MN-major
-            auto issue_s = [&](int j) {
-                const int s = j & 1;
-                bar_wait(k_full + s, (j >> 1) & 1);
-                tc_fence_after();
-#pragma unroll
-                for (int kk = 0; kk < HD / 16; ++kk) {
-#ifdef MMFS_ATTN_TIMING_EXPERIMENTS
-                    if (p.debug & 2) break;
-#endif
-                    // 64-element box along hd, then 32 B inside the 128-byte swizzle atom
-                    umma_f16(tmem_s0 + (uint32_t)s * kBN,
-                             smem_desc(s_addr(sQ) + (kk >> 2) * QBOX_BYTES + (kk & 3) * 32, 16, 1024),
-                             smem_desc(s_addr(sK) + s * KV_BYTES + (kk >> 2) * KBOX_BYTES + (kk & 3) * 32, 16, 1024),
-                             idesc_s, kk > 0);
-                }
-                umma_commit(s_full + s);    // S_j complete -> softmax may read it
-                umma_commit(k_empty + s);   // ... and K stage s may be refilled
-            };
-            bar_wait(q_full, 0);
-            if (n_tiles > 0) issue_s(0);
-            for (int j = 0; j < n_tiles; ++j) {
-                if (j + 1 < n_tiles) issue_s(j + 1);     // overlaps with the softmax of tile j
-                const int s = j & 1;
-                bar_wait(p_full, j & 1);                 // P_j in smem, O rescaled if needed
-                bar_wait(v_full + s, (j >> 1) & 1);
-                tc_fence_after();
-#pragma unroll
-                for (int kk = 0; kk < kBN / 16; ++kk) {
-#ifdef MMFS_ATTN_TIMING_EXPERIMENTS
-                    if (p.debug & 2) break;
-#endif
-                    // P: K-major, K = keys (one 64-key box).  V: MN-major, 16 key rows of 128 B per k-step,
-                    // hd halves KBOX_BYTES apart (LBO)
-                    // P_j sits in the first 32 columns of S buffer s (TMEM A operand): 16 keys = 8 columns per k-step
-                    umma_f16_ts(tmem_o, tmem_s0 + (uint32_t)s * kBN + kk * 8,
-                                smem_desc(s_addr(sV) + s * KV_BYTES + kk * 16 * 128, KBOX_BYTES, 1024), idesc_o, (j > 0) || (kk > 0));
-                }
-                umma_commit(o_ready);
-                umma_commit(v_empty + s);
-            }
-        }
-    } else {
-        // ============================== softmax / correction / epilogue ==============================
-        const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
-        const int row = quarter * 32 + lane;          // query row within the tile == TMEM lane
-        const int tid = threadIdx.x - 64;             // 0..127 (for cooperative loads)
-        const int q_abs = q0 + row;
-        const uint32_t lane_sel = (uint32_t)(quarter * 32) << 16;
-        // m_ref: the maximum the exponentials are taken against.  It follows the true running maximum
-        // lazily -- only when that grew by more than 2^kRescaleThreshold -- which is exact (O and l are
-        // rescaled consistently, p <= 2^8 fits bf16/f16) and saves most TMEM round trips on O.
-        float m_ref = -INFINITY, l_run = 0.f;
-        const int causal_limit = p.causal ? (p.past + q_abs) : 0x7fffffff;   // last visible key index
-        const int warp_causal_limit = p.causal ? (p.past + q0 + quarter * 32) : 0x7fffffff;   // ... of the warp's first row
-
-        for (int j = 0; j < n_tiles; ++j) {
-            const int s = j & 1;
-            const int k0 = j * kBN;
-            if (p.key_mask != nullptr) {              // stage the mask bytes of this tile (double-buffered by s)
-                if (tid < kBN) {
-                    const int kj = k0 + tid;
-                    s_kadd[s * kBN + tid] = (kj < p.Tkv && p.key_mask[(long)b * p.Tkv + kj]) ? 0.f : -INFINITY;
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-            }
-            bar_wait(s_full + s, (j >> 1) & 1);
-            tc_fence_after();
-#ifdef MMFS_ATTN_TIMING_EXPERIMENTS   // never in the shipped library: results are garbage
-            if (p.debug & 1) {      // keep lock-step with the MMA warp (p_full must not run two phases ahead)
-                if (j > 0) bar_wait(o_ready, (j - 1) & 1);
-                tc_fence_before(); bar_arrive(p_full); continue;
-            }
-#endif
-            // warp-uniform on purpose (lane 0 of the warp has the tightest causal limit): a per-lane condition makes
-            // the compiler predicate the whole mask code into the hot loop (2.5x the instructions of an unmasked tile)
-            const bool need_mask = (k0 + kBN - 1 > warp_causal_limit) || (k0 + kBN > p.Tkv) || (p.key_mask != nullptr);
-
-            float sc[kBN];
-            tmem_ld64(tmem_s0 + (uint32_t)s * kBN + lane_sel, sc);
-            if (need_mask) {
-                // Two cheap forms instead of three compares + a shared-memory byte per element (the first version: ~900
-                // instructions for a masked tile against ~230 for a plain one, and every causal query tile ends in two
-                // masked tiles): key padding is ADDED (0 / -inf per key, staged once per tile, broadcast LDS.128 +
-                // packed adds); causality and the ragged tail are one count per row -- columns [0, cnt) are visible.
-                if (p.key_mask != nullptr) {
-                    const float4 *ka = reinterpret_cast<const float4 *>(s_kadd + s * kBN);
-#pragma unroll
-                    for (int i = 0; i < kBN; i += 4) {
-                        const float4 a = ka[i >> 2];
-                        unpack_f32x2(add_f32x2(pack_f32x2(sc[i], sc[i + 1]), pack_f32x2(a.x, a.y)), sc[i], sc[i + 1]);
-                        unpack_f32x2(add_f32x2(pack_f32x2(sc[i + 2], sc[i + 3]), pack_f32x2(a.z, a.w)), sc[i + 2], sc[i + 3]);
-                    }
-                }
-                const int cnt = min(p.Tkv - k0, p.causal ? causal_limit - k0 + 1 : kBN);
-#pragma unroll
-                for (int i = 0; i < kBN; ++i) sc[i] = (i < cnt) ? sc[i] : -INFINITY;
-            }
-            float m_tile = fmaxf(sc[0], sc[1]);
-#pragma unroll
-            for (int i = 2; i < kBN; i += 2) m_tile = fmaxf(m_tile, fmaxf(sc[i], sc[i + 1]));   // FMNMX3
-            const float m_cand = fmaxf(m_ref, m_tile);
-            const bool grow = (m_cand > m_ref) && (m_ref == -INFINITY || (m_cand - m_ref) * p.scale_log2e > kRescaleThreshold);
-            const float alpha = grow ? ((m_ref == -INFINITY) ? 0.f : fast_exp2((m_ref - m_cand) * p.scale_log2e)) : 1.f;
-            if (grow) m_ref = m_cand;
-            const float m_scaled = (m_ref == -INFINITY) ? 0.f : m_ref * p.scale_log2e;
-
-            // P = exp2(S * scale_log2e - m_ref), row sum, pack to 16 bit.  The affine map and the row sum use the
-            // packed fp32 pipe (fma.rn.f32x2 / add.rn.f32x2: one issue slot per two elements); exp2 is MUFU.
-            const uint64_t sc2 = pack_f32x2(p.scale_log2e, p.scale_log2e), neg_m2 = pack_f32x2(-m_scaled, -m_scaled);
-            uint64_t l2a = 0ull, l2b = 0ull;        // two independent packed accumulators (bit pattern of +0.f, +0.f)
-            uint32_t pk[kBN / 2];
-#pragma unroll
-            for (int i = 0; i < kBN; i += 4) {
-                float x0, x1, x2, x3;
-                unpack_f32x2(fma_f32x2(pack_f32x2(sc[i], sc[i + 1]), sc2, neg_m2), x0, x1);   // masked: exp2(-inf) = 0
-                unpack_f32x2(fma_f32x2(pack_f32x2(sc[i + 2], sc[i + 3]), sc2, neg_m2), x2, x3);
-                const float e0 = fast_exp2(x0), e1 = fast_exp2(x1), e2 = fast_exp2(x2), e3 = fast_exp2(x3);
-                l2a = add_f32x2(l2a, pack_f32x2(e0, e1));
-                l2b = add_f32x2(l2b, pack_f32x2(e2, e3));
-                pk[i >> 1] = pack2<T>(e0, e1);
-                pk[(i >> 1) + 1] = pack2<T>(e2, e3);
-            }
-            float la, lb, lc, ld;
-            unpack_f32x2(l2a, la, lb);
-            unpack_f32x2(l2b, lc, ld);
-            const float l_tile = (la + lb) + (lc + ld);
-            l_run = l_run * alpha + l_tile;
-
-            // O is rescaled only after the previous P V retired; otherwise the softmax of tile j does not depend on it
-            // (P_j goes into S_j's own TMEM columns)
-            const bool any_grow = __any_sync(0xffffffffu, grow) && (j > 0);
-            if (any_grow) {
-                bar_wait(o_ready, (j - 1) & 1);
-                tc_fence_after();
-            }
-            if (any_grow) {                           // warp-uniform: tcgen05.ld/st are warp-collective
-#pragma unroll 1
-                for (int c = 0; c < HD; c += 32) {
-                    float o[32];
-                    tmem_ld32(tmem_o + lane_sel + c, o);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) o[i] *= alpha;
-                    tmem_st32(tmem_o + lane_sel + c, o);
-                }
-            }
-            tmem_st32_u32(tmem_s0 + (uint32_t)s * kBN + lane_sel, pk);   // row = lane, keys 2c, 2c+1 in column c
-            // protocol guard: P V(j-1) retired (it was issued a whole softmax earlier) before p_full moves on, so the
-            // MMA thread can never find this barrier two phases ahead of the one it waits for
-            if (j > 0 && !any_grow) bar_wait(o_ready, (j - 1) & 1);
-            tc_fence_before();
-            bar_arrive(p_full);
-        }
-
-        // epilogue: O / l -> global
-        if (n_tiles > 0) {
-            bar_wait(o_ready, (n_tiles - 1) & 1);
-            tc_fence_after();
-        }
-        const float inv = (l_run > 0.f) ? 1.f / l_run : 0.f;   // fully masked row -> zeros
-        // tcgen05.ld is warp-collective (.sync.aligned): every lane executes it, rows past Tq only skip the store
-        T *op = static_cast<T *>(p.out) + (long)b * p.o_bs + (long)q_abs * p.o_ts + (long)h * HD;
-#pragma unroll 1
-        for (int c = 0; c < HD; c += 32) {
-            float o[32];
-            if (n_tiles > 0) {           // CTA-uniform
-                tmem_ld32(tmem_o + lane_sel + c, o);
-            } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) o[i] = 0.f;
-            }
-            if (q_abs < p.Tq) {
-#pragma unroll
-                for (int qd = 0; qd < 4; ++qd) {
-                    uint4 w;
-                    w.x = pack2<T>(o[qd * 8 + 0] * inv, o[qd * 8 + 1] * inv);
-                    w.y = pack2<T>(o[qd * 8 + 2] * inv, o[qd * 8 + 3] * inv);
-                    w.z = pack2<T>(o[qd * 8 + 4] * inv, o[qd * 8 + 5] * inv);
-                    w.w = pack2<T>(o[qd * 8 + 6] * inv, o[qd * 8 + 7] * inv);
-                    *reinterpret_cast<uint4 *>(op + c + qd * 8) = w;
-                }
-            }
-            __syncwarp();
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// Persistent variant.  A sweep over sequence lengths (tools/attn_sweep.py, 2560 CTAs each time) fits the kernel above
-// to  t_CTA = 12 us + 0.9 us x key tiles  of CTA slot time: launch, barrier init, TMEM allocation, the Q / K0 / V0 load
-// round trip, the pipeline fill of the first tile and the O read-out are paid per (query tile, head, batch) item and
-// are NOT hidden by the second resident CTA, because one CTA alone is softmax-latency bound -- at the cfg-3 prefill
-// (17 key tiles per item on average) that is ~40 % of the run.  Here 2 CTAs per SM stay resident and walk a work list:
-//   * items (batch-major, longest query tile first, heads fastest -- the order of the grid above) are handed out by an
-//     atomic counter (list scheduling: 1.01-1.04x the ideal makespan; a static round robin is 1.14-1.19x);
-//   * barriers, TMEM and the tensor maps are set up once; every per-tile barrier runs on a GLOBAL tile counter, so the
-//     K / V ring and the S / P ping-pong continue across items without a drain;
-//   * the producer requests the next item's Q (after `q_empty`: the last S MMA of the current item retired), K0, V0
-//     while the current item's last softmax, P V and O read-out run; the MMA thread issues the next item's first S
-//     MMA under the O read-out and waits for `o_free` only before it overwrites O.
-template <typename T, int HD>
-__global__ void __launch_bounds__(kAttnThreads, 2)
-attn_fwd_persistent_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                           const __grid_constant__ CUtensorMap map_v, const AttnParams p, unsigned *__restrict__ sched, int n_work) {
+                const __grid_constant__ CUtensorMap map_v, const AttnParams p, unsigned *__restrict__ sched, int n_work) {
     constexpr int NBOX = HD / 64;
     constexpr uint32_t QBOX_BYTES = kBM * 128, KBOX_BYTES = kBN * 128;
     constexpr uint32_t Q_BYTES = NBOX * QBOX_BYTES, KV_BYTES = NBOX * KBOX_BYTES;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
+    // SWIZZLE_128B tiles need 1024-byte alignment; the dynamic window starts at offset 0 of the CTA's shared memory
+    // (no static __shared__ in this kernel), which the __align__ above requests.
     if ((s_addr(smem_raw) & 1023u) != 0u) { asm volatile("trap;"); }
     uint8_t *sQ = smem_raw;
     uint8_t *sK = sQ + Q_BYTES;
     uint8_t *sV = sK + 2 * KV_BYTES;
     uint64_t *bars = reinterpret_cast<uint64_t *>(sV + 2 * KV_BYTES);
-    uint64_t *q_full = bars + 0, *k_full = bars + 1 /*[2]*/, *v_full = bars + 3 /*[2]*/, *k_empty = bars + 5 /*[2]*/,
-             *v_empty = bars + 7 /*[2]*/, *s_full = bars + 9 /*[2]*/, *p_full = bars + 11, *o_ready = bars + 12,
-             *q_empty = bars + 13, *o_free = bars + 14, *item_full = bars + 15 /*[2]*/, *item_empty = bars + 17 /*[2]*/;
-    uint32_t *tmem_base_smem = reinterpret_cast<uint32_t *>(bars + 19);
-    int *s_item = reinterpret_cast<int *>(bars + 19) + 2;         // [2]
-    float *s_kadd = reinterpret_cast<float *>(bars + 22);        // [2][64], 16-byte aligned
+    uint64_t *q_full = bars + 0, *q_empty = bars + 1, *k_full = bars + 2 /*[2]*/, *k_empty = bars + 4 /*[2]*/,
+             *v_full = bars + 6 /*[2]*/, *v_empty = bars + 8 /*[2]*/, *item_full = bars + 10 /*[2]*/, *item_empty = bars + 12 /*[2]*/;
+    int *s_item = reinterpret_cast<int *>(bars + 14);            // [2]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_q = (p.Tq + kBM - 1) / kBM;
     // item w -> (batch, query tile, head): batch-major, longest tile first inside a batch entry, heads fastest
-    auto decode = [&](int w, int &m_tile, int &h, int &b, int &q0, int &n_tiles) {
+    auto decode = [&](int w, int &h, int &b, int &q0, int &n_tiles) {
         b = w / (n_q * p.H);
         const int r = w - b * (n_q * p.H);
         const int mi = r / p.H;
         h = r - mi * p.H;
-        m_tile = p.causal ? n_q - 1 - mi : mi;
-        q0 = m_tile * kBM;
+        q0 = (p.causal ? n_q - 1 - mi : mi) * kBM;
         int kv_end = p.Tkv;
         if (p.causal) kv_end = min(p.Tkv, p.past + min(q0 + kBM, p.Tq));
         n_tiles = (kv_end + kBN - 1) / kBN;
@@ -359,30 +68,19 @@ attn_fwd_persistent_kernel(const __grid_constant__ CUtensorMap map_q, const __gr
 
     if (threadIdx.x == 0) {
         bar_init(q_full, 1);
+        bar_init(q_empty, kConsumers);
         for (int i = 0; i < 2; ++i) {
-            bar_init(k_full + i, 1); bar_init(v_full + i, 1); bar_init(k_empty + i, 1); bar_init(v_empty + i, 1); bar_init(s_full + i, 1);
-            bar_init(item_full + i, 1); bar_init(item_empty + i, 129);          // MMA thread + 128 softmax threads
+            bar_init(k_full + i, 1); bar_init(v_full + i, 1); bar_init(k_empty + i, kConsumers); bar_init(v_empty + i, kConsumers);
+            bar_init(item_full + i, 1); bar_init(item_empty + i, kConsumers);
         }
-        bar_init(p_full, 128);
-        bar_init(o_ready, 1);
-        bar_init(q_empty, 1);
-        bar_init(o_free, 128);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_addr(tmem_base_smem)), "r"(kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_smem;
-    const uint32_t tmem_s0 = tmem_base, tmem_o = tmem_base + 2 * kBN;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ============================== scheduler + TMA producer ==============================
         if (lane == 0) {
-            int w = blockIdx.x;                                      // the first item is static (grid <= n_work)
+            int w = blockIdx.x;
             int g = 0;                                               // global tile counter
             for (int qn = 0;; ++qn) {
                 const int slot = qn & 1;
@@ -390,9 +88,10 @@ attn_fwd_persistent_kernel(const __grid_constant__ CUtensorMap map_q, const __gr
                 s_item[slot] = w < n_work ? w : -1;
                 bar_arrive(item_full + slot);
                 if (w >= n_work) break;
-                const int w_next = (int)gridDim.x + (int)atomicAdd(sched, 1u);   // fetched early: the latency hides under this item
-                int m_tile, h, b, q0, n_tiles;
-                decode(w, m_tile, h, b, q0, n_tiles);
+                // non-persistent launch: one item per CTA.  Persistent: fetched early, the latency hides under this item
+                const int w_next = sched ? (int)gridDim.x + (int)atomicAdd(sched, 1u) : n_work;
+                int h, b, q0, n_tiles;
+                decode(w, h, b, q0, n_tiles);
                 if (qn > 0) bar_wait(q_empty, (qn - 1) & 1);        // the previous item's S MMAs no longer read Q
                 bar_expect_tx(q_full, Q_BYTES);
 #pragma unroll
@@ -414,197 +113,135 @@ attn_fwd_persistent_kernel(const __grid_constant__ CUtensorMap map_q, const __gr
                 w = w_next;
             }
         }
-    } else if (warp == 1) {
-        // ============================== MMA issuer (one thread) ==============================
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = instr_desc(AttnFmt<T>::code, 0, kBM, kBN);
-            constexpr uint32_t idesc_o = instr_desc(AttnFmt<T>::code, 1, kBM, HD);
-            auto issue_s = [&](int g) {
-                const int s = g & 1;
-                bar_wait(k_full + s, (g >> 1) & 1);
-                tc_fence_after();
-#pragma unroll
-                for (int kk = 0; kk < HD / 16; ++kk)
-                    umma_f16(tmem_s0 + (uint32_t)s * kBN,
-                             smem_desc(s_addr(sQ) + (kk >> 2) * QBOX_BYTES + (kk & 3) * 32, 16, 1024),
-                             smem_desc(s_addr(sK) + s * KV_BYTES + (kk >> 2) * KBOX_BYTES + (kk & 3) * 32, 16, 1024),
-                             idesc_s, kk > 0);
-                umma_commit(s_full + s);
-                umma_commit(k_empty + s);
-            };
-            int g = 0;
-            for (int qn = 0;; ++qn) {
-                const int slot = qn & 1;
-                bar_wait(item_full + slot, (qn >> 1) & 1);
-                const int w = s_item[slot];
-                bar_arrive(item_empty + slot);
-                if (w < 0) break;
-                int m_tile, h, b, q0, n_tiles;
-                decode(w, m_tile, h, b, q0, n_tiles);
-                bar_wait(q_full, qn & 1);
-                if (n_tiles > 0) issue_s(g);
-                if (n_tiles <= 1) umma_commit(q_empty);             // Q is free once the item's last S MMA retires
-                for (int j = 0; j < n_tiles; ++j, ++g) {
-                    if (j + 1 < n_tiles) {
-                        issue_s(g + 1);                              // overlaps with the softmax of tile j
-                        if (j + 2 == n_tiles) umma_commit(q_empty);
-                    }
-                    const int s = g & 1;
-                    bar_wait(p_full, g & 1);
-                    bar_wait(v_full + s, (g >> 1) & 1);
-                    if (j == 0 && qn > 0) bar_wait(o_free, (qn - 1) & 1);   // the previous item's O has been read out
-                    tc_fence_after();
-#pragma unroll
-                    for (int kk = 0; kk < kBN / 16; ++kk)
-                        umma_f16_ts(tmem_o, tmem_s0 + (uint32_t)s * kBN + kk * 8,
-                                    smem_desc(s_addr(sV) + s * KV_BYTES + kk * 16 * 128, KBOX_BYTES, 1024), idesc_o, (j > 0) || (kk > 0));
-                    umma_commit(o_ready);
-                    umma_commit(v_empty + s);
-                }
-            }
-        }
-    } else {
-        // ============================== softmax / correction / epilogue ==============================
-        const int quarter = warp & 3;
-        const int row = quarter * 32 + lane;
-        const int tid = threadIdx.x - 64;
-        const uint32_t lane_sel = (uint32_t)(quarter * 32) << 16;
-        int g = 0;
-        for (int qn = 0;; ++qn) {
-            const int slot = qn & 1;
-            bar_wait(item_full + slot, (qn >> 1) & 1);
-            const int w = s_item[slot];
-            bar_arrive(item_empty + slot);
-            if (w < 0) break;
-            int m_tile, h, b, q0, n_tiles;
-            decode(w, m_tile, h, b, q0, n_tiles);
-            const int q_abs = q0 + row;
-            float m_ref = -INFINITY, l_run = 0.f;
-            const int causal_limit = p.causal ? (p.past + q_abs) : 0x7fffffff;
-            const int warp_causal_limit = p.causal ? (p.past + q0 + quarter * 32) : 0x7fffffff;
-
-            for (int j = 0; j < n_tiles; ++j, ++g) {
-                const int s = g & 1;
-                const int k0 = j * kBN;
-                if (p.key_mask != nullptr) {
-                    if (tid < kBN) {
-                        const int kj = k0 + tid;
-                        s_kadd[s * kBN + tid] = (kj < p.Tkv && p.key_mask[(long)b * p.Tkv + kj]) ? 0.f : -INFINITY;
-                    }
-                    asm volatile("bar.sync 1, 128;" ::: "memory");
-                }
-                bar_wait(s_full + s, (g >> 1) & 1);
-                tc_fence_after();
-                const bool need_mask = (k0 + kBN - 1 > warp_causal_limit) || (k0 + kBN > p.Tkv) || (p.key_mask != nullptr);
-                float sc[kBN];
-                tmem_ld64(tmem_s0 + (uint32_t)s * kBN + lane_sel, sc);
-                if (need_mask) {
-                    if (p.key_mask != nullptr) {
-                        const float4 *ka = reinterpret_cast<const float4 *>(s_kadd + s * kBN);
-#pragma unroll
-                        for (int i = 0; i < kBN; i += 4) {
-                            const float4 a = ka[i >> 2];
-                            unpack_f32x2(add_f32x2(pack_f32x2(sc[i], sc[i + 1]), pack_f32x2(a.x, a.y)), sc[i], sc[i + 1]);
-                            unpack_f32x2(add_f32x2(pack_f32x2(sc[i + 2], sc[i + 3]), pack_f32x2(a.z, a.w)), sc[i + 2], sc[i + 3]);
-                        }
-                    }
-                    const int cnt = min(p.Tkv - k0, p.causal ? causal_limit - k0 + 1 : kBN);
-#pragma unroll
-                    for (int i = 0; i < kBN; ++i) sc[i] = (i < cnt) ? sc[i] : -INFINITY;
-                }
-                float m_tile_max = fmaxf(sc[0], sc[1]);
-#pragma unroll
-                for (int i = 2; i < kBN; i += 2) m_tile_max = fmaxf(m_tile_max, fmaxf(sc[i], sc[i + 1]));
-                const float m_cand = fmaxf(m_ref, m_tile_max);
-                const bool grow = (m_cand > m_ref) && (m_ref == -INFINITY || (m_cand - m_ref) * p.scale_log2e > kRescaleThreshold);
-                const float alpha = grow ? ((m_ref == -INFINITY) ? 0.f : fast_exp2((m_ref - m_cand) * p.scale_log2e)) : 1.f;
-                if (grow) m_ref = m_cand;
-                const float m_scaled = (m_ref == -INFINITY) ? 0.f : m_ref * p.scale_log2e;
-                const uint64_t sc2 = pack_f32x2(p.scale_log2e, p.scale_log2e), neg_m2 = pack_f32x2(-m_scaled, -m_scaled);
-                uint64_t l2a = 0ull, l2b = 0ull;
-                uint32_t pk[kBN / 2];
-#pragma unroll
-                for (int i = 0; i < kBN; i += 4) {
-                    float x0, x1, x2, x3;
-                    unpack_f32x2(fma_f32x2(pack_f32x2(sc[i], sc[i + 1]), sc2, neg_m2), x0, x1);
-                    unpack_f32x2(fma_f32x2(pack_f32x2(sc[i + 2], sc[i + 3]), sc2, neg_m2), x2, x3);
-                    const float e0 = fast_exp2(x0), e1 = fast_exp2(x1), e2 = fast_exp2(x2), e3 = fast_exp2(x3);
-                    l2a = add_f32x2(l2a, pack_f32x2(e0, e1));
-                    l2b = add_f32x2(l2b, pack_f32x2(e2, e3));
-                    pk[i >> 1] = pack2<T>(e0, e1);
-                    pk[(i >> 1) + 1] = pack2<T>(e2, e3);
-                }
-                float la, lb, lc, ld;
-                unpack_f32x2(l2a, la, lb);
-                unpack_f32x2(l2b, lc, ld);
-                l_run = l_run * alpha + ((la + lb) + (lc + ld));
-
-                const bool any_grow = __any_sync(0xffffffffu, grow) && (j > 0);
-                if (any_grow) {
-                    bar_wait(o_ready, (g - 1) & 1);
-                    tc_fence_after();
-#pragma unroll 1
-                    for (int c = 0; c < HD; c += 32) {
-                        float o[32];
-                        tmem_ld32(tmem_o + lane_sel + c, o);
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) o[i] *= alpha;
-                        tmem_st32(tmem_o + lane_sel + c, o);
-                    }
-                }
-                tmem_st32_u32(tmem_s0 + (uint32_t)s * kBN + lane_sel, pk);
-                if (j > 0 && !any_grow) bar_wait(o_ready, (g - 1) & 1);   // protocol guard (see the kernel above)
-                tc_fence_before();
-                bar_arrive(p_full);
-            }
-
-            // epilogue: O / l -> global; O is released to the next item as soon as its last columns are in registers
-            if (n_tiles > 0) {
-                bar_wait(o_ready, (g - 1) & 1);
-                tc_fence_after();
-            }
-            const float inv = (l_run > 0.f) ? 1.f / l_run : 0.f;
-            T *op = static_cast<T *>(p.out) + (long)b * p.o_bs + (long)q_abs * p.o_ts + (long)h * HD;
-#pragma unroll 1
-            for (int c = 0; c < HD; c += 32) {
-                float o[32];
-                if (n_tiles > 0) {
-                    tmem_ld32(tmem_o + lane_sel + c, o);
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) o[i] = 0.f;
-                }
-                if (c + 32 == HD) {
-                    tc_fence_before();
-                    bar_arrive(o_free);
-                }
-                if (q_abs < p.Tq) {
-#pragma unroll
-                    for (int qd = 0; qd < 4; ++qd) {
-                        uint4 wv;
-                        wv.x = pack2<T>(o[qd * 8 + 0] * inv, o[qd * 8 + 1] * inv);
-                        wv.y = pack2<T>(o[qd * 8 + 2] * inv, o[qd * 8 + 3] * inv);
-                        wv.z = pack2<T>(o[qd * 8 + 4] * inv, o[qd * 8 + 5] * inv);
-                        wv.w = pack2<T>(o[qd * 8 + 6] * inv, o[qd * 8 + 7] * inv);
-                        *reinterpret_cast<uint4 *>(op + c + qd * 8) = wv;
-                    }
-                }
-                __syncwarp();
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
+    // ============================== consumer warpgroups: S, softmax, O ==============================
+    const int wg = warp >> 2;                        // 64-row half of the query tile
+    const int quad = lane >> 2, tq = lane & 3;
+    const int row_in_tile = wg * 64 + (warp & 3) * 16 + quad;   // + 8 for the second row of the fragment
+    const uint32_t q_base = s_addr(sQ) + wg * 64 * 128;
+    int g = 0;
+    for (int qn = 0;; ++qn) {
+        const int slot = qn & 1;
+        bar_wait(item_full + slot, (qn >> 1) & 1);
+        const int w = s_item[slot];
+        bar_arrive(item_empty + slot);
+        if (w < 0) break;
+        int h, b, q0, n_tiles;
+        decode(w, h, b, q0, n_tiles);
+        const int r0 = q0 + row_in_tile;             // rows r0 and r0 + 8
+        float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l: this thread's columns only
+        float o[HD / 2];
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+        bar_wait(q_full, qn & 1);
+        if (n_tiles == 0) bar_arrive(q_empty);
+
+        for (int j = 0; j < n_tiles; ++j, ++g) {
+            const int s = g & 1;
+            const int k0 = j * kBN;
+            float sc[kBN / 2];
+            bar_wait(k_full + s, (g >> 1) & 1);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < HD / 16; ++kk)     // 64-element box along hd, then 32 B inside the 128-byte swizzle atom
+                Wgmma<T>::ss_n64(sc, smem_desc(q_base + (kk >> 2) * QBOX_BYTES + (kk & 3) * 32, 16, 1024),
+                                 smem_desc(s_addr(sK) + s * KV_BYTES + (kk >> 2) * KBOX_BYTES + (kk & 3) * 32, 16, 1024), kk > 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(sc);
+            bar_arrive(k_empty + s);
+            if (j + 1 == n_tiles) bar_arrive(q_empty);
+
+            // masks: key padding, ragged tail, causality (key index <= past + query index)
+            const bool need_mask = (k0 + kBN > p.Tkv) || (p.key_mask != nullptr) ||
+                                   (p.causal && k0 + kBN - 1 > p.past + q0 + wg * 64);
+            if (need_mask) {
+#pragma unroll
+                for (int jj = 0; jj < kBN / 8; ++jj)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int key = k0 + jj * 8 + 2 * tq + c;
+                        bool vis = key < p.Tkv;
+                        if (vis && p.key_mask != nullptr) vis = p.key_mask[(long)b * p.Tkv + key] != 0;
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            const bool ok = vis && (!p.causal || key <= p.past + r0 + 8 * i);
+                            if (!ok) sc[jj * 4 + 2 * i + c] = -INFINITY;
+                        }
+                    }
+            }
+            float alpha[2], neg_m[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int jj = 0; jj < kBN / 8; ++jj) mx = fmaxf(mx, fmaxf(sc[jj * 4 + 2 * i], sc[jj * 4 + 2 * i + 1]));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                const float m_new = fmaxf(m_run[i], mx);
+                alpha[i] = (m_new == -INFINITY) ? 1.f : fast_exp2((m_run[i] - m_new) * p.scale_log2e);   // exp2(-inf) = 0
+                m_run[i] = m_new;
+                neg_m[i] = (m_new == -INFINITY) ? 0.f : -m_new * p.scale_log2e;
+            }
+            // P = exp2(S * scale_log2e - m), packed to 16 bit as the A fragments of the four k16 steps of P V
+            uint32_t pa[kBN / 16][4];
+            float ls[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jj = 0; jj < kBN / 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const float e0 = fast_exp2(fmaf(sc[jj * 4 + 2 * i], p.scale_log2e, neg_m[i]));   // masked: exp2(-inf) = 0
+                    const float e1 = fast_exp2(fmaf(sc[jj * 4 + 2 * i + 1], p.scale_log2e, neg_m[i]));
+                    ls[i] += e0 + e1;
+                    pa[jj >> 1][(jj & 1) * 2 + i] = pack2<T>(e0, e1);
+                }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) l_run[i] = l_run[i] * alpha[i] + ls[i];
+#pragma unroll
+            for (int jj = 0; jj < HD / 8; ++jj) {
+                o[jj * 4 + 0] *= alpha[0]; o[jj * 4 + 1] *= alpha[0];
+                o[jj * 4 + 2] *= alpha[1]; o[jj * 4 + 3] *= alpha[1];
+            }
+
+            bar_wait(v_full + s, (g >> 1) & 1);
+            reg_fence(o);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < kBN / 16; ++kk) {  // V: MN-major, 16 key rows of 128 B per k-step, hd boxes KBOX_BYTES apart
+                const uint64_t dv = smem_desc(s_addr(sV) + s * KV_BYTES + kk * 16 * 128, KBOX_BYTES, 1024);
+                if constexpr (HD == 64) Wgmma<T>::rs_n64(o, pa[kk], dv, 1);
+                else Wgmma<T>::rs_n128(o, pa[kk], dv, 1);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(o);
+            bar_arrive(v_empty + s);
+        }
+
+        // epilogue: O / l -> global
+        T *out = static_cast<T *>(p.out) + (long)b * p.o_bs + (long)h * HD;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            float l = l_run[i];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = (l > 0.f) ? 1.f / l : 0.f;     // fully masked row -> zeros
+            const int q = r0 + 8 * i;
+            if (q < p.Tq) {
+                T *op = out + (long)q * p.o_ts + 2 * tq;
+#pragma unroll
+                for (int jj = 0; jj < HD / 8; ++jj)
+                    *reinterpret_cast<uint32_t *>(op + jj * 8) = pack2<T>(o[jj * 4 + 2 * i] * inv, o[jj * 4 + 2 * i + 1] * inv);
+            }
+        }
     }
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
 // (B, T, H, hd) tensor with element strides bs / ts (heads dense): dims innermost-first {hd, H, T, B}
-// Encoding a tensor map costs a driver call (~1-2 us on the host, three per launch); the decoder calls this op
+// Encoding a tensor map costs a driver call on the host (three per launch); the decoder calls this op
 // with the same few (pointer, shape, strides) combinations layer after layer, so the last encodings are kept per
 // host thread.  A map depends only on its arguments (it holds no device state), so a hit is always valid.
 struct MapKey {
@@ -654,27 +291,19 @@ static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUten
     const int dev = current_device();
     const int n_q = (p.Tq + kBM - 1) / kBM;
     const long n_work = (long)n_q * p.H * p.B;
-    if (sched != nullptr && n_work > 2L * num_sms() && n_work < (1L << 30)) {     // more items than resident CTAs: persistent
-        constexpr size_t smem = (size_t)(HD / 64) * (kBM * 128 + 4 * kBN * 128) + 22 * 8 + 2 * kBN * sizeof(float) + 16;
-        auto kern = attn_fwd_persistent_kernel<T, HD>;
-        static bool attr_set[kMaxDevices] = {};
-        if (dev < 0 || dev >= kMaxDevices || !attr_set[dev]) {
-            MMFS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            if (dev >= 0 && dev < kMaxDevices) attr_set[dev] = true;
-        }
-        kern<<<2 * num_sms(), kAttnThreads, smem, st>>>(mq, mk, mv, p, sched, (int)n_work);
-        MMFS_CUDA(cudaGetLastError());
-        return MMFS_OK;
-    }
-    constexpr size_t smem = (size_t)(HD / 64) * (kBM * 128 + 4 * kBN * 128) + 14 * 8 + 2 * kBN * sizeof(float) + 16;
+    if (n_work >= (1L << 30)) { set_error("attn_forward: %ld work items", n_work); return MMFS_EUNSUPPORTED; }
+    constexpr size_t smem = (size_t)(HD / 64) * (kBM * 128 + 4 * kBN * 128) + 14 * 8 + 2 * sizeof(int);
     auto kern = attn_fwd_kernel<T, HD>;
     static bool attr_set[kMaxDevices] = {};          // the attribute is per device
     if (dev < 0 || dev >= kMaxDevices || !attr_set[dev]) {
         MMFS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         if (dev >= 0 && dev < kMaxDevices) attr_set[dev] = true;
     }
-    dim3 grid(p.H, n_q, p.B);
-    kern<<<grid, kAttnThreads, smem, st>>>(mq, mk, mv, p);
+    // more items than resident CTAs: persistent, otherwise one item per CTA
+    const int resident = attn_ctas_per_sm<HD>() * num_sms();
+    const bool persistent = sched != nullptr && n_work > resident;
+    const int grid = persistent ? resident : (int)n_work;
+    kern<<<grid, kAttnThreads, smem, st>>>(mq, mk, mv, p, persistent ? sched : nullptr, (int)n_work);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -707,11 +336,6 @@ static int attn_forward_impl(const void *q, const void *k, const void *v, void *
     AttnParams p;
     p.out = out; p.key_mask = key_mask; p.B = B; p.H = H; p.Tq = Tq; p.Tkv = Tkv; p.causal = causal; p.past = past;
     p.o_bs = o_bs; p.o_ts = o_ts; p.scale_log2e = scale * 1.4426950408889634f;
-    p.debug = 0;
-#ifdef MMFS_ATTN_TIMING_EXPERIMENTS
-    static const int debug = getenv("MMFS_ATTN_DEBUG") ? atoi(getenv("MMFS_ATTN_DEBUG")) : 0;
-    p.debug = debug;
-#endif
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == MMFS_BF16)
         return hd == 64 ? launch_attn<__nv_bfloat16, 64>(mq, mk, mv, p, sched, st) : launch_attn<__nv_bfloat16, 128>(mq, mk, mv, p, sched, st);

@@ -15,7 +15,7 @@
 // lane whole keys (row-contiguous 16-byte loads, q broadcast from shared memory), phase 2 gives
 // every lane channels (coalesced V rows), online softmax across chunks.
 #include "common.cuh"
-#include "sampler_common.cuh"   // MixFma (FHFMA)
+#include "sampler_common.cuh"   // MixFma (mixed-precision FMA)
 
 namespace mmfs {
 
@@ -103,8 +103,7 @@ attn_generic_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *_
 
 // ------------------------------------------------------------------------------------------------------------
 // Decode (q_len = 1 over a KV cache): split-KV ("flash decoding").  The row-per-warp kernel above gives a decode step
-// B*H = 160 warps for the whole GPU, each walking 2k keys serially with scalar loads (3.4 ms per layer at the cfg-3
-// cache).  Here grid = (ceil(Tkv / 256), H, B): every CTA reduces 256 keys of one (b, h) -- lane = key for the
+// B*H = 160 warps for the whole GPU, each walking 2k keys serially with scalar loads.  Here grid = (ceil(Tkv / 256), H, B): every CTA reduces 256 keys of one (b, h) -- lane = key for the
 // scores (16-byte loads along the key row, q broadcast from shared memory), lane = channels for P V (coalesced V
 // rows) -- and writes an (m, l, acc[hd]) partial; a second kernel merges the partials.  HBM-bound: K and V are read
 // exactly once.
@@ -222,13 +221,13 @@ attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const
 }
 
 // hd = 128, 16-bit elements (the Llama decode step): every load is a fully used 16-byte vector.
-//   Q K^T : 8 lanes per key (2 x LDG.128 each = the key's 256 bytes), 4 keys per warp step; the products are FHFMA
+//   Q K^T : 8 lanes per key (2 x LDG.128 each = the key's 256 bytes), 4 keys per warp step; the products are mixed-precision FMA
 //           (16-bit k x 16-bit q + fp32 accumulator, exact products, no unpack), the scale is applied to the fp32 dot;
 //   P V   : 16 lanes per key (LDG.128 = 8 channels each), 2 keys per warp step.
 // Loads are issued in explicit BATCHES of eight 16-byte vectors per lane (4 KB per warp), double-buffered in registers,
 // with the key-validity bits balloted once per warp up front: the first version of this kernel tested the mask byte,
 // branched and loaded key by key, which left two loads in flight per warp (SASS: LDG.U8 -> BRA -> 2 x LDG.128 -> SHFL per
-// key; 43 us per layer at the cfg-3 cache = 3.9 TB/s).  A masked key inside the range is still loaded (clamped address)
+// key).  A masked key inside the range is still loaded (clamped address)
 // and discarded.
 // A warp reduces 64 keys in one pass (no running rescale); the CTA's four warps are combined in shared memory into one
 // (m, l, acc[128]) partial, and the LAST CTA of a (b, h) to arrive (a ticket per (b, h) in the scratch buffer, zeroed by
@@ -283,7 +282,7 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
         // Software pipeline over eight batches (K0..K3, V0..V3) with two register buffers: the loads of batch i+1 are
         // issued BEFORE the arithmetic of batch i, and V0 is requested before the softmax reductions (V does not depend
         // on P), so every warp keeps one 4 KB batch in flight from its first instruction to its last.  (Without this
-        // a warp has nothing in flight while it computes: ncu r02, 39.8 us, DRAM 54 %, 67 % long-scoreboard stalls.)
+        // a warp has nothing in flight while it computes.)
         const T *vb = v + b * v_bs + (long)h * HD + ch;
         auto load_k = [&](uint4 (&r)[8], int bt) {
 #pragma unroll
@@ -410,10 +409,9 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
     orow[d] = from_op<T>(den > 0.f ? num / den : 0.f);           // fully masked row -> zeros
 }
 
-// (Tried and dropped, profiles/r02_decode_attn_staged_vs_batched.log: staging a warp's whole 64-key K and V tiles in
-// shared memory with cp.async -- 32 KB per warp requested up front, one memory round trip per CTA, 6 warps per SM --
-// ran at 62 us against 41.8 us: with so few warps the score / softmax / P V arithmetic out of shared memory is
-// latency-exposed (ncu: IPC 0.82, 8.7 % occupancy, DRAM 35 %).)
+// (Alternative not taken: staging a warp's whole 64-key K and V tiles in shared memory with cp.async -- 32 KB per warp
+// requested up front, 6 warps per SM -- leaves so few warps that the score / softmax / P V arithmetic out of shared
+// memory is latency-exposed; tools/decode_attn_ab.py compares the variants.)
 template <typename T>
 __global__ void attn_decode_merge_kernel(const float *__restrict__ part, T *__restrict__ out, int H, int hd, int n_split,
                                          long o_bs) {
@@ -474,7 +472,7 @@ static int launch_attn_generic(const void *q, const void *k, const void *v, void
                                long v_bs, long v_ts, long o_bs, long o_ts, float scale, int causal, int past, cudaStream_t st) {
     const long n_rows = (long)B * H * Tq;
     const long blocks = (n_rows + kAttnWarps - 1) / kAttnWarps;
-    const int grid = (int)(blocks < 148L * 16 ? blocks : 148L * 16);
+    const int grid = (int)(blocks < (long)num_sms() * 16 ? blocks : (long)num_sms() * 16);
     const size_t smem = (size_t)kAttnWarps * (hd + kAttnChunk) * sizeof(float);
     attn_generic_kernel<T><<<grid, 32 * kAttnWarps, smem, st>>>((const T *)q, (const T *)k, (const T *)v, (T *)out, key_mask,
                                                               n_rows, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts,

@@ -35,7 +35,7 @@ int num_sms() {
         if (dev < kMaxDevices) cached[dev] = n;
         return n;
     }
-    return 148;  // B200
+    return 132;  // H100 SXM
 }
 
 // per-thread device scratch for the host-buffer entry points

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libmmfs_b200.so (sm_100a only).
+// common.cuh -- shared helpers for libmmfs_b200.so (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

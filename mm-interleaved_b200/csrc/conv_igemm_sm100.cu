@@ -1,4 +1,4 @@
-// conv_igemm_sm100.cu -- 2-D convolution as an implicit GEMM on the 5th-generation tensor cores (NHWC, bf16 / f16).
+// conv_igemm_sm100.cu -- 2-D convolution as an implicit GEMM on the Hopper tensor cores (wgmma; NHWC, bf16 / f16).
 //
 // The SD-2.1 UNet convolutions of the denoise step (3x3 stride 1 / 2, 1x1 shortcuts; arithmetic in diffusers 0.20,
 // called from utils/monkey_patch/sd_unet_forward_monkey_patch.py:235-366 -- cuDNN in the reference) as ONE kernel:
@@ -8,21 +8,23 @@
 //     is the SAME-shaped box of the input shifted by (kh-p, kw-p): one 4-D TMA load {64 ch, TW, TH, TB} with the tensor
 //     map's element strides carrying the conv stride, and TMA's out-of-bounds zero fill providing the padding
 //     (negative / overshooting coordinates).  It lands in shared memory as 128 rows x 128 B, SWIZZLE_128B -- exactly a
-//     K-major UMMA A operand;
+//     K-major wgmma A operand;
 //   * the B tile is a {64, BN} box of the weights stored (Cout, KH, KW, Cin) = (N, K) K-major;
-//   * k loop = KH*KW*(Cin/64) pipeline stages of 4 tcgen05.mma (M=128, N=BN=160, K=16) each, accumulator in TMEM;
-//   * 3-stage TMA <-> MMA mbarrier pipeline, warp 0 = producer, warp 1 = MMA issuer (one thread), warps 2-5 = epilogue
-//     (one output pixel per thread: tcgen05.ld, + bias / per-(b,n) time-embedding term / residual, 16-byte NHWC stores);
-//   * 111 KB shared memory + 256 TMEM columns per CTA -> 2 CTAs per SM, epilogue of one overlaps mainloop of the other.
+//   * k loop = KH*KW*(Cin/64) pipeline stages; warpgroups 0 and 1 each own 64 of the 128 pixels and issue 4 wgmma
+//     m64n160k16 per stage into a register accumulator, keeping one stage's MMAs in flight while the next one's wait;
+//   * 4-stage TMA -> wgmma mbarrier pipeline, warp 8 = TMA producer; epilogue straight from the accumulator fragment
+//     (+ bias / per-(b,n) time-embedding term / residual, 4-byte NHWC stores);
+//   * 144 KB shared memory, 1 CTA per SM (two would need <= 96 registers per thread; the 64 x 160 fp32 accumulator
+//     alone takes 80).
 // Roofline: tensor (2*M*N*K flop).
 #include "tc_common.cuh"
 
 namespace mmfs {
 
 constexpr int kConvBN = 160;          // Cout tile: 320 / 640 / 1280 = 2 / 4 / 8 x 160
-constexpr int kConvStages = 3;
-constexpr int kConvThreads = 192;
-constexpr uint32_t kConvTmemCols = 256;
+constexpr int kConvStages = 4;
+constexpr int kConvThreads = 288;     // 2 consumer warpgroups + 1 producer warp
+constexpr int kConvConsumers = 256;
 
 struct ConvParams {
     void *out;
@@ -31,10 +33,6 @@ struct ConvParams {
     int TW, TH, TB;                         // M tile = TB x TH x TW = 128 output pixels
     int tiles_w, tiles_h;                   // tiles per image along w / h
 };
-
-template <typename T> struct ConvFmt;
-template <> struct ConvFmt<__nv_bfloat16> { static constexpr int code = 1; };
-template <> struct ConvFmt<__half> { static constexpr int code = 0; };
 
 template <typename T> __device__ __forceinline__ uint32_t cpack2(float a, float b);
 template <> __device__ __forceinline__ uint32_t cpack2<__nv_bfloat16>(float a, float b) {
@@ -45,16 +43,22 @@ template <> __device__ __forceinline__ uint32_t cpack2<__half>(float a, float b)
     __half2 t = __floats2half2_rn(a, b);
     return *reinterpret_cast<uint32_t *>(&t);
 }
+template <typename T> __device__ __forceinline__ float2 cunpack2(const T *p);
+template <> __device__ __forceinline__ float2 cunpack2<__nv_bfloat16>(const __nv_bfloat16 *p) {
+    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(p));
+}
+template <> __device__ __forceinline__ float2 cunpack2<__half>(const __half *p) {
+    return __half22float2(*reinterpret_cast<const __half2 *>(p));
+}
 
 template <typename T>
-__global__ void __launch_bounds__(kConvThreads, 2)
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const ConvParams p) {
     constexpr uint32_t A_BYTES = 128 * 128, B_BYTES = kConvBN * 128, STAGE_BYTES = A_BYTES + B_BYTES;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     if ((s_addr(smem_raw) & 1023u) != 0u) { asm volatile("trap;"); }
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + kConvStages * STAGE_BYTES);
-    uint64_t *full = bars, *empty = bars + kConvStages, *acc_full = bars + 2 * kConvStages;
-    uint32_t *tmem_base_smem = reinterpret_cast<uint32_t *>(bars + 2 * kConvStages + 1);
+    uint64_t *full = bars, *empty = bars + kConvStages;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // M tile -> (batch group, h tile, w tile)
@@ -67,20 +71,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
     const int n_k = p.KH * p.KW * kc;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < kConvStages; ++i) { bar_init(full + i, 1); bar_init(empty + i, 1); }
-        bar_init(acc_full, 1);
+        for (int i = 0; i < kConvStages; ++i) { bar_init(full + i, 1); bar_init(empty + i, kConvConsumers); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_addr(tmem_base_smem)), "r"(kConvTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = *tmem_base_smem;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             for (int it = 0; it < n_k; ++it) {
                 const int s = it % kConvStages;
@@ -95,68 +91,51 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_consta
                 tma_load_2d(sa + A_BYTES, &map_w, full + s, tap * p.Cin + cb * 64, n0);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = instr_desc(ConvFmt<T>::code, 0, 128, kConvBN);
-            for (int it = 0; it < n_k; ++it) {
-                const int s = it % kConvStages;
-                bar_wait(full + s, (it / kConvStages) & 1);
-                tc_fence_after();
-                const uint32_t sa = s_addr(smem_raw) + s * STAGE_BYTES;
+        return;
+    }
+
+    const int wg = warp >> 2;                         // pixels [64 wg, 64 wg + 64) of the tile
+    float acc[kConvBN / 2];
 #pragma unroll
-                for (int kk = 0; kk < 4; ++kk)
-                    umma_f16(tmem_acc, smem_desc(sa + kk * 32, 16, 1024), smem_desc(sa + A_BYTES + kk * 32, 16, 1024), idesc,
-                             (it > 0) || (kk > 0));
-                umma_commit(empty + s);
-            }
-            umma_commit(acc_full);
-        }
-    } else {
-        const int quarter = warp & 3;
-        const int row = quarter * 32 + lane;                      // output pixel within the tile == TMEM lane
-        const uint32_t lane_sel = (uint32_t)(quarter * 32) << 16;
+    for (int i = 0; i < kConvBN / 2; ++i) acc[i] = 0.f;
+    for (int it = 0; it < n_k; ++it) {
+        const int s = it % kConvStages;
+        bar_wait(full + s, (it / kConvStages) & 1);
+        const uint32_t sa = s_addr(smem_raw) + s * STAGE_BYTES;
+        reg_fence(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+            Wgmma<T>::ss_n160(acc, smem_desc(sa + wg * 64 * 128 + kk * 32, 16, 1024), smem_desc(sa + A_BYTES + kk * 32, 16, 1024), 1);
+        wgmma_commit();
+        wgmma_wait<1>();                              // the previous stage's MMAs have retired: release its buffers
+        reg_fence(acc);
+        if (it > 0) bar_arrive(empty + (it - 1) % kConvStages);
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
+
+    // epilogue: thread holds pixels (row, row + 8) x channels 8 j + 2 (lane % 4) + {0, 1}
+    const int tq = lane & 3;
+    const T *bp = p.bias ? static_cast<const T *>(p.bias) + n0 + 2 * tq : nullptr;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
         const int pw = row % p.TW, phh = (row / p.TW) % p.TH, pb = row / (p.TW * p.TH);
         const int b = b0 + pb, ho = h0 + phh, wo = w0 + pw;
-        const bool ok = (b < p.B) && (ho < p.Ho) && (wo < p.Wo);
+        if (b >= p.B || ho >= p.Ho || wo >= p.Wo) continue;
         const size_t pix = ((size_t)b * p.Ho + ho) * p.Wo + wo;
-        T *op = static_cast<T *>(p.out) + pix * p.Cout + n0;
-        const T *rp = p.residual ? static_cast<const T *>(p.residual) + pix * p.Cout + n0 : nullptr;
-        const T *ap = p.add_bc ? static_cast<const T *>(p.add_bc) + (size_t)b * p.Cout + n0 : nullptr;
-        const T *bp = p.bias ? static_cast<const T *>(p.bias) + n0 : nullptr;
-        bar_wait(acc_full, 0);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < kConvBN; c += 32) {
-            float acc[32];
-            tmem_ld32(tmem_acc + lane_sel + c, acc);              // warp-collective: every lane takes part
-            if (ok) {
+        T *op = static_cast<T *>(p.out) + pix * p.Cout + n0 + 2 * tq;
+        const T *rp = p.residual ? static_cast<const T *>(p.residual) + pix * p.Cout + n0 + 2 * tq : nullptr;
+        const T *ap = p.add_bc ? static_cast<const T *>(p.add_bc) + (size_t)b * p.Cout + n0 + 2 * tq : nullptr;
 #pragma unroll
-                for (int qd = 0; qd < 4; ++qd) {
-                    float e[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) e[i] = acc[qd * 8 + i];
-                    if (bp) { float f[8]; Vec16<T>::unpack(*reinterpret_cast<const uint4 *>(bp + c + qd * 8), f);
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) e[i] += f[i]; }
-                    if (ap) { float f[8]; Vec16<T>::unpack(*reinterpret_cast<const uint4 *>(ap + c + qd * 8), f);
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) e[i] += f[i]; }
-                    if (rp) { float f[8]; Vec16<T>::unpack(*reinterpret_cast<const uint4 *>(rp + c + qd * 8), f);
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) e[i] += f[i]; }
-                    uint4 w;
-                    w.x = cpack2<T>(e[0], e[1]); w.y = cpack2<T>(e[2], e[3]); w.z = cpack2<T>(e[4], e[5]); w.w = cpack2<T>(e[6], e[7]);
-                    *reinterpret_cast<uint4 *>(op + c + qd * 8) = w;
-                }
-            }
-            __syncwarp();
+        for (int j = 0; j < kConvBN / 8; ++j) {
+            float e0 = acc[j * 4 + 2 * i], e1 = acc[j * 4 + 2 * i + 1];
+            if (bp) { const float2 f = cunpack2<T>(bp + j * 8); e0 += f.x; e1 += f.y; }
+            if (ap) { const float2 f = cunpack2<T>(ap + j * 8); e0 += f.x; e1 += f.y; }
+            if (rp) { const float2 f = cunpack2<T>(rp + j * 8); e0 += f.x; e1 += f.y; }
+            *reinterpret_cast<uint32_t *>(op + j * 8) = cpack2<T>(e0, e1);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "r"(kConvTmemCols) : "memory");
     }
 }
 
@@ -208,7 +187,7 @@ extern "C" int mmfs_conv2d_nhwc(const void *x, const void *w, const void *bias, 
     p.out = out; p.bias = bias; p.add_bc = add_bc; p.residual = residual;
     p.B = B; p.Ho = Ho; p.Wo = Wo; p.Cin = Cin; p.Cout = Cout; p.KH = KH; p.KW = KW; p.stride = stride; p.pad = pad;
     p.TW = TW; p.TH = TH; p.TB = TB; p.tiles_w = Wo / TW; p.tiles_h = Ho / TH;
-    const size_t smem = (size_t)kConvStages * (128 * 128 + kConvBN * 128) + (2 * kConvStages + 1) * 8 + 16;
+    const size_t smem = (size_t)kConvStages * (128 * 128 + kConvBN * 128) + 2 * kConvStages * 8;
     dim3 grid((unsigned)(p.tiles_w * p.tiles_h * (B / TB)), (unsigned)(Cout / kConvBN));
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == MMFS_BF16) {

@@ -3,9 +3,8 @@
 // 217-280, with the RMSNorm in front of them, :53-70, and the SwiGLU between them, :188-189, folded in).
 //
 // At M = batch (4 at cfg 5) every weight byte is used once per token: the op is a stream of W out of HBM (27 GB per
-// token for the 13 B decoder), not a tensor-core problem.  What the round-2 decode profile showed for cuBLAS here:
-// 5.9-6.0 TB/s on the two wide projections, 4.8 TB/s on the two N = 5120 ones (80-odd CTAs for 148 SMs), plus a
-// separate RMSNorm / SwiGLU kernel in front of each pair.  This kernel:
+// token for the 13 B decoder), not a tensor-core problem.  cuBLAS needs a separate RMSNorm / SwiGLU kernel in front
+// of each pair, and its N = 5120 projections launch fewer CTAs than there are SMs.  This kernel:
 //   * persistent, one CTA of 16 warps per SM.  The work is numbered in STEPS: step (block b, J) = the 32 weight rows of
 //     block b x the 512 columns J*512 .. J*512+511, block-major; the steps are cut into equal contiguous ranges, one
 //     per CTA ("stream-K" at 32 KB granularity): every SM streams the same number of bytes whatever N is;
@@ -16,17 +15,15 @@
 //     the B fragments of two MMAs whose A fragments are the matching 16 bytes of x row g.  No shuffles, no unpacking,
 //     no shared-memory staging of W.  Rows 8-15 of the m16 tile are unused.  (The math is ~2 % of
 //     the tensor pipe; the legacy mma path is used because the output tile is 8 x 8 and the operand arrives in
-//     registers -- tcgen05's M = 128 tile, TMEM allocation and commit protocol buy nothing for an HBM-bound stream.)
+//     registers -- wgmma's 64-row warpgroup tile and shared-memory operands buy nothing for an HBM-bound stream.)
 //   * memory-level parallelism: every lane keeps 3-4 steps x 4 cp.async (16-byte, L2-only) copies of ITS OWN future
 //     operands in flight into private 16-byte slots of a shared-memory ring and reads them back itself (no barrier: a
 //     thread sees its own completed copies after cp.async.wait_group) -- 96-128 KB in flight per SM, across block
 //     boundaries and across the reduction barriers.  Plain loads into a register ring do not get there: a warp has six
-//     scoreboards, so twelve individually tracked loads serialise (measured at 8-row blocks: 1.7 TB/s re-issuing one
-//     load per step, 3.6 TB/s in groups of four; cp.async: 4.3 TB/s but ISSUE-bound at 33 instructions per 512 bytes --
-//     hence four row groups per step: one x fragment, one cursor update, one commit per 2 KB).
-//     (The first version of this kernel staged W through a shared-memory ring filled by cp.async.bulk row pieces and
-//     ldmatrix: 2.4-3.0 TB/s with 1 KB pieces, 5.2 TB/s with 5 KB pieces -- profiles/r02_skinny_linear_tma_ring_ab.log:
-//     the 1-D bulk copies cost ~30 ns + 23 ns/KB each on the SM's copy engine, an asymptote below the cuBLAS kernels.)
+//     scoreboards, so twelve individually tracked loads serialise; cp.async at 8-row blocks is issue-bound (33
+//     instructions per 512 bytes) -- hence four row groups per step: one x fragment, one cursor update, one commit per
+//     2 KB.  (The first version of this kernel staged W through a shared-memory ring filled by cp.async.bulk row pieces
+//     and ldmatrix; every 1-D bulk copy pays a fixed cost on the SM's copy engine, which caps that design.)
 //   * x is staged ONCE per CTA in shared memory by the consumer warps while the producer already streams W, through
 //     the prologue: plain copy | RMSNorm(x) * weight (LlamaRMSNorm's rounding points: T(x * rstd), then * weight in T) |
 //     SwiGLU of a [gate | up] row pair (T(silu(gate)) * up in T) -- the same arithmetic as the stand-alone kernels in
@@ -107,8 +104,8 @@ __device__ __forceinline__ uint4 sk_perm(const uint4 &v) { return make_uint4(v.x
 
 // ---- x -> shared memory through the prologue (all 512 threads) ----------------------------------------------------------
 // All global loads of a pass are issued in batches of kSkXBatch independent vectors per thread BEFORE anything is done
-// with them: the first version walked the rows with load -> use -> load and cost 8-15 us per call (x sits in L2, ~0.4 us
-// per dependent round trip, up to 32 of them for the 13824-wide SwiGLU operand) -- the whole gap to the library kernels.
+// with them: walking the rows with load -> use -> load pays one dependent L2 round trip per vector (up to 32 of them
+// for the 13824-wide SwiGLU operand).
 constexpr int kSkXBatch = 8;
 
 template <typename T, int NT, bool PERM>

@@ -123,8 +123,8 @@ constexpr int kLnChunks = 8;
 
 // CH = 16-byte vectors per lane (1, 2, 4 or 8: rows of up to 32*CH*VEC elements).  The row is kept as raw 16-byte
 // registers and unpacked three times (sum, centred squares, output): 4 registers per vector instead of 8 floats, so
-// the common CH <= 4 instantiations stay under 64 registers and 32+ warps per SM hide the load latency (the first
-// version held the row as floats for CH = 8 always: 126 registers, 16 warps per SM, 1.1-1.5 TB/s).
+// the common CH <= 4 instantiations stay under 64 registers and 32+ warps per SM hide the load latency (holding the
+// row as floats for CH = 8 always needs 126 registers, i.e. 16 warps per SM).
 template <typename T, int CH>
 __global__ void __launch_bounds__(256, CH == 8 ? 2 : 4) layernorm_warp_kernel(const T *__restrict__ x, const T *__restrict__ w,
                                                               const T *__restrict__ b, T *__restrict__ y, long rows, int cols, float eps) {
@@ -381,7 +381,7 @@ static int launch_all(int which, const void *a, const void *b, const void *c, vo
         case 2: { // rope: d=q (in place), a=k (in place, cast away const), e=cos f=sin c=pos; n0=tokens i0=H i1=hd i2=q_stride i3=k_stride i4=pos_per_batch i5=T
             const int per_tok = i0 * 2 * ((i1 / 2) / (16 / (int)sizeof(T)));
             const int threads = per_tok >= 256 ? 256 : ((per_tok + 31) / 32) * 32;
-            const int grid = (int)(n0 < 148L * 32 ? n0 : 148L * 32);
+            const int grid = (int)(n0 < (long)num_sms() * 32 ? n0 : (long)num_sms() * 32);
             rope_qk_kernel<T><<<grid, threads, 0, st>>>((T *)d, (T *)const_cast<void *>(a), (const float *)e, (const float *)f,
                                                      (const int64_t *)c, n0, i0, i1, i2, i3, i4, i5);
             break;
@@ -389,9 +389,9 @@ static int launch_all(int which, const void *a, const void *b, const void *c, vo
         case 3: { // swiglu / geglu: a=gate_up d=out n0=rows i0=I i1=variant (0 silu [gate|up], 1 gelu [value|gate])
             const int nvec = i0 / (16 / (int)sizeof(T));
             const int threads = nvec >= 512 ? 256 : (nvec >= 64 ? 64 : 32);
-            const int gx = (int)(n0 < 148L * 64 ? n0 : 148L * 64);
+            const int gx = (int)(n0 < (long)num_sms() * 64 ? n0 : (long)num_sms() * 64);
             int gy = 1;                                   // fewer CTAs than SMs: slice the columns (two vectors per thread)
-            if (gx < 148) { gy = (nvec + 2 * threads - 1) / (2 * threads); if (gy > 64) gy = 64; if (gy < 1) gy = 1; }
+            if (gx < num_sms()) { gy = (nvec + 2 * threads - 1) / (2 * threads); if (gy > 64) gy = 64; if (gy < 1) gy = 1; }
             const dim3 grid(gx, gy);
             if (i1 == 1)
                 swiglu_kernel<T, 1, true><<<grid, threads, 0, st>>>((const T *)a, (T *)d, n0, i0);
@@ -455,7 +455,7 @@ static int launch_rope_append(void *q, const void *k, const void *v, const float
                               int qs, int ks, int vs, long cbs, long cts, int ppb, cudaStream_t st) {
     const int items = H * ((hd / 2) / (16 / (int)sizeof(T))) * 2 + H * hd / (16 / (int)sizeof(T));
     const int threads = items >= 256 ? 256 : ((items + 31) / 32) * 32;
-    const int grid = (int)(n_tok < 148L * 32 ? n_tok : 148L * 32);
+    const int grid = (int)(n_tok < (long)num_sms() * 32 ? n_tok : (long)num_sms() * 32);
     rope_append_kernel<T><<<grid, threads, 0, st>>>((T *)q, (const T *)k, (const T *)v, cos_t, sin_t, pos, (T *)kc, (T *)vc, slot_dev,
                                                  slot_host, n_tok, H, hd, qs, ks, vs, cbs, cts, ppb, T_len);
     MMFS_CUDA(cudaGetLastError());

@@ -1,4 +1,4 @@
-// mmfs_sampler_sm100.cu -- fused MMFS sampler for sm_100a.
+// mmfs_sampler_sm100.cu -- fused MMFS sampler for sm_90a.
 //
 // Replaces the un-fused middle of the reference's MMFS.forward
 //   ops/modules/mmfs.py:178-273  (relpos embedding add, offset / weight views and rearranges,

@@ -1,4 +1,4 @@
-// msda_bwd_sm100.cu -- multi-scale deformable attention BACKWARD for sm_100a (training path; SURVEY.md 8f rank 4).
+// msda_bwd_sm100.cu -- multi-scale deformable attention BACKWARD for sm_90a (training path; SURVEY.md 8f rank 4).
 //
 // Replaces ms_deform_attn_cuda_backward (ops/src/cuda/ms_deform_attn_cuda.cu:84-166) and the nine col2im kernels
 // of ops/src/cuda/ms_deform_im2col_cuda.cuh:304-923 (+ launcher :959-1330) with ONE kernel that reuses the forward's

@@ -1,9 +1,9 @@
-// msda_fwd_sm100.cu -- multi-scale deformable attention forward for sm_100a.
+// msda_fwd_sm100.cu -- multi-scale deformable attention forward for sm_90a.
 //
 // Replaces the reference's thread-per-output-scalar kernel
 //   ops/src/cuda/ms_deform_im2col_cuda.cuh:240-302 (ms_deformable_im2col_gpu_kernel)
 //   ops/src/cuda/ms_deform_im2col_cuda.cuh:36-87   (ms_deform_attn_im2col_bilinear)
-// with a B200-first design (nothing here is translated from the reference kernel):
+// with a H100-first design (nothing here is translated from the reference kernel):
 //
 //   * one WARP per output row (b, q, m); every warp-level fetch moves 512 B: the warp is
 //     split into RPI = 32 / (D*sizeof(T)/16) "slots", each slot fetches one 16-byte-
@@ -313,10 +313,9 @@ static int launch_rows(const void *value, const int64_t *shapes, const int64_t *
     MMFS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern, 32 * kWarpsPerCta, smem));
     if (ctas_per_sm < 1) { set_error("msda: kernel does not fit on an SM (smem %zu)", smem); return MMFS_EUNSUPPORTED; }
     const int nsm = num_sms();
-    // rows per warp per tile: short tiles win on every measured shape (profiles/r01_msda_sweep_v3.json: cfg 3
-    // 144 us at 2 vs 170 us at 8; SD Lq 4096 110 vs 131; Lq 1024 35-40 vs 41): neighbouring q-tiles of one head still
-    // share the L1-resident value slab through the per-SM tile swizzle, and short tiles balance the tail of the
-    // persistent grid.  Tiny problems (decode, Lq = 1) use 1.
+    // rows per warp per tile: short tiles -- neighbouring q-tiles of one head still share the L1-resident value slab
+    // through the per-SM tile swizzle, and short tiles balance the tail of the persistent grid (tools/msda_sweep.py
+    // times the alternatives).  Tiny problems (decode, Lq = 1) use 1.
     int rpw = g_rows_per_warp;
     if (rpw <= 0) {
         rpw = 2;
@@ -343,7 +342,7 @@ static int launch_generic(const void *value, const int64_t *shapes, const int64_
                           unsigned flags, cudaStream_t st) {
     const long total = (long)N * Lq * M * D;
     const long blocks = (total + 255) / 256;
-    const int grid = (int)(blocks < 148L * 32 ? blocks : 148L * 32);
+    const int grid = (int)(blocks < (long)num_sms() * 32 ? blocks : (long)num_sms() * 32);
     msda_fwd_generic_kernel<T><<<grid, 256, 0, st>>>((const T *)value, shapes, starts, (const T *)loc,
                                                        (const T *)attn, (T *)out, total, S, M, D, L, Lq, P, flags);
     MMFS_CUDA(cudaGetLastError());
@@ -439,7 +438,7 @@ extern "C" int mmfs_msda_index_stream(const int64_t *shapes, const int64_t *star
     MMFS_CHECK_ARG(shapes && starts && loc && idx, "msda_index_stream: null pointer argument");
     cudaStream_t st = (cudaStream_t)stream;
     const long blocks = (total + 255) / 256;
-    const int grid = (int)(blocks < 148L * 32 ? blocks : 148L * 32);
+    const int grid = (int)(blocks < (long)num_sms() * 32 ? blocks : (long)num_sms() * 32);
     switch (dtype) {
         case MMFS_F32: msda_index_stream_kernel<float><<<grid, 256, 0, st>>>(shapes, starts, (const float *)loc, idx, total, M, D, L, P); break;
         case MMFS_F16: msda_index_stream_kernel<__half><<<grid, 256, 0, st>>>(shapes, starts, (const __half *)loc, idx, total, M, D, L, P); break;

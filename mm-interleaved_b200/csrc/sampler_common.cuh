@@ -56,13 +56,9 @@ __device__ __forceinline__ bool corner_valid(int corner, int h_low, int w_low, i
 }
 
 __device__ __forceinline__ void fma2(float &a0, float &a1, float w0, float w1, float v0, float v1) {
-    // Blackwell packed fp32 FMA (fma.rn.f32x2): two accumulator updates per issue slot.
-    unsigned long long acc, vv, ww;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(acc) : "f"(a0), "f"(a1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(vv) : "f"(v0), "f"(v1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ww) : "f"(w0), "f"(w1));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(ww), "l"(vv));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a0), "=f"(a1) : "l"(acc));
+    // two independent fp32 FMAs (Hopper has no packed fp32 pipe)
+    a0 = __fmaf_rn(w0, v0, a0);
+    a1 = __fmaf_rn(w1, v1, a1);
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -96,7 +92,7 @@ static __device__ uint4 g_zero_row[32];
 
 struct __align__(16) Tap {  // mailbox record handed from the index-math lane to the fetching slot
     long long off;          // byte offset from the head slab origin (or to g_zero_row)
-    float w0, w1;           // lerp weight * attention weight, duplicated for fma.rn.f32x2
+    float w0, w1;           // lerp weight * attention weight, duplicated for fma2
 };
 
 template <typename T> __device__ __forceinline__ float elem_to_f32(const T *p);
@@ -174,23 +170,23 @@ __device__ __forceinline__ void gather_pass(const Tap *taps, unsigned livemask, 
     }
 }
 
-// Mixed-precision FMA of sm_100 (SASS FHFMA): d = a(16-bit, half selected in the register) * b(16-bit) + c(fp32).
-// It consumes the packed value register directly -- no unpack -- at the price of a 16-bit weight.
+// Mixed-precision FMA: d = a(16-bit) * b(16-bit) + c(fp32) with one rounding.  Both 16-bit operands widen to fp32
+// exactly, so an fp32 FMA on the widened values gives the same result; the saving is the 16-bit weight's register.
 template <typename T> struct MixFma;
 template <> struct MixFma<__nv_bfloat16> {
     __device__ __forceinline__ static void fma(float &acc, uint16_t v, uint16_t w) {
-        asm("fma.rn.f32.bf16 %0, %1, %2, %0;" : "+f"(acc) : "h"(v), "h"(w));
+        acc = __fmaf_rn(__uint_as_float((uint32_t)v << 16), __uint_as_float((uint32_t)w << 16), acc);
     }
     __device__ __forceinline__ static uint16_t cvt(float w) { __nv_bfloat16 t = __float2bfloat16_rn(w); return *reinterpret_cast<uint16_t *>(&t); }
 };
 template <> struct MixFma<__half> {
     __device__ __forceinline__ static void fma(float &acc, uint16_t v, uint16_t w) {
-        asm("fma.rn.f32.f16 %0, %1, %2, %0;" : "+f"(acc) : "h"(v), "h"(w));
+        acc = __fmaf_rn(__half2float(__ushort_as_half(v)), __half2float(__ushort_as_half(w)), acc);
     }
     __device__ __forceinline__ static uint16_t cvt(float w) { __half t = __float2half_rn(w); return *reinterpret_cast<uint16_t *>(&t); }
 };
 
-// gather_pass with 16-bit tap weights (MMFS_MSDA_W16): 8 FHFMA per 16-byte fetch instead of 8 unpack + 4 FFMA2
+// gather_pass with 16-bit tap weights (MMFS_MSDA_W16): 8 mixed-precision FMA per 16-byte fetch instead of 8 unpack + 8 FFMA
 template <typename T, int D>
 __device__ __forceinline__ void gather_pass_w16(const Tap *taps, unsigned livemask, const char *vbase, int slot,
                                                 float (&acc)[16 / sizeof(T)]) {

@@ -18,7 +18,7 @@ def shard_range(n_items: int, rank: int, world: int) -> List[int]:
 def gather_results(local: torch.Tensor, n_items: int, rank: int, world: int, group=None) -> torch.Tensor:
     """All-gather the per-rank result rows (same trailing shape on every rank) and put them back in global
     batch order.  Ranks may own different numbers of rows (n_items not divisible by world): rows are padded
-    to the maximum for the collective.  NCCL on GPUs (NVLink 5 / NVSwitch), gloo in the CPU tests."""
+    to the maximum for the collective.  NCCL on GPUs (NVLink / NVSwitch), gloo in the CPU tests."""
     import torch.distributed as dist
     if world == 1:
         return local

@@ -2,7 +2,7 @@
 
 ``MSDeformAttnFunction.apply(value, shapes, level_start_index, sampling_locations,
 attention_weights, im2col_step)`` keeps the reference signature; the forward runs the
-sm_100a kernel.  Unlike the reference (``@custom_fwd`` without ``cast_inputs``,
+sm_90a kernel.  Unlike the reference (``@custom_fwd`` without ``cast_inputs``,
 func.py:26), a dtype mismatch between ``value`` and the location / weight tensors --
 which the reference op would mis-read (SURVEY.md section 7 hard part iv) -- is resolved by
 casting them to ``value.dtype``.

@@ -1,14 +1,14 @@
-"""Llama decoder with injected MMFS cross-attention, B200-native.
+"""Llama decoder with injected MMFS cross-attention, H100-native.
 
 Mirrors the module / parameter naming and the forward signatures of the reference's
 ``mm_interleaved/models/decoders/modeling_llama_mmfs.py`` (LlamaRMSNorm :53, LlamaMLP :175,
 LlamaAttention :192, LlamaMMFSAttention :311, LlamaDecoderLayer :370, LlamaModel :562) so that a
 reference checkpoint's state dict loads unchanged (``layers.N.self_attn.q_proj.weight`` ...), but
-the forward is built for B200:
+the forward is built for H100:
 
 * q/k/v and gate/up projections run as ONE cuBLAS GEMM each on concatenated weights; o_proj and
   down_proj fold the residual add into the GEMM (``addmm``, beta = 1);
-* RMSNorm, RoPE, SwiGLU and attention are hand-written sm_100a kernels (ops.py); q/k/v stay in the
+* RMSNorm, RoPE, SwiGLU and attention are hand-written sm_90a kernels (ops.py); q/k/v stay in the
   GEMM's (B, T, H, hd) layout -- no transposes, no materialised (B, H, T, T) score tensor, no
   additive 4-D mask (causality + key padding are applied inside the attention kernel);
 * the MMFS cross-attention uses the fused sampler (mmfs.py); RMSNorm(vision) and
@@ -110,9 +110,8 @@ class _CatWeight:
 
 
 # Decode-step linears (at most 8 tokens in flight): ``ops.linear_skinny`` -- this repo's HBM-streaming kernel with the
-# RMSNorm / SwiGLU in front folded in -- or cuBLAS + the stand-alone norm / activation kernel.  Measured on the 13 B
-# decoder at batch 4 (profiles/r02_skinny_linear_ab.log): 151 us per layer against 130 us for cuBLAS, so cuBLAS stays the
-# default (DESIGN.md section 4.7); MMFS_SKINNY_LINEARS=1 or ``llama_mmfs.SKINNY_DECODE_LINEARS = True`` switches.
+# RMSNorm / SwiGLU in front folded in -- or cuBLAS + the stand-alone norm / activation kernel.  cuBLAS is the default
+# (DESIGN.md section 4.7); MMFS_SKINNY_LINEARS=1 or ``llama_mmfs.SKINNY_DECODE_LINEARS = True`` switches.
 SKINNY_DECODE_LINEARS = os.environ.get("MMFS_SKINNY_LINEARS", "0") == "1"
 
 

@@ -762,7 +762,7 @@ class MMInterleaved(InterleavedForward):
 
     # ---------------------------------------------------------------------------------------------------------
     def enable_cuda_graphs(self, tokenizer: bool = True) -> "MMInterleaved":
-        """Replay the visual tokenizer (~2400 kernels of 5-50 us per 16 images) from a CUDA graph captured once per
+        """Replay the visual tokenizer (~2400 small kernels per 16 images) from a CUDA graph captured once per
         image-batch shape (SURVEY.md 8 f3).  Inference only; the tokenizer's outputs then live in static buffers that
         the next call overwrites -- everything this class returns to the caller is cloned out of them."""
         from ._graphs import GraphedCallable

@@ -1,4 +1,4 @@
-"""``MMFS`` -- Multi-Image Multi-Scale Feature Synchronizer, B200-native.
+"""``MMFS`` -- Multi-Image Multi-Scale Feature Synchronizer, H100-native.
 
 Drop-in for the reference module ``mm_interleaved.models.utils.ops.modules.mmfs.MMFS``
 (ops/modules/mmfs.py:25-276): same constructor arguments, same parameter / state-dict names
@@ -11,7 +11,7 @@ Drop-in for the reference module ``mm_interleaved.models.utils.ops.modules.mmfs.
 * the per-image conditioning ``Linear(q1 + relpos_embed[r])`` (mmfs.py:178-191) is factored by
   linearity into ``Linear(q1)`` (one GEMM producing offsets and logits for all heads) plus a
   ``(max_num_image_per_seq, C)`` table ``W @ relpos_embed`` looked up inside the sampler kernel;
-* mask add, null-slot softmax, location arithmetic and the deformable gather are one sm_100a
+* mask add, null-slot softmax, location arithmetic and the deformable gather are one sm_90a
   kernel (csrc/mmfs_sampler_sm100.cu); the (N,Lq,M,L,P,2) / (N,Lq,M,L,P) tensors never exist;
 * ``value_proj(input_flatten)`` is cached while the same feature tensor is passed again (decode
   steps, denoise steps) -- the reference recomputes it every call (mmfs.py:165).
@@ -163,9 +163,9 @@ class MMFS(nn.Module):
                                f"(got {self.max_num_image_per_seq})")
         if reference_points.shape[-1] != 2:
             # the box form (mmfs.py:251-258) is not used by any caller on the interleaved forward path
-            raise NotImplementedError("MMFS (B200): only 2-D reference points are implemented")
+            raise NotImplementedError("MMFS (H100): only 2-D reference points are implemented")
         if not query.is_cuda:
-            raise RuntimeError("MMFS (B200) runs on CUDA tensors only (no CPU fallback)")
+            raise RuntimeError("MMFS (H100) runs on CUDA tensors only (no CPU fallback)")
 
         if value is None:
             value = self.project_value(input_flatten, input_padding_mask)

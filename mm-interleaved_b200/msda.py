@@ -2,7 +2,7 @@
 ``MultiScaleDeformableAttention`` (ops/src/vision.cpp:13-16, ops/src/ms_deform_attn.h:20-61).
 
 Host code stays PyTorch (device memory, streams); the arithmetic is the hand-written
-sm_100a kernel behind the C ABI (csrc/msda_fwd_sm100.cu).
+sm_90a kernel behind the C ABI (csrc/msda_fwd_sm100.cu).
 """
 from __future__ import annotations
 
@@ -92,7 +92,7 @@ def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_l
     _require(grad_output.is_cuda and grad_output.is_contiguous() and grad_output.dtype == value.dtype and
              tuple(grad_output.shape) == (N, Lq, M * D), "grad_output must be a contiguous CUDA tensor (N, Lq, M*D) of value's dtype")
     if value.dtype == torch.float64:
-        raise NotImplementedError("ms_deform_attn_backward: float64 is not implemented on the B200 path")
+        raise NotImplementedError("ms_deform_attn_backward: float64 is not implemented on the H100 path")
     gl = torch.empty((N, Lq, M, L, P, 2), dtype=torch.float32, device=value.device)
     ga = torch.empty((N, Lq, M, L, P), dtype=torch.float32, device=value.device)
     if deterministic:

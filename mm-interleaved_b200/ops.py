@@ -140,7 +140,7 @@ def geglu(value_gate: torch.Tensor) -> torch.Tensor:
 def attention(q, k, v, key_mask=None, causal=True, past=0, scale=None, force_generic=False) -> torch.Tensor:
     """softmax(q k^T * scale + mask) v.  q (B,Tq,H,hd), k/v (B,Tkv,H,hd) -- any batch / token strides, heads
     dense; key_mask (B,Tkv) bool/uint8 (1 = attend) or None; causal: query i sees keys j <= past + i.
-    Returns (B, Tq, H*hd).  Prefill shapes go to the tcgen05 kernel, decode / odd shapes to the
+    Returns (B, Tq, H*hd).  Prefill shapes go to the wgmma kernel, decode / odd shapes to the
     bandwidth kernel (see csrc/attn_generic_sm100.cu)."""
     B, Tq, H, hd = q.shape
     Tkv = k.shape[1]

@@ -4,7 +4,7 @@ mm_interleaved/models/utils/monkey_patch/__init__.py:1-5), pointed at this repos
 Call them where ``inference.py`` / ``evaluate.py`` call ``replace_blip2_attn_with_qknorm_attn()`` etc., i.e. after
 ``import mm_interleaved...`` and BEFORE ``MMInterleaved(**config.model)`` is constructed (inference.py:291).  Every
 function rebinds the reference class objects wherever a reference module already holds them (``from ..x import MMFS``
-creates a second binding in the importer's namespace), so construction afterwards builds the B200 modules while the
+creates a second binding in the importer's namespace), so construction afterwards builds the H100 modules while the
 reference's own ``MMInterleaved`` / ``LlamaModel`` / ``ImageDecoder`` glue, state-dict names and checkpoints stay as
 they are.  Nothing here imports the reference: the functions look the modules up in ``sys.modules`` / by name and raise
 if the reference package is not importable.
@@ -74,7 +74,7 @@ def replace_msda_b200() -> None:
         mod.ms_deform_attn_forward = _msda.ms_deform_attn_forward
         mod.ms_deform_attn_backward = _msda.ms_deform_attn_backward
         mod._b200_dropin = True
-        mod.__doc__ = "B200 drop-in for the reference's compiled extension (libmmfs_b200.so behind ctypes)"
+        mod.__doc__ = "H100 drop-in for the reference's compiled extension (libmmfs_b200.so behind ctypes)"
         sys.modules["MultiScaleDeformableAttention"] = mod
     for name in (f"{_REF}.models.utils.ops.functions.ms_deform_attn_func",
                  f"{_REF}.models.encoders.vit_adapter.ops.functions.ms_deform_attn_func"):
@@ -97,7 +97,7 @@ def replace_mmfs_b200() -> None:
 def replace_llama_b200() -> None:
     """The decoder building blocks of decoders/modeling_llama_mmfs.py (LlamaRMSNorm :53, LlamaMLP :175, LlamaAttention
     :192, LlamaMMFSAttention :311, LlamaDecoderLayer :370): parameter names are identical, so the reference's
-    ``LlamaModel`` / ``LlamaForCausalLM`` construct and load checkpoints unchanged and run the B200 layer."""
+    ``LlamaModel`` / ``LlamaForCausalLM`` construct and load checkpoints unchanged and run the H100 layer."""
     from . import llama_mmfs as b
     replace_mmfs_b200()
     ref = _module(f"{_REF}.models.decoders.modeling_llama_mmfs")

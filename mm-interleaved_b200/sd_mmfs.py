@@ -1,4 +1,4 @@
-"""``MMFSBlock`` / ``MMFSNet`` -- the MMFS conditioning branch of the SD-2.1 UNet, B200-native.
+"""``MMFSBlock`` / ``MMFSNet`` -- the MMFS conditioning branch of the SD-2.1 UNet, H100-native.
 
 Mirrors ``mm_interleaved/models/decoders/sd_mmfs.py`` (MMFSBlock :44-145, MMFSNet :154-272): same
 constructor arguments, parameter names (``mmfs_down_blocks.N.{query_norm,feat_norm,mmfs.*,pos_embed,conv}``,

@@ -1,4 +1,4 @@
-"""SD-2.1-base UNet denoise step with the MMFS conditioning hook, B200-native assembly.
+"""SD-2.1-base UNet denoise step with the MMFS conditioning hook, H100-native assembly.
 
 The reference does not contain the UNet arithmetic: it monkey-patches diffusers 0.20.0's
 ``UNet2DConditionModel.forward`` (utils/monkey_patch/sd_unet_forward_monkey_patch.py:17-371) to take three
@@ -11,10 +11,10 @@ naming so that a reference checkpoint's ``unet.*`` keys map one-to-one, and keep
 signature.  **Parity is unpinned** (no reference-side test, golden vector or importable implementation exists
 here); the block-level formulas are checked against plain PyTorch statements in tests/test_unet_gpu.py.
 
-B200 side: every self- and cross-attention runs in this repo's tcgen05 kernel (T in {4096, 1024, 256, 64},
+H100 side: every self- and cross-attention runs in this repo's wgmma kernel (T in {4096, 1024, 256, 64},
 head size 64, kv = 77 for cross attention), the MMFS branch in the fused sampler (sd_mmfs.py), LayerNorms in the
 warp-per-row kernel, and every 3x3 / 1x1 convolution with Cin % 64 == 0 and Cout % 160 == 0 (all but conv_in / conv_out
-when the model is bf16/f16 and channels-last) in the implicit-GEMM tcgen05 kernel (csrc/conv_igemm_sm100.cu) with the
+when the model is bf16/f16 and channels-last) in the implicit-GEMM wgmma kernel (csrc/conv_igemm_sm100.cu) with the
 ResNet block's time-embedding add and residual add fused into its epilogue; GroupNorm(+SiLU) runs in an NHWC kernel
 (csrc/groupnorm_nhwc_sm100.cu) because torch's CUDA group_norm returns NCHW and would force a layout round trip
 around every convolution.
@@ -43,7 +43,7 @@ def _gn(mod: nn.GroupNorm, x: torch.Tensor, silu: bool) -> torch.Tensor:
 
 def _conv(mod: nn.Conv2d, x: torch.Tensor, add_bc: Optional[torch.Tensor] = None,
           residual: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``mod(x) [+ add_bc[:, :, None, None]] [+ residual]`` -- on the tcgen05 implicit-GEMM kernel when the layer
+    """``mod(x) [+ add_bc[:, :, None, None]] [+ residual]`` -- on the wgmma implicit-GEMM kernel when the layer
     qualifies (ops.conv2d_supported), else on the library convolution."""
     stride, pad = mod.stride[0], mod.padding[0]
     if USE_CONV_KERNEL and x.is_contiguous(memory_format=torch.channels_last) and ops.conv2d_supported(x, mod.weight, stride, pad):
@@ -305,9 +305,8 @@ class GraphedUNet:
     """One UNet evaluation captured in a CUDA graph and replayed for every denoise step -- of every loop of the same
     shape.
 
-    An evaluation is ~1200 launches of 5-100 us kernels; issued eagerly, a third of the wall time of a step is launch
-    gaps (20 ms of kernels in 28 ms at batch 16).  Capturing + instantiating the graph costs ~400 ms, more than one
-    50-step loop saves, so the graph must outlive the loop: ``sample`` and ``timestep`` (per step) and the context, the
+    An evaluation is ~1200 kernel launches; issued eagerly, part of the wall time of a step is launch gaps.  Capturing
+    + instantiating the graph costs more than one 50-step loop saves, so the graph must outlive the loop: ``sample`` and ``timestep`` (per step) and the context, the
     mask and the MMFS image-side state (per loop) all live in static buffers.  ``load`` refills the per-loop ones --
     the image-side state through ``MMFSNet.prepare(features, out=...)``, i.e. recomputed eagerly into the storage the
     graph reads -- and ``__call__`` replays.  The returned tensor lives in the graph's memory pool: consume it before
@@ -377,9 +376,9 @@ def denoise_loop(unet, latents, cond, uncond, mmfs_features, mmfs_mask, mmfs_mod
     feats2 = [torch.cat([f, f], 0) for f in mmfs_features] if mmfs_features is not None else None
     mask2 = torch.cat([mmfs_mask, mmfs_mask], 0) if mmfs_mask is not None else None
     if cuda_graph is None:
-        # Capturing + instantiating the ~1200-node graph costs ~400 ms (measured, batch 16) -- more than the launch
-        # overhead it removes from ONE 50-step loop (1934 vs 1540 ms) -- so a graph is used only when the caller keeps
-        # it across loops (graph_cache), with the per-loop MMFS state refreshed in place (GraphedUNet.load).
+        # Capturing + instantiating the ~1200-node graph costs more than the launch overhead it removes from ONE
+        # 50-step loop, so a graph is used only when the caller keeps it across loops (graph_cache), with the per-loop
+        # MMFS state refreshed in place (GraphedUNet.load).
         cuda_graph = graph_cache is not None and latents.is_cuda
     runner = None
     if cuda_graph and graph_cache is not None:

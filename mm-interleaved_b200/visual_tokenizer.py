@@ -1,4 +1,4 @@
-"""Visual tokenizer: CLIP ViT-L/14 + ViT-Adapter + Q-Former resampler, B200-native.
+"""Visual tokenizer: CLIP ViT-L/14 + ViT-Adapter + Q-Former resampler, H100-native.
 
 Mirrors the module tree / parameter names and the ``forward(image) -> {vis_embed, image_embeds,
 multiscale_features}`` contract of the reference's
@@ -10,8 +10,8 @@ multiscale_features}`` contract of the reference's
   decoders/perceiver.py:7-30 + utils/monkey_patch/blip2_qknorm_monkey_patch.py:37-152   Q-Former with qk LayerNorm
 so a reference checkpoint's ``visual_tokenizer.*`` keys load unchanged (HF naming for the CLIP encoder layers and
 the BLIP-2 Q-Former).  Arithmetic on the hot spots runs in this repo's kernels: all attention (CLIP patch self-
-attention T = 257, 16 x 64; Q-Former self / cross attention 12 x 64) through ``ops.attention`` (tcgen05 in bf16/f16),
-every MSDeformAttn through the sm_100a sampler (D = 32, P = 4, L in {3, 1}), LayerNorms through ``ops.layernorm``;
+attention T = 257, 16 x 64; Q-Former self / cross attention 12 x 64) through ``ops.attention`` (wgmma in bf16/f16),
+every MSDeformAttn through the sm_90a sampler (D = 32, P = 4, L in {3, 1}), LayerNorms through ``ops.layernorm``;
 dense linears / convolutions are library calls (cuBLAS / cuDNN).  The CLIP-encoder and Q-Former arithmetic of the
 reference lives in transformers 4.31 / xformers (not under /root/reference): parity for those blocks is checked
 against transformers 5.x stand-ins only ("parity unpinned", DESIGN.md section 2).

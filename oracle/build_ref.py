@@ -42,12 +42,12 @@ def main():
     assert n == 2, f"expected to patch 2 dispatch sites, found {n}"
     open(cu, "w").write(patched)
     vis = os.path.join(tmp, "src", "vision.cpp")
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     from torch.utils.cpp_extension import load
     srcs = [vis, os.path.join(tmp, "src", "cpu", "ms_deform_attn_cpu.cpp"), cu]
     load(name=NAME, sources=srcs, extra_include_paths=[os.path.join(tmp, "src")],
          extra_cflags=["-DWITH_CUDA", "-O2"],
-         extra_cuda_cflags=["-DWITH_CUDA", "-gencode", "arch=compute_100a,code=sm_100a", "-DCUDA_HAS_FP16=1",
+         extra_cuda_cflags=["-DWITH_CUDA", "-gencode", "arch=compute_90a,code=sm_90a", "-DCUDA_HAS_FP16=1",
                             "-D__CUDA_NO_HALF_OPERATORS__", "-D__CUDA_NO_HALF_CONVERSIONS__", "-D__CUDA_NO_HALF2_OPERATORS__"],
          build_directory=OUT, verbose="-v" in sys.argv, is_python_module=True)
     for f in glob.glob(os.path.join(OUT, "*")):

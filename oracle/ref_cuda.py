@@ -1,6 +1,6 @@
 """oracle/ref_cuda.py -- load the reference's own CUDA op (built by oracle/build_ref.py into oracle/_ref/).
 
-TEST INFRASTRUCTURE ONLY.  Gives the GPU tests and the sweep tool the REAL reference kernel on the B200:
+TEST INFRASTRUCTURE ONLY.  Gives the GPU tests and the sweep tool the REAL reference kernel on the H100:
 ``ms_deform_attn_forward(value, shapes, level_start_index, sampling_loc, attn_weight, im2col_step)`` exactly as
 ops/src/vision.cpp:13-16 exposes it (fp64 / fp32 / fp16; no bf16 dispatch, cu:65)."""
 from __future__ import annotations

@@ -12,6 +12,7 @@ are outputs of the reference's own code run here:
 """
 from __future__ import annotations
 
+import json
 import os
 import sys
 
@@ -162,7 +163,7 @@ LLAMA_TINY = dict(vocab_size=64, hidden_size=256, intermediate_size=512, num_hid
 def seeded_state_dict(template, seed):
     """Deterministic weights for any module with the reference's parameter names: iterate the names in sorted
     order with one CPU generator.  Used both here (loaded into the reference) and by the tests (loaded
-    into the B200 modules), so the multi-MB weights need not be stored in the fixtures."""
+    into the H100 modules), so the multi-MB weights need not be stored in the fixtures."""
     g = torch.Generator().manual_seed(seed)
     out = {}
     for name in sorted(template.keys()):
@@ -239,7 +240,7 @@ LLAMA_TC = dict(B=2, T=200, n_img=3, seed=123, left_pad=5)      # > 128 rows: tw
 
 def make_llama_tc(ref_ns):
     """The same tiny reference LlamaModel (head_dim 128) on a 200-token prompt: long enough that this repo's 16-bit run
-    takes the tcgen05 attention kernel (>= 16 query rows) in every layer, jointly with the fused MMFS sampler.  The
+    takes the wgmma attention kernel (>= 16 query rows) in every layer, jointly with the fused MMFS sampler.  The
     golden is the reference's fp32 output; the GPU test runs fp16 / bf16 against it (tests/test_llama_gpu.py)."""
     from transformers import LlamaConfig
     cfg = LlamaConfig(**{k: v for k, v in LLAMA_TINY.items() if k not in ("cross_attention_frequency", "spatial_shapes", "image_embed_dim")},
@@ -538,9 +539,60 @@ def make_tokenizer(full=False):
     print(f"{path}: {os.path.getsize(path) / 1024:.0f} KiB")
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# Outputs of three reference functions the CPU tests compare against: ms_deform_attn_core_pytorch (fp64 and fp32) on
+# three seeded location modes, one MMFS module (weights + output) and the 1-D sin-cos position table (a fixed sample of
+# the larger ones), plus the state-dict layouts of the reference LlamaModel and MMFSNet, so that those comparisons run
+# without the reference tree.
+SINCOS_CASES = ((16, 40), (5120, 7), (64, 2048))
+SINCOS_SAMPLE = 8192          # entries kept of a table larger than this
+
+
+def sincos_sample_index(numel):
+    return torch.randint(0, numel, (SINCOS_SAMPLE,), generator=torch.Generator().manual_seed(0)).sort().values
+
+
+def ref_llama_config():
+    """transformers ``LlamaConfig`` of LLAMA_TINY as the reference's LlamaModel takes it."""
+    from transformers import LlamaConfig
+    extra = ("cross_attention_frequency", "spatial_shapes", "image_embed_dim")
+    cfg = LlamaConfig(**{k: v for k, v in LLAMA_TINY.items() if k not in extra}, hidden_act="silu")
+    for k in extra:
+        setattr(cfg, k, LLAMA_TINY[k])
+    return cfg
+
+
+def make_reference_checks(ref):
+    from oracle import make_msda_inputs
+    out = {}
+    for seed, mode in enumerate(["uniform", "clustered", "edges"]):
+        v, s, st, loc, a = make_msda_inputs(2, [(12, 10), (6, 5), (3, 3)], 3, 16, 50, 5, seed=seed, loc_mode=mode)
+        out[f"msda_core_f64_{mode}"] = ref.func.ms_deform_attn_core_pytorch(v.double(), s, loc.double(), a.double()).numpy()
+        out[f"msda_core_f32_{mode}"] = ref.func.ms_deform_attn_core_pytorch(v, s, loc, a).numpy()
+    case = dict(MMFS_CASES["llm_tiny"], seed=77, N=2, Lq=5)
+    mod = mmfs_case_module(ref, case)
+    query, refpts, feat, ss, starts, mask = mmfs_case_inputs(case)
+    with torch.no_grad():
+        out["mmfs_out"] = mod(query, refpts, feat, ss, starts, None, mask).numpy()
+    for k, t in mod.state_dict().items():
+        out["mmfs_param/" + k] = t.numpy()
+    # state-dict layout ({name: shape}) of the reference LlamaModel and MMFSNet at the tiny configurations
+    layouts = {"llama": ref.llama.LlamaModel(ref_llama_config()).state_dict(), "mmfsnet": ref.sd_mmfs.MMFSNet(**MMFSNET_TINY).state_dict()}
+    for name, sd in layouts.items():
+        out[f"layout_{name}"] = np.array(json.dumps({k: list(v.shape) for k, v in sd.items()}, sort_keys=True))
+    for dim, n in SINCOS_CASES:
+        t = ref.pos_embed.get_1d_sincos_pos_embed_from_grid(dim, np.arange(n, dtype=np.float32))
+        if t.size > SINCOS_SAMPLE:
+            t = t.reshape(-1)[sincos_sample_index(t.size).numpy()]
+        out[f"sincos_{dim}_{n}"] = t
+    path = os.path.join(HERE, "reference_checks.npz")
+    np.savez_compressed(path, **out)
+    print(f"{path}: {os.path.getsize(path) / 1024:.0f} KiB")
+
+
 if __name__ == "__main__":
     torch.manual_seed(0)
-    which = sys.argv[1:] or ["msda", "mmfs", "llama", "mmfsnet", "adapter", "imgdec", "tokenizer"]
+    which = sys.argv[1:] or ["msda", "mmfs", "llama", "mmfsnet", "adapter", "imgdec", "tokenizer", "reference_checks"]
     if "tokenizer" in which:
         make_tokenizer()
     if "tokenizer_full" in which:
@@ -558,3 +610,5 @@ if __name__ == "__main__":
         main()
     if "mmfs" in which:
         make_mmfs(ref_loader.load())
+    if "reference_checks" in which:
+        make_reference_checks(ref_loader.load())

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 attention kernel against an fp32 PyTorch statement of
+"""GPU parity of the wgmma attention kernel against an fp32 PyTorch statement of
 softmax(q k^T / sqrt(d) + mask) v on the same bf16/f16-rounded inputs.
 
 Tolerance, elementwise: P is rounded to the 16-bit type before the second MMA (as in the reference, where
@@ -43,7 +43,7 @@ CASES = [
     (2, 2, 640, 640, 128, True, 0, True),       # five query tiles, padding mask
     (1, 3, 1000, 1000, 64, False, 0, False),    # ragged tails of the last query tile and of the key tiles
     (1, 2, 384, 900, 128, True, 516, True),     # chunked prefill on a cache
-    (3, 40, 640, 640, 128, True, 0, True),      # 600 items > 296 resident CTAs: the persistent work-list kernel, masks
+    (3, 40, 640, 640, 128, True, 0, True),      # 600 items > resident CTAs (1 per SM at hd 128): persistent kernel, masks
     (2, 24, 1000, 1000, 64, False, 0, False),   # persistent, hd 64, ragged tails
     (40, 10, 130, 130, 128, True, 0, False),    # persistent, two-tile items incl. a 2-row query tile
 ]

@@ -1,4 +1,4 @@
-"""GPU parity of the implicit-GEMM tcgen05 convolution against F.conv2d in fp32 on the same bf16-rounded operands.
+"""GPU parity of the implicit-GEMM wgmma convolution against F.conv2d in fp32 on the same bf16-rounded operands.
 Tolerance: |err| <= 2e-2 * max|ref| (bf16 output rounding + fp32 accumulation order), mean |err| <= 2e-3 * max|ref|."""
 import pytest
 import torch

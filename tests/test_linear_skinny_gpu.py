@@ -9,7 +9,7 @@ DEV = "cuda"
 CASES = [
     # M, N, K, prologue, residual
     (4, 15360, 5120, 1, False),     # q/k/v of the 13 B decoder with the input RMSNorm folded in
-    (4, 5120, 5120, 0, True),       # o_proj + residual (blocks cut by range boundaries: 320 blocks on 148 SMs)
+    (4, 5120, 5120, 0, True),       # o_proj + residual (blocks cut by range boundaries: 320 blocks on 132 SMs)
     (4, 27648, 5120, 1, False),     # gate | up with the post-attention RMSNorm
     (4, 5120, 13824, 2, True),      # down_proj of silu(gate) * up, + residual
     (1, 4736, 512, 0, False),       # one step per block

@@ -1,4 +1,4 @@
-"""GPU parity of the B200 Llama-MMFS decoder and its kernels.
+"""GPU parity of the H100 Llama-MMFS decoder and its kernels.
 
 Tolerances: fp32 model output vs the reference's fp32 golden: |err| <= 1e-3*|ref| + 2e-5 at non-padding
 positions (north-star 1e-3 rel; fully masked = padding query rows are unspecified, DESIGN.md);
@@ -171,12 +171,11 @@ def test_model_bf16_tracks_fp32_reference():
                                                    (torch.float32, 1.0e-5, 1.0e-5)])
 def test_long_prompt_takes_the_tcgen05_kernel_and_tracks_the_reference_golden(dtype, max_tol, rms_tol):
     """A 200-token left-padded prompt through the tiny decoder in 16 bit: every layer's self-attention goes through the
-    tcgen05 kernel (two query tiles, four key tiles, padding mask, causal diagonal) and every second layer through the
+    wgmma kernel (two query tiles, four key tiles, padding mask, causal diagonal) and every second layer through the
     fused MMFS sampler -- jointly against the fp32 output of the REFERENCE LlamaModel on the same weights and inputs
     (tests/golden/llama_tc.npz, generated by make_golden.make_llama_tc from the reference's own modeling file).
-    Tolerances are for 16-bit storage through 3 layers: max error relative to max |ref|, and relative RMS error (measured
-    on a B200: fp16 1.5e-3 / 1.2e-3, bf16 1.1e-2 / 9.6e-3).  fp32 takes the bandwidth kernel (the tensor-core kernel is
-    16-bit only) and must match to 1e-5 (measured 7e-7)."""
+    Tolerances are for 16-bit storage through 3 layers: max error relative to max |ref|, and relative RMS error.  fp32
+    takes the bandwidth kernel (the tensor-core kernel is 16-bit only) and must match to 1e-5."""
     import os
 
     import numpy as np
@@ -224,7 +223,7 @@ def test_full_width_layers_match_the_oracle(dtype, max_tol, rms_tol):
     over 32^2 + 16^2 + 8^2 feature maps of 3 images, seeded weights): one MMFS layer + one plain layer on a 160-token
     left-padded prompt against the oracle restatement of the reference layers (oracle/llama.py, pinned by the tiny
     goldens) on the host.  fp32 takes the bandwidth attention kernel and the generic sampler's fp32 path; bf16 the
-    tcgen05 kernel and the specialised 16-bit sampler -- the kernels and shapes of the benchmarked step."""
+    wgmma kernel and the specialised 16-bit sampler -- the kernels and shapes of the benchmarked step."""
     from oracle.llama import llama_model_ref
     from mm_interleaved_b200.llama_mmfs import LlamaMMFSConfig, LlamaModel
     model = LlamaModel(LlamaMMFSConfig(**FULL_WIDTH))

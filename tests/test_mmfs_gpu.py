@@ -1,4 +1,4 @@
-"""GPU parity of the B200 ``MMFS`` module (fused sampler kernel) against the committed outputs of
+"""GPU parity of the H100 ``MMFS`` module (fused sampler kernel) against the committed outputs of
 the reference module (tests/golden/mmfs_*.npz) and against the CPU oracle's intermediates.
 
 Tolerances:

@@ -1,5 +1,5 @@
 """MMFSNet (SD-UNet conditioning branch, decoders/sd_mmfs.py:154-272): CPU oracle pinned to the committed reference
-outputs, and the B200 module against the same golden on the GPU (fp32: |err| <= 1e-3*|ref| + 1e-5*max|ref|)."""
+outputs, and the H100 module against the same golden on the GPU (fp32: |err| <= 1e-3*|ref| + 1e-5*max|ref|)."""
 import os
 
 import numpy as np

@@ -1,5 +1,5 @@
 """GPU parity of the MSDA backward against (a) autograd through the CPU restatement of the reference's PyTorch core
-in fp64 and (b) the reference's OWN CUDA backward (oracle/_ref) on the same B200.
+in fp64 and (b) the reference's OWN CUDA backward (oracle/_ref) on the same H100.
 Tolerance fp32: |err| <= 1e-4 * max|ref| per tensor (atomics: summation order differs); 16-bit: 2e-2 * max|ref|."""
 import pytest
 import torch

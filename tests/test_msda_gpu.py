@@ -275,8 +275,8 @@ def _ref_op():
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16, torch.float64])
 @pytest.mark.parametrize("case", [0, 1, 2, 3, 5])
 def test_against_the_reference_cuda_op(case, dtype):
-    """The reference's OWN kernel (ops/src/cuda/ms_deform_im2col_cuda.cuh, compiled unmodified for sm_100a by
-    oracle/build_ref.py) run on the same B200 on the same inputs."""
+    """The reference's OWN kernel (ops/src/cuda/ms_deform_im2col_cuda.cuh, compiled unmodified for sm_90a by
+    oracle/build_ref.py) run on the same H100 on the same inputs."""
     ref = _ref_op()
     m = _mod()
     N, shapes, M, D, Lq, P = CASES[case]

@@ -1,83 +1,117 @@
-"""The reference's ``replace_*()`` start-up mechanism (inference.py:10-24) pointed at the B200 classes: after
-``replace_*_b200()`` the REFERENCE's own ``LlamaModel`` / ``LlamaMMFSAttention`` / ``MMFSNet`` constructors build B200
-modules, and a state dict saved from the unpatched reference loads into them with ``strict=True``.  CPU-only
-(construction + state-dict load; compute needs the GPU).  Skipped where /root/reference is absent (the GPU box)."""
+"""The reference's ``replace_*()`` start-up mechanism (inference.py:10-24) pointed at this repository's classes.
+``replace_*_b200()`` finds the reference modules by name in ``sys.modules``, so stand-in modules registered under the
+reference's module names exercise every rebinding and ``restore_reference()``.  Checkpoint compatibility: the
+substituted modules, and the top-level ``MMInterleaved``, have exactly the reference's state-dict layout (names and
+shapes), so a checkpoint saved from the reference loads with ``strict=True``; the reference layouts (``LlamaModel`` and
+``MMFSNet`` at the tiny test configurations) are stored in tests/golden/reference_checks.npz by
+tests/golden/make_golden.py.  CPU-only (construction + state-dict load; compute needs the GPU)."""
+import json
+import os
 import sys
+import types
 
+import numpy as np
 import pytest
 import torch
 
-from oracle import ref_loader
-
-pytestmark = pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present (GPU box)")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_checks.npz")
 
 
-def _ref_llama_config():
-    from transformers import LlamaConfig
-    from tests.golden.make_golden import LLAMA_TINY
-    extra = ("cross_attention_frequency", "spatial_shapes", "image_embed_dim")
-    cfg = LlamaConfig(**{k: v for k, v in LLAMA_TINY.items() if k not in extra}, hidden_act="silu")
-    for k in extra:
-        setattr(cfg, k, LLAMA_TINY[k])
-    return cfg
+def _ref_layout(name):
+    return {k: tuple(v) for k, v in json.loads(str(np.load(GOLDEN)[f"layout_{name}"])).items()}
 
 
-def test_replace_functions_rebind_the_reference_and_checkpoints_load():
+def _zeros(layout):
+    return {k: torch.zeros(v) for k, v in layout.items()}
+
+
+def _stub_reference(monkeypatch):
+    """Stand-ins for the reference modules patch.py rebinds, registered under the reference's module names: each
+    defines the reference's class names, ``sd_mmfs`` / ``ops.modules`` hold second bindings of ``MMFS`` the way
+    ``from ..x import MMFS`` creates them, and ``modeling_llama_mmfs.build_layer`` is reference-style glue that looks
+    the layer class up in its module at call time."""
+    def mod(name, **attrs):
+        m = types.ModuleType(name)
+        for k, v in attrs.items():
+            setattr(m, k, v)
+        monkeypatch.setitem(sys.modules, name, m)
+        return m
+
+    cls = {n: type(n, (), {}) for n in ("MMFS", "LlamaRMSNorm", "LlamaMLP", "LlamaAttention", "LlamaMMFSAttention",
+                                         "LlamaDecoderLayer", "MMFSNet", "MMFSBlock", "VisualTokenizer",
+                                         "PerceiverResampler")}
+    ns = types.SimpleNamespace(cls=cls, ext=types.ModuleType("MultiScaleDeformableAttention"))   # the compiled op
+    mod("mm_interleaved")
+    ns.msda_func = mod("mm_interleaved.models.utils.ops.functions.ms_deform_attn_func", MSDA=ns.ext)
+    ns.msda_func_vit = mod("mm_interleaved.models.encoders.vit_adapter.ops.functions.ms_deform_attn_func", MSDA=ns.ext)
+    ns.mmfs = mod("mm_interleaved.models.utils.ops.modules.mmfs", MMFS=cls["MMFS"])
+    ns.ops_modules = mod("mm_interleaved.models.utils.ops.modules", MMFS=cls["MMFS"])
+    ns.llama = mod("mm_interleaved.models.decoders.modeling_llama_mmfs",
+                   **{n: cls[n] for n in ("LlamaRMSNorm", "LlamaMLP", "LlamaAttention", "LlamaMMFSAttention",
+                                          "LlamaDecoderLayer")})
+    exec("def build_layer():\n    return LlamaDecoderLayer", vars(ns.llama))
+    ns.sd_mmfs = mod("mm_interleaved.models.decoders.sd_mmfs", MMFS=cls["MMFS"], MMFSNet=cls["MMFSNet"],
+                     MMFSBlock=cls["MMFSBlock"])
+    ns.tokenizer = mod("mm_interleaved.models.encoders.visual_tokenizer", VisualTokenizer=cls["VisualTokenizer"])
+    ns.perceiver = mod("mm_interleaved.models.decoders.perceiver", PerceiverResampler=cls["PerceiverResampler"])
+    monkeypatch.delitem(sys.modules, "MultiScaleDeformableAttention", raising=False)
+    return ns
+
+
+def test_replace_functions_rebind_the_reference_and_checkpoints_load(monkeypatch):
+    """``replace_*_b200()`` rebinds every reference binding of the substituted classes (including second bindings and
+    the ``MultiScaleDeformableAttention`` extension module), reference glue then builds this repository's classes,
+    ``restore_reference()`` undoes all of it, and reference checkpoints load into the substituted modules with
+    ``strict=True``."""
     import mm_interleaved_b200 as b200
     from mm_interleaved_b200 import patch
-    ns = ref_loader.load()
-    if ns.llama is None or ns.sd_mmfs is None:
-        pytest.skip("reference decoders do not import in this environment")
-    ref_mmfs_cls, ref_layer_cls, ref_net_cls = ns.mmfs.MMFS, ns.llama.LlamaDecoderLayer, ns.sd_mmfs.MMFSNet
-    cfg = _ref_llama_config()
-    ref_sd = ns.llama.LlamaModel(cfg).state_dict()                       # unpatched reference: the checkpoint layout
-    from tests.golden.make_golden import MMFSNET_TINY
-    ref_net_sd = ref_net_cls(**MMFSNET_TINY).state_dict()
+    from tests.golden.make_golden import LLAMA_TINY, MMFSNET_TINY
+    ns = _stub_reference(monkeypatch)
+    c = ns.cls
     try:
         b200.replace_mmfs_b200()
-        assert ns.mmfs.MMFS is b200.MMFS and ns.sd_mmfs.MMFS is b200.MMFS   # (the llama file imports it lazily, :325)
-        assert sys.modules["mm_interleaved.models.utils.ops.modules"].MMFS is b200.MMFS
-        assert sys.modules["MultiScaleDeformableAttention"].ms_deform_attn_forward is b200.ms_deform_attn_forward
-        assert ns.func.MSDA is sys.modules["MultiScaleDeformableAttention"]
-        # reference LlamaMMFSAttention (still the reference class) now builds the B200 MMFS inside
-        xattn = ns.llama.LlamaMMFSAttention(cfg, layer_idx=0)
-        assert type(xattn.attn) is b200.MMFS and type(xattn).__module__.startswith("mm_interleaved.")
-        xattn.load_state_dict({k[len("layers.0.llama_cross_attn."):]: v for k, v in ref_sd.items()
-                               if k.startswith("layers.0.llama_cross_attn.")}, strict=True)
+        assert ns.mmfs.MMFS is b200.MMFS and ns.sd_mmfs.MMFS is b200.MMFS and ns.ops_modules.MMFS is b200.MMFS
+        ext = sys.modules["MultiScaleDeformableAttention"]
+        assert ext.ms_deform_attn_forward is b200.ms_deform_attn_forward
+        assert ns.msda_func.MSDA is ext and ns.msda_func_vit.MSDA is ext
 
         b200.replace_llama_b200()
         for name in ("LlamaRMSNorm", "LlamaMLP", "LlamaAttention", "LlamaMMFSAttention", "LlamaDecoderLayer"):
             assert getattr(ns.llama, name) is getattr(b200, name)
-        model = ns.llama.LlamaModel(cfg)                                  # the reference's own LlamaModel glue
-        assert type(model).__module__.startswith("mm_interleaved.")
-        assert all(type(l) is b200.LlamaDecoderLayer for l in model.layers)
-        assert type(model.layers[0].llama_cross_attn.attn) is b200.MMFS and type(model.norm) is b200.LlamaRMSNorm
-        missing, unexpected = model.load_state_dict(ref_sd, strict=True)
-        assert not missing and not unexpected
-        assert set(model.state_dict().keys()) == set(ref_sd.keys())
+        assert ns.llama.build_layer() is b200.LlamaDecoderLayer      # the reference's glue now builds this repo's layer
 
         b200.replace_visual_b200()
         assert ns.sd_mmfs.MMFSNet is b200.MMFSNet and ns.sd_mmfs.MMFSBlock is b200.MMFSBlock
-        net = ns.sd_mmfs.MMFSNet(**MMFSNET_TINY)
-        net.load_state_dict(ref_net_sd, strict=True)
+        assert ns.tokenizer.VisualTokenizer is b200.visual_tokenizer.VisualTokenizer
+        assert ns.perceiver.PerceiverResampler is b200.visual_tokenizer.PerceiverResampler
 
         b200.replace_all_b200()                                           # idempotent
-        assert ns.llama.LlamaDecoderLayer is b200.LlamaDecoderLayer
+        assert ns.llama.LlamaDecoderLayer is b200.LlamaDecoderLayer and ns.mmfs.MMFS is b200.MMFS
     finally:
         patch.restore_reference()
-    assert ns.mmfs.MMFS is ref_mmfs_cls and ns.sd_mmfs.MMFS is ref_mmfs_cls and ns.llama.LlamaDecoderLayer is ref_layer_cls
-    assert ns.sd_mmfs.MMFSNet is ref_net_cls
+    assert ns.mmfs.MMFS is c["MMFS"] and ns.sd_mmfs.MMFS is c["MMFS"] and ns.ops_modules.MMFS is c["MMFS"]
+    assert ns.llama.LlamaDecoderLayer is c["LlamaDecoderLayer"] and ns.llama.build_layer() is c["LlamaDecoderLayer"]
+    assert ns.sd_mmfs.MMFSNet is c["MMFSNet"] and ns.tokenizer.VisualTokenizer is c["VisualTokenizer"]
+    assert ns.msda_func.MSDA is ns.ext and ns.msda_func_vit.MSDA is ns.ext
+    assert "MultiScaleDeformableAttention" not in sys.modules
+
+    # checkpoints: the substituted modules have exactly the reference's state-dict layout
+    ref_llama, ref_net = _ref_layout("llama"), _ref_layout("mmfsnet")
+    model = b200.LlamaModel(b200.LlamaMMFSConfig(**LLAMA_TINY))
+    assert {k: tuple(v.shape) for k, v in model.state_dict().items()} == ref_llama
+    missing, unexpected = model.load_state_dict(_zeros(ref_llama), strict=True)
+    assert not missing and not unexpected
+    net = b200.MMFSNet(**MMFSNET_TINY)
+    assert {k: tuple(v.shape) for k, v in net.state_dict().items()} == ref_net
+    net.load_state_dict(_zeros(ref_net), strict=True)
 
 
 def test_b200_top_level_model_keeps_the_reference_state_dict_layout():
-    """``MMInterleaved`` (B200) exposes the reference's parameter names for the parts whose reference classes import
+    """``MMInterleaved`` (H100) exposes the reference's parameter names for the parts whose reference classes import
     here (decoder + text head + glue): every key of the reference ``LlamaModel`` / ``TextDecoder`` layout exists."""
     import mm_interleaved_b200 as b200
     from tests.golden.make_golden import LLAMA_TINY
-    ns = ref_loader.load()
-    if ns.llama is None:
-        pytest.skip("reference decoder does not import")
-    ref_keys = {"mm_decoder." + k for k in ns.llama.LlamaModel(_ref_llama_config()).state_dict().keys()}
+    ref_keys = {"mm_decoder." + k for k in _ref_layout("llama")}
     tiny_vt = dict(clip_config=b200.visual_tokenizer.CLIPVisionConfigLite(hidden_size=64, intermediate_size=128,
                                                                         num_hidden_layers=4, num_attention_heads=4,
                                                                         image_size=32, patch_size=8),

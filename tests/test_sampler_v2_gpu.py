@@ -4,7 +4,7 @@ Oracle = the scalar C restatement of the reference kernel (oracle/msda_ref.c, cu
 locations / attention weights the EMIT kernel materialises from the same inputs (those are pinned to the reference
 module's intermediates in tests/test_mmfs_gpu.py).  Bars:
   * fp32 tap weights (``exact_weights``): |out - oracle_fp32_accumulator| <= one storage ulp of it;
-  * default (tap weights rounded to the element type, FHFMA): <= one storage ulp + eps_T * sum_k |w_k v_k| with
+  * default (tap weights rounded to the element type, mixed-precision FMA): <= one storage ulp + eps_T * sum_k |w_k v_k| with
     eps_T = 2^-8 (bf16) / 2^-11 (f16), the unit roundoff -- the bound derived in the kernel's header, evaluated with the
     oracle on |value|;
   * specialised vs generic kernel on the full cfg-3 layer shape: <= 2 storage ulps (+ the weight-rounding term in the

@@ -74,7 +74,7 @@ def test_sd21_configuration_shapes_and_bf16_denoise_step():
 
 
 def test_conv_kernel_path_matches_library_path_bf16():
-    """Same bf16 weights, tcgen05 implicit-GEMM convolutions (fused temb / residual epilogues) vs the cuDNN path:
+    """Same bf16 weights, wgmma implicit-GEMM convolutions (fused temb / residual epilogues) vs the cuDNN path:
     |err| <= 3e-2 * max|ref| (bf16 rounding points differ: the fused epilogue rounds once instead of three times)."""
     from mm_interleaved_b200 import ops, unet_sd
     torch.manual_seed(0)

@@ -103,8 +103,8 @@ def test_tiny_unet_with_mmfs_hook_matches_independent_oracle(use_kernels):
 @pytest.mark.gpu
 def test_full_width_blocks_bf16_kernels_vs_oracle():
     """One SD-2.1-width ResNet block (320 -> 640 at 32x32, with the 1x1 shortcut and the time-embedding add) and one
-    transformer block (5 heads x 64, 1024-wide context, T = 1024) on this repo's bf16 kernels (tcgen05 implicit-GEMM
-    convolution, NHWC GroupNorm+SiLU, tcgen05 attention, LayerNorm, GEGLU) vs the fp32 oracle on the same weights."""
+    transformer block (5 heads x 64, 1024-wide context, T = 1024) on this repo's bf16 kernels (wgmma implicit-GEMM
+    convolution, NHWC GroupNorm+SiLU, wgmma attention, LayerNorm, GEGLU) vs the fp32 oracle on the same weights."""
     from mm_interleaved_b200 import unet_sd
     torch.manual_seed(3)
     res = unet_sd.ResnetBlock2D(320, 640, 1280).eval()

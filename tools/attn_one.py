@@ -1,4 +1,4 @@
-"""Run the tcgen05 attention kernel on one BASELINE shape (ncu target) and print CUDA-event timings."""
+"""Run the wgmma attention kernel on one BASELINE shape (ncu target) and print CUDA-event timings."""
 import os
 import sys
 

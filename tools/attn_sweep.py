@@ -1,5 +1,6 @@
-"""Per-CTA fixed cost vs per-tile cost of the tcgen05 attention kernel: time non-causal and causal problems of different
-lengths with the number of CTAs held near 2560 (8.6 waves of 296 slots) and fit  t_cta = c0 + n_tiles * t_tile."""
+"""Per-CTA fixed cost vs per-tile cost of the wgmma attention kernel: time non-causal and causal problems of different
+lengths with the number of work items held near 2560 and fit  t_cta = c0 + n_tiles * t_tile, where the CTA slots are the
+resident CTAs of the hd-128 kernel (one per SM)."""
 import os
 import sys
 
@@ -11,6 +12,7 @@ from mm_interleaved_b200 import ops  # noqa: E402
 
 g = torch.Generator(device="cuda").manual_seed(0)
 hd = 128
+slots = torch.cuda.get_device_properties(0).multi_processor_count   # 1 resident CTA per SM at hd 128
 rows = []
 for causal in (False, True):
     for T in (256, 512, 1024, 2048, 4096):
@@ -34,4 +36,4 @@ for causal in (False, True):
         flops = 4.0 * B * H * T * T * hd * (0.5 if causal else 1.0)
         rows.append((causal, T, n_cta, tiles, t))
         print(f"causal={int(causal)} T={T:5d} B={B:3d} H={H:3d} ctas={n_cta:5d} key-tiles={tiles:7d}: {t:8.1f} us  {flops / t / 1e6:7.1f} TFLOP/s  "
-              f"{t * 296 / n_cta:6.2f} us per CTA slot-time, {t * 296 / tiles:6.3f} us per tile")
+              f"{t * slots / n_cta:6.2f} us per CTA slot-time, {t * slots / tiles:6.3f} us per tile")

@@ -1,7 +1,7 @@
 """Greedy decode timing of the Llama-13B MMFS decoder (random weights, bf16): prefill on B x 2048-token 4-image
 sequences, then N new tokens with (a) the eager loop over the pre-allocated in-place KV cache, (b) the CUDA-graphed
 decode step (InterleavedForward.enable_decode_graphs) and (c) the reference-style cat-per-token cache.
-Weight-read floor per token: 13.0 B parameters x 2 B / measured HBM GB/s.  Prints one JSON object (-> profiles/)."""
+Weight-read floor per token: 13.0 B parameters x 2 B / peak HBM GB/s (workloads.measured_peaks).  Prints one JSON object."""
 import json
 import os
 import sys

@@ -1,6 +1,6 @@
-"""A/B for the Llama dense linears (VERDICT r01 item 5): this repo's tcgen05 implicit-GEMM mainloop at KH = KW = 1 (which IS a
-plain GEMM: M = 128-pixel tiles, N = 160, K = 64 per stage, cta_group::1, 2 CTAs/SM) against cuBLAS (torch F.linear) on
-the decoder's shapes, same box, CUDA events, median of `reps`.  Prints one JSON object (-> profiles/)."""
+"""A/B for the Llama dense linears: this repo's wgmma implicit-GEMM mainloop at KH = KW = 1 (which IS a plain GEMM:
+M = 128-pixel tiles, N = 160, K = 64 per stage, one CTA per SM) against cuBLAS (torch F.linear) on the decoder's shapes,
+same GPU, CUDA events, median of `reps`.  Prints one JSON object."""
 import json
 import os
 import sys

@@ -1,5 +1,5 @@
-"""Time the reference's own CUDA op (oracle/_ref, compiled unmodified for sm_100a) against this repo's kernel on the
-same B200, same inputs (fp16 and fp32 -- the reference has no bf16 dispatch).  CUDA events, L2 flushed."""
+"""Time the reference's own CUDA op (oracle/_ref, compiled unmodified for sm_90a) against this repo's kernel on the
+same H100, same inputs (fp16 and fp32 -- the reference has no bf16 dispatch).  CUDA events, L2 flushed."""
 import json
 import os
 import sys

@@ -1,6 +1,6 @@
 """Fused MMFS sampler on the cfg-3 layer shape (B = 4 sequences, 2048 tokens, 4 images): generic kernel vs the
 specialised kernel (fp32 / 16-bit tap weights) over rows-per-warp settings; CUDA events, L2 flushed between runs,
-median of `reps`.  Prints one line per setting and a final JSON list (-> profiles/)."""
+median of `reps`.  Prints one line per setting and a final JSON list."""
 import json
 import os
 import sys

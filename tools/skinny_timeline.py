@@ -21,9 +21,10 @@ with torch.no_grad():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(); ops.linear_skinny(x, ws[i % 4]); e1.record()
         torch.cuda.synchronize()
-buf = (ctypes.c_ulonglong * (4 * 148))()
-assert lib.mmfs_linear_skinny_probe(buf, 148) == 0
-t = torch.tensor(list(buf), dtype=torch.float64).view(148, 4)
+n_cta = torch.cuda.get_device_properties(0).multi_processor_count   # the kernel runs one CTA per SM
+buf = (ctypes.c_ulonglong * (4 * n_cta))()
+assert lib.mmfs_linear_skinny_probe(buf, n_cta) == 0
+t = torch.tensor(list(buf), dtype=torch.float64).view(n_cta, 4)
 t0 = t[:, 0].min()
 t = (t - t0) / 1e3
 print(f"N={N} K={K} ({N * K * 2 / 1e6:.0f} MB), event time of the last call {e0.elapsed_time(e1) * 1e3:.1f} us")
