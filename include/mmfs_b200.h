@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define MMFS_B200_ABI_VERSION 1
+#define MMFS_B200_ABI_VERSION 2
 
 /* status codes */
 #define MMFS_OK            0
@@ -40,14 +40,12 @@ extern "C" {
 #define MMFS_MSDA_STRICT 1u /* also fetch taps whose attention weight is exactly 0 (the
                                reference multiplies them in, which only matters when
                                `value` holds inf/nan); default skips those fetches */
-#define MMFS_MSDA_W16    2u /* 16-bit element types only: round each tap weight (lerp * attention weight) to the
-                               element type and accumulate value x weight with one fp32 FMA of the widened 16-bit
-                               operands -- fewer instructions per fetch; the reference keeps fp32 weights, so
-                               this is opt-in (error << one storage ulp of the result) */
 
 /* flags for mmfs_sampler_forward (in addition to MMFS_MSDA_STRICT) */
-#define MMFS_SAMPLER_EXACT_WEIGHTS 4u /* keep fp32 tap weights in the specialised 16-bit kernel (default there: weights
-                                         rounded to the element type, mixed-precision FMA accumulate; bound in mmfs_sampler_v2_sm100.cu) */
+#define MMFS_SAMPLER_EXACT_WEIGHTS 4u /* keep fp32 tap weights in the specialised 16-bit kernel for this call (without
+                                         it that kernel rounds each tap weight to the element type and accumulates with
+                                         a mixed-precision FMA; error bound in mmfs_sampler_v2_sm100.cu).  Bit 2u is
+                                         unused. */
 #define MMFS_SAMPLER_GENERIC       8u /* force the generic kernel (A/B runs, tests) */
 
 int mmfs_abi_version(void);
@@ -129,13 +127,6 @@ int mmfs_msda_forward_host(const void *value, const int64_t *spatial_shapes, con
                            int dtype, unsigned flags, void *stream);
 void mmfs_release_scratch(void);
 
-/* Tuning knobs (benchmarks / tests only): rows per warp per tile (0 = automatic); mapping bit 0 =
- * plain tile order instead of the per-SM swizzle. */
-int mmfs_msda_set_tuning(int rows_per_warp, int mapping);
-/* Same for the specialised fused sampler: rows per warp per tile (0 = automatic); wmode 1 = 16-bit tap weights +
- * mixed-precision FMA (default), 0 = fp32 tap weights everywhere. */
-int mmfs_sampler_set_tuning(int rows_per_warp, int wmode);
-
 /*
  * Fused MMFS sampler: relpos-conditioned offsets / logits, image mask, null-slot softmax, sampling
  * locations and the deformable gather in one kernel.
@@ -205,24 +196,6 @@ int mmfs_swiglu(const void *gate_up, void *out, long rows, int inter, int dtype,
  * GELU), on one (rows, 2*inter) buffer holding [value | gate]. */
 int mmfs_geglu(const void *value_gate, void *out, long rows, int inter, int dtype, void *stream);
 
-/* Decode-step linear: y[M, N] = prologue(x)[M, K] . w[N, K]^T (+ residual[M, N]) for M <= 8 rows, f16 / bf16 -- the
- * q/k/v, o_proj, gate/up and down projections of one generated token (LlamaAttention.forward
- * decoders/modeling_llama_mmfs.py:217-280, LlamaMLP.forward :188-189) with the operator in front of them folded in:
- *   prologue 0: x as given;  1: LlamaRMSNorm(x) * norm_weight (:53-70, eps);  2: x is [M, 2K] = [gate | up] and the
- *   operand is act_fn(gate) * up (:188-189).
- * residual (may be NULL, may alias y) is added in fp32 before the single rounding of the result.  w rows are streamed
- * from HBM exactly once (HBM roofline: N * K * sizeof(T) bytes).  N % 32 == 0, K % 512 == 0, all pointers 16-byte aligned,
- * contiguous rows.  scratch: mmfs_linear_skinny_scratch_floats(N) floats that must be ZERO before the first call; every
- * call leaves them zero again (arrival tickets of the split between SMs + fp32 partial tiles), so one zeroed buffer of
- * the largest N serves every call made on one stream.  MMFS_EUNSUPPORTED for shapes outside these limits. */
-long mmfs_linear_skinny_scratch_floats(int N);
-/* measurement hooks: mode 0 = default (tensor-map TMA kernel when N % 128 == 0), 1 = per-lane cp.async kernel, 2 = TMA
- * kernel, + 4 = record per-CTA {entry, first stage, last stage, exit} globaltimer stamps, read back by ..._probe */
-int mmfs_linear_skinny_set_tuning(int mode);
-int mmfs_linear_skinny_probe(unsigned long long *host_out, int n_ctas);
-int mmfs_linear_skinny(const void *x, const void *w, void *y, const void *residual, const void *norm_weight, float *scratch,
-                       int M, int N, int K, int prologue, float eps, int dtype, void *stream);
-
 /*
  * softmax(q k^T * scale + mask) v for decode (q_len = 1 over a KV cache) and small / odd shapes;
  * the tensor-core path for prefill shapes is mmfs_attn_forward.
@@ -240,8 +213,6 @@ int mmfs_attn_generic(const void *q, const void *k, const void *v, void *out, co
  * private to the call until it completes (per-(b, h) arrival tickets, zeroed by the call itself on `stream`, + partials).
  * causal != 0: the query sits at position `past` and sees keys 0..past.  f32 / f16 / bf16, hd % 32 == 0, hd <= 256. */
 long mmfs_attn_decode_scratch_floats(int B, int H, int Tkv, int hd);
-/* measurement hook: warps per 256-key CTA of the hd-128 16-bit decode kernel: 4 (64 keys per warp, default) or 8 (32) */
-int mmfs_attn_decode_set_tuning(int warps);
 int mmfs_attn_decode(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask, float *scratch,
                      int B, int H, int Tkv, int hd, long q_bs, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs,
                      float scale, int causal, int past, int dtype, void *stream);

@@ -14,7 +14,6 @@ LIB_PATH = os.environ.get("MMFS_B200_LIB", os.path.join(_HERE, "libmmfs_b200.so"
 OK, EINVAL, EUNSUPPORTED, ECUDA = 0, -1, -2, -3
 F32, F16, BF16, F64 = 0, 1, 2, 3
 MSDA_STRICT = 1
-MSDA_W16 = 2
 SAMPLER_EXACT_WEIGHTS = 4
 SAMPLER_GENERIC = 8
 
@@ -33,8 +32,6 @@ SIGNATURES = {
     "mmfs_msda_index_stream": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "mmfs_msda_forward_host": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _U, _P]),
     "mmfs_release_scratch": (None, []),
-    "mmfs_msda_set_tuning": (_I, [_I, _I]),
-    "mmfs_sampler_set_tuning": (_I, [_I, _I]),
     "mmfs_sampler_forward": (_I, [_P] * 10 + [_I] * 13 + [_U, _P]),
     "mmfs_sampler_locw": (_I, [_P] * 10 + [_I] * 11 + [_P]),
     "mmfs_rmsnorm": (_I, [_P, _P, _P, _L, _I, _F, _I, _P]),
@@ -43,15 +40,10 @@ SIGNATURES = {
     "mmfs_rope_qk_append": (_I, [_P] * 9 + [_L, _L] + [_I] * 6 + [_L, _L, _I, _I, _P]),
     "mmfs_swiglu": (_I, [_P, _P, _L, _I, _I, _P]),
     "mmfs_geglu": (_I, [_P, _P, _L, _I, _I, _P]),
-    "mmfs_linear_skinny_scratch_floats": (_L, [_I]),
-    "mmfs_linear_skinny_set_tuning": (_I, [_I]),
-    "mmfs_linear_skinny_probe": (_I, [_P, _I]),
-    "mmfs_linear_skinny": (_I, [_P] * 6 + [_I] * 4 + [_F, _I, _P]),
     "mmfs_attn_generic": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P]),
     "mmfs_groupnorm_nhwc": (_I, [_P] * 5 + [_I] * 4 + [_F, _I, _I, _P]),
     "mmfs_conv2d_nhwc": (_I, [_P] * 6 + [_I] * 10 + [_P]),
     "mmfs_attn_decode_scratch_floats": (_L, [_I] * 4),
-    "mmfs_attn_decode_set_tuning": (_I, [_I]),
     "mmfs_attn_decode": (_I, [_P] * 6 + [_I] * 4 + [_L] * 6 + [_F, _I, _I, _I, _P]),
     "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P]),
     "mmfs_attn_forward_persistent": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
@@ -71,8 +63,8 @@ def lib() -> ctypes.CDLL:
             fn = getattr(handle, name)  # AttributeError if the ABI is incomplete
             fn.restype = res
             fn.argtypes = args
-        if handle.mmfs_abi_version() != 1:
-            raise RuntimeError(f"libmmfs_b200.so ABI {handle.mmfs_abi_version()} != 1")
+        if handle.mmfs_abi_version() != 2:
+            raise RuntimeError(f"libmmfs_b200.so ABI {handle.mmfs_abi_version()} != 2")
         _lib = handle
     return _lib
 

@@ -1,15 +1,12 @@
 """Dispatch to the wgmma flash-attention kernel (csrc/attn_fwd_sm100.cu)."""
 from __future__ import annotations
 
-import os
-
 import torch
 
 from . import _lib
 from .msda import _DTYPE_CODE
 
-MIN_QUERY_ROWS = int(os.environ.get("MMFS_ATTN_TC_MIN_ROWS", "16"))   # below this the GEMV-style kernel wins
-PERSISTENT = os.environ.get("MMFS_ATTN_PERSISTENT", "1") != "0"         # work-list kernel when items > resident CTAs
+MIN_QUERY_ROWS = 16   # below this the GEMV-style kernel wins
 _SMS = {}
 
 
@@ -29,7 +26,7 @@ def forward(q, k, v, out, key_mask, causal, past, scale):
         sms = _SMS[q.device.index] = torch.cuda.get_device_properties(q.device).multi_processor_count
     # resident CTAs per SM: 1 at hd 128, 2 at hd 64 (attn_ctas_per_sm in csrc/attn_fwd_sm100.cu); the persistent
     # kernel only pays off with more items than resident CTAs
-    if PERSISTENT and B * H * ((Tq + 127) // 128) > (2 if hd == 64 else 1) * sms:
+    if B * H * ((Tq + 127) // 128) > (2 if hd == 64 else 1) * sms:
         # one zeroed word per call (a fill kernel; inside a CUDA graph it is re-zeroed on every replay): the kernel's
         # work counter must be private to the launch
         counter = torch.zeros((1,), dtype=torch.int32, device=q.device)

@@ -245,14 +245,15 @@ __device__ __forceinline__ float dot16_mixed(const uint4 &ka, const uint4 &kb, c
     return d0 + d1;
 }
 
-template <typename T, int WARPS>
-__global__ void __launch_bounds__(32 * WARPS, WARPS == 4 ? 5 : 2)
+template <typename T>
+__global__ void __launch_bounds__(32 * kDecWarps, 5)
 attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *__restrict__ v,
                             const uint8_t *__restrict__ key_mask, float *__restrict__ part, unsigned *__restrict__ tickets,
                             T *__restrict__ out, int H, int Tkv, long q_bs, long k_bs, long k_ts, long v_bs, long v_ts,
                             long o_bs, float scale, int last_key) {
-    constexpr int HD = 128, KPW = kDecKeys / WARPS, NB = KPW / 16;   // 64 (4 warps) or 32 (8 warps) keys per warp
-    static_assert((WARPS == 4 || WARPS == 8) && 32 * WARPS >= HD, "one thread per channel in the combine / merge steps");
+    constexpr int WARPS = kDecWarps, HD = 128, KPW = kDecKeys / WARPS;
+    static_assert(KPW == 64, "the pipeline below walks a warp's keys in four batches of 16");
+    static_assert(32 * WARPS >= HD, "one thread per channel in the combine / merge steps");
     __shared__ float s_p[WARPS][KPW];
     __shared__ __align__(16) float s_acc[WARPS][HD];
     __shared__ float s_m[WARPS], s_l[WARPS];
@@ -270,7 +271,7 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
     if (k0 <= last_key) {                                         // warp-uniform
         const int ja = k0 + lane, jb = ja + 32;
         const bool oa = ja <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + ja]);
-        const bool ob = KPW == 64 && jb <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + jb]);
+        const bool ob = jb <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + jb]);
         ok_lo = __ballot_sync(0xffffffffu, oa);
         ok_hi = __ballot_sync(0xffffffffu, ob);
     }
@@ -323,16 +324,12 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
         uint4 ra[8], rb[8];
         load_k(ra, 0);
         load_k(rb, 1); scores(ra, 0);
-        if constexpr (NB == 4) {
-            load_k(ra, 2); scores(rb, 1);
-            load_k(rb, 3); scores(ra, 2);
-            load_v(ra, 0); scores(rb, 3);
-        } else {
-            load_v(ra, 0); scores(rb, 1);
-        }
+        load_k(ra, 2); scores(rb, 1);
+        load_k(rb, 3); scores(ra, 2);
+        load_v(ra, 0); scores(rb, 3);
         __syncwarp();
         // ---- softmax over the warp's keys ----------------------------------------------------------------------
-        const float s0 = s_p[warp][lane], s1 = KPW == 64 ? s_p[warp][(lane + 32) % KPW] : -INFINITY;
+        const float s0 = s_p[warp][lane], s1 = s_p[warp][lane + 32];
         m = fmaxf(s0, s1);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -342,17 +339,13 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
         for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
         __syncwarp();
         s_p[warp][lane] = p0;
-        if constexpr (KPW == 64) s_p[warp][lane + 32] = p1;
+        s_p[warp][lane + 32] = p1;
         __syncwarp();
         // ---- P V ---------------------------------------------------------------------------------------------
         load_v(rb, 1); pv(ra, 0);
-        if constexpr (NB == 4) {
-            load_v(ra, 2); pv(rb, 1);
-            load_v(rb, 3); pv(ra, 2);
-            pv(rb, 3);
-        } else {
-            pv(rb, 1);
-        }
+        load_v(ra, 2); pv(rb, 1);
+        load_v(rb, 3); pv(ra, 2);
+        pv(rb, 3);
 #pragma unroll
         for (int c = 0; c < 8; ++c) acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], 16);
     }
@@ -411,7 +404,7 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
 
 // (Alternative not taken: staging a warp's whole 64-key K and V tiles in shared memory with cp.async -- 32 KB per warp
 // requested up front, 6 warps per SM -- leaves so few warps that the score / softmax / P V arithmetic out of shared
-// memory is latency-exposed; tools/decode_attn_ab.py compares the variants.)
+// memory is latency-exposed.)
 template <typename T>
 __global__ void attn_decode_merge_kernel(const float *__restrict__ part, T *__restrict__ out, int H, int hd, int n_split,
                                          long o_bs) {
@@ -433,8 +426,6 @@ __global__ void attn_decode_merge_kernel(const float *__restrict__ part, T *__re
     }
 }
 
-static int g_dec_warps = 4;   // warps per 256-key CTA of the hd-128 decode kernel (mmfs_attn_decode_set_tuning)
-
 static inline long decode_ticket_floats(int B, int H) { return ((long)B * H + 3) / 4 * 4; }   // keeps the partials 16-byte aligned
 
 template <typename T>
@@ -448,12 +439,9 @@ static int launch_attn_decode(const void *q, const void *k, const void *v, void 
             unsigned *tickets = reinterpret_cast<unsigned *>(scratch);          // [B * H], then the partials
             float *part = scratch + decode_ticket_floats(B, H);
             if (n_split > 1) MMFS_CUDA(cudaMemsetAsync(tickets, 0, sizeof(unsigned) * (size_t)B * H, st));
-            if (g_dec_warps == 8)
-                attn_decode_split128_kernel<T, 8><<<grid, 256, 0, st>>>((const T *)q, (const T *)k, (const T *)v, key_mask, part, tickets,
-                                                                     (T *)out, H, Tkv, q_bs, k_bs, k_ts, v_bs, v_ts, o_bs, scale, last_key);
-            else
-                attn_decode_split128_kernel<T, 4><<<grid, 128, 0, st>>>((const T *)q, (const T *)k, (const T *)v, key_mask, part, tickets,
-                                                                     (T *)out, H, Tkv, q_bs, k_bs, k_ts, v_bs, v_ts, o_bs, scale, last_key);
+            attn_decode_split128_kernel<T><<<grid, 32 * kDecWarps, 0, st>>>((const T *)q, (const T *)k, (const T *)v, key_mask, part,
+                                                                          tickets, (T *)out, H, Tkv, q_bs, k_bs, k_ts, v_bs, v_ts,
+                                                                          o_bs, scale, last_key);
             MMFS_CUDA(cudaGetLastError());
             return MMFS_OK;
         }
@@ -499,12 +487,6 @@ extern "C" int mmfs_attn_generic(const void *q, const void *k, const void *v, vo
         case MMFS_BF16: return launch_attn_generic<__nv_bfloat16>(q, k, v, out, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts, scale, causal, past, st);
         default: set_error("attn_generic: dtype %d unsupported", dtype); return MMFS_EINVAL;
     }
-}
-
-extern "C" int mmfs_attn_decode_set_tuning(int warps) {
-    MMFS_CHECK_ARG(warps == 0 || warps == 4 || warps == 8, "attn_decode_set_tuning: warps 0 (default) / 4 / 8");
-    g_dec_warps = warps == 0 ? 4 : warps;
-    return MMFS_OK;
 }
 
 extern "C" long mmfs_attn_decode_scratch_floats(int B, int H, int Tkv, int hd) {

@@ -65,7 +65,6 @@ __global__ void __launch_bounds__(32 * kWarpsPerCta, 3) mmfs_sampler_kernel(cons
     const int C = M * P * 2 + M * n_lvl * (P + 1);
     const long long row_bytes = (long long)M * D * (int)sizeof(T);
     const bool strict = a.flags & MMFS_MSDA_STRICT;
-    const bool w16 = a.flags & MMFS_MSDA_W16;
     const int slot = lane / LPR;
     const float nullv = round_to<T>(a.null_logit);
     const int per_img = n_lvl * P;                            // sampling items of one image
@@ -96,7 +95,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerCta, 3) mmfs_sampler_kernel(cons
         pre_r = 0;
         if (lane < n_img) pre_r = a.relpos[((size_t)c.b * n_img + lane) * a.Lq_r + (a.Lq_r == 1 ? 0 : c.q)];
     };
-    RowCursor cur = walk.first(a.ctas_per_sm, a.nsm, a.swizzle);
+    RowCursor cur = walk.first(a.ctas_per_sm, a.nsm);
     if (cur.ok) prefetch(cur);
 
     while (cur.ok) {
@@ -216,7 +215,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerCta, 3) mmfs_sampler_kernel(cons
                 __syncwarp();
                 emit_taps(taps, lane, live, g, aw, lv.x, lv.y, lv.z, row_bytes, zero_off);
                 __syncwarp();
-                gather_pass_any<T, D>(taps, livemask, vbase, slot, acc, w16);
+                gather_pass<T, D>(taps, livemask, vbase, slot, acc);
             }
         }
         if (!EMIT) store_row<T, D>(acc, static_cast<T *>(a.out) + qm * D, lane);
@@ -250,7 +249,7 @@ static int launch_sampler(SamplerArgs a, int N, cudaStream_t st) {
     a.qtiles = (a.Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw);
     a.ntiles = (long)N * a.M * a.qtiles;
     if (a.ntiles > 0x3fffffffL) { set_error("mmfs_sampler: too many tiles"); return MMFS_EUNSUPPORTED; }
-    a.ctas_per_sm = ctas_per_sm; a.nsm = nsm; a.swizzle = 1;
+    a.ctas_per_sm = ctas_per_sm; a.nsm = nsm;
     const long full = (long)nsm * ctas_per_sm;
     const unsigned grid = (unsigned)(a.ntiles < full ? a.ntiles : full);
     kern<<<grid, 32 * kWarpsPerCta, smem, st>>>(a);

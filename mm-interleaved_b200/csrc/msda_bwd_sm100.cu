@@ -94,7 +94,7 @@ msda_bwd_rows_kernel(const T *__restrict__ value, const int64_t *__restrict__ sh
     walk.itiles = (int)ntiles; walk.igrid = (int)gridDim.x; walk.qtiles = qtiles; walk.M = M; walk.Lq = Lq;
     walk.rows_per_warp = rows_per_warp; walk.warp = warp;
 
-    for (RowCursor cur = walk.first(ctas_per_sm, nsm, 1); cur.ok; cur = walk.next(cur)) {
+    for (RowCursor cur = walk.first(ctas_per_sm, nsm); cur.ok; cur = walk.next(cur)) {
         const int b = cur.b, m = cur.m, q = cur.q;
         const size_t qm = ((size_t)b * Lq + q) * M + m;
         const T *locp = loc + qm * (size_t)LP * 2;

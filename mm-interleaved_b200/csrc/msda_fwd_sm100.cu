@@ -39,7 +39,7 @@ msda_fwd_rows_kernel(const T *__restrict__ value, const int64_t *__restrict__ sh
                      const T *__restrict__ attn, T *__restrict__ out,
                      int S, int M, int L, int Lq, int P, int p_shift, unsigned flags,
                      int rows_per_warp, int qtiles, long ntiles, int ctas_per_sm, int nsm,
-                     int stage_elems, int bulk_ok, int swizzle) {
+                     int stage_elems, int bulk_ok) {
     constexpr int VEC = 16 / (int)sizeof(T);  // channels per lane
     constexpr int LPR = D / VEC;              // lanes per value row
     static_assert(D % VEC == 0 && LPR >= 1 && LPR <= 32 && (LPR & (LPR - 1)) == 0, "unsupported D");
@@ -65,7 +65,6 @@ msda_fwd_rows_kernel(const T *__restrict__ value, const int64_t *__restrict__ sh
     const int LP = L * P;
     const long long row_bytes = (long long)M * D * (int)sizeof(T);
     const bool strict = flags & MMFS_MSDA_STRICT;
-    const bool w16 = flags & MMFS_MSDA_W16;
     const int slot = lane / LPR;
     const uint32_t loc_bytes = (uint32_t)(2 * LP * (int)sizeof(T)), att_bytes = (uint32_t)(LP * (int)sizeof(T));
 
@@ -90,7 +89,7 @@ msda_fwd_rows_kernel(const T *__restrict__ value, const int64_t *__restrict__ sh
         }
     };
 
-    RowCursor cur = walk.first(ctas_per_sm, nsm, swizzle);
+    RowCursor cur = walk.first(ctas_per_sm, nsm);
     unsigned n_staged = 0;  // rows staged so far: buffer = n & 1, parity = (n >> 1) & 1
     if (cur.ok) stage_row(cur.b, cur.m, cur.q, 0);
 
@@ -137,7 +136,7 @@ msda_fwd_rows_kernel(const T *__restrict__ value, const int64_t *__restrict__ sh
             emit_taps(taps, lane, live, g, a, lv.x, lv.y, lv.z, row_bytes, zero_off);
             __syncwarp();
             // ---- phase 2 -------------------------------------------------------------------
-            gather_pass_any<T, D>(taps, livemask, vbase, slot, acc, w16);
+            gather_pass<T, D>(taps, livemask, vbase, slot, acc);
         }
 
         store_row<T, D>(acc, out + (((size_t)b * Lq + q) * M + m) * D, lane);
@@ -219,7 +218,7 @@ msda_fwd_generic_kernel(const T *__restrict__ value, const int64_t *__restrict__
                         const T *__restrict__ attn, T *__restrict__ out,
                         long total, int S, int M, int D, int L, int Lq, int P, unsigned flags) {
     using OP = typename OpMath<T>::type;
-    const bool strict = flags & MMFS_MSDA_STRICT;   // (MMFS_MSDA_W16 only affects the warp-per-row kernel)
+    const bool strict = flags & MMFS_MSDA_STRICT;
     for (long idx = (long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
         const int c = (int)(idx % D);
         const long qm = idx / D;
@@ -288,9 +287,6 @@ msda_index_stream_kernel(const int64_t *__restrict__ shapes, const int64_t *__re
 // ------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------
-static int g_rows_per_warp = 0;  // 0 = automatic
-static int g_mapping = 0;        // bit0: 1 = plain tile order (no per-SM swizzle)
-
 template <typename T, int D>
 static int launch_rows(const void *value, const int64_t *shapes, const int64_t *starts, const void *loc,
                        const void *attn, void *out, int N, int S, int M, int L, int Lq, int P,
@@ -314,13 +310,10 @@ static int launch_rows(const void *value, const int64_t *shapes, const int64_t *
     if (ctas_per_sm < 1) { set_error("msda: kernel does not fit on an SM (smem %zu)", smem); return MMFS_EUNSUPPORTED; }
     const int nsm = num_sms();
     // rows per warp per tile: short tiles -- neighbouring q-tiles of one head still share the L1-resident value slab
-    // through the per-SM tile swizzle, and short tiles balance the tail of the persistent grid (tools/msda_sweep.py
-    // times the alternatives).  Tiny problems (decode, Lq = 1) use 1.
-    int rpw = g_rows_per_warp;
-    if (rpw <= 0) {
-        rpw = 2;
-        while (rpw > 1 && (long)N * M * ((Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw)) < 2L * nsm * ctas_per_sm) rpw >>= 1;
-    }
+    // through the per-SM tile swizzle, and short tiles balance the tail of the persistent grid.  Tiny problems
+    // (decode, Lq = 1) use 1.
+    int rpw = 2;
+    while (rpw > 1 && (long)N * M * ((Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw)) < 2L * nsm * ctas_per_sm) rpw >>= 1;
     const int qtiles = (Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw);
     const long ntiles = (long)N * M * qtiles;
     if (ntiles > 0x3fffffffL) { set_error("msda: too many tiles (%ld)", ntiles); return MMFS_EUNSUPPORTED; }
@@ -330,8 +323,7 @@ static int launch_rows(const void *value, const int64_t *shapes, const int64_t *
                          ((2 * LP * sizeof(T)) % 16 == 0) && ((LP * sizeof(T)) % 16 == 0);
     kern<<<grid, 32 * kWarpsPerCta, smem, st>>>(
         (const T *)value, shapes, starts, (const T *)loc, (const T *)attn, (T *)out,
-        S, M, L, Lq, P, p_shift, flags, rpw, qtiles, ntiles, ctas_per_sm, nsm, stage_elems,
-        bulk_ok ? 1 : 0, (g_mapping & 1) ? 0 : 1);
+        S, M, L, Lq, P, p_shift, flags, rpw, qtiles, ntiles, ctas_per_sm, nsm, stage_elems, bulk_ok ? 1 : 0);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -356,7 +348,7 @@ static int dispatch_d(const void *value, const int64_t *shapes, const int64_t *s
 #define MMFS_CASE(DD) \
     case DD: return launch_rows<T, DD>(value, shapes, starts, loc, attn, out, N, S, M, L, Lq, P, flags, st);
     const bool aligned16 = ((uintptr_t)value % 16 == 0) && ((uintptr_t)out % 16 == 0);
-    if (aligned16 && L * P <= kSmallLP && g_rows_per_warp == 0 && (D == 32 || D == 64 || D == 128)) {
+    if (aligned16 && L * P <= kSmallLP && (D == 32 || D == 64 || D == 128)) {
         constexpr int VEC = 16 / (int)sizeof(T);
         const long total = (long)N * Lq * M * (D / VEC);
         const long blocks = (total + 255) / 256;
@@ -385,16 +377,6 @@ static int dispatch_d(const void *value, const int64_t *shapes, const int64_t *s
 }  // namespace mmfs
 
 using namespace mmfs;
-
-extern "C" int mmfs_msda_set_tuning(int rows_per_warp, int mapping) {
-    if (rows_per_warp < 0 || rows_per_warp > 64) {
-        set_error("mmfs_msda_set_tuning: rows_per_warp must be in [0, 64]");
-        return MMFS_EINVAL;
-    }
-    g_rows_per_warp = rows_per_warp;
-    g_mapping = mapping;
-    return MMFS_OK;
-}
 
 static int check_msda_args(const void *value, const int64_t *shapes, const int64_t *starts, const void *loc,
                            const void *attn, const void *out, int N, int S, int M, int D, int L, int Lq, int P, int dtype) {

@@ -177,61 +177,12 @@ template <> struct MixFma<__nv_bfloat16> {
     __device__ __forceinline__ static void fma(float &acc, uint16_t v, uint16_t w) {
         acc = __fmaf_rn(__uint_as_float((uint32_t)v << 16), __uint_as_float((uint32_t)w << 16), acc);
     }
-    __device__ __forceinline__ static uint16_t cvt(float w) { __nv_bfloat16 t = __float2bfloat16_rn(w); return *reinterpret_cast<uint16_t *>(&t); }
 };
 template <> struct MixFma<__half> {
     __device__ __forceinline__ static void fma(float &acc, uint16_t v, uint16_t w) {
         acc = __fmaf_rn(__half2float(__ushort_as_half(v)), __half2float(__ushort_as_half(w)), acc);
     }
-    __device__ __forceinline__ static uint16_t cvt(float w) { __half t = __float2half_rn(w); return *reinterpret_cast<uint16_t *>(&t); }
 };
-
-// gather_pass with 16-bit tap weights (MMFS_MSDA_W16): 8 mixed-precision FMA per 16-byte fetch instead of 8 unpack + 8 FFMA
-template <typename T, int D>
-__device__ __forceinline__ void gather_pass_w16(const Tap *taps, unsigned livemask, const char *vbase, int slot,
-                                                float (&acc)[16 / sizeof(T)]) {
-    constexpr int VEC = 16 / (int)sizeof(T);
-    constexpr int LPR = D / VEC;
-    constexpr int RPI = 32 / LPR;
-    constexpr int NIT = 128 / RPI;
-    constexpr int G = NIT < 8 ? NIT : 8;
-    constexpr int PPG = (G * RPI) / 4;
-    static_assert(VEC == 8, "16-bit element types only");
-#pragma unroll 1
-    for (int g0 = 0; g0 < NIT; g0 += G) {
-        const unsigned pm = (PPG >= 32) ? livemask : ((livemask >> ((g0 * RPI) / 4)) & ((1u << PPG) - 1u));
-        if (pm == 0u) continue;
-        Tap t[G];
-        uint4 v[G];
-#pragma unroll
-        for (int it = 0; it < G; ++it) {
-            const int tix = (g0 + it) * RPI + slot;
-            *reinterpret_cast<uint4 *>(&t[it]) =
-                *reinterpret_cast<const uint4 *>(&taps[(tix & 3) * kTapStride + (tix >> 2)]);
-        }
-#pragma unroll
-        for (int it = 0; it < G; ++it) v[it] = ldg_nc_v4(vbase + t[it].off);
-#pragma unroll
-        for (int it = 0; it < G; ++it) {
-            const uint16_t w = MixFma<T>::cvt(t[it].w0);
-            const uint32_t r[4] = {v[it].x, v[it].y, v[it].z, v[it].w};
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                MixFma<T>::fma(acc[2 * k], (uint16_t)(r[k] & 0xffffu), w);
-                MixFma<T>::fma(acc[2 * k + 1], (uint16_t)(r[k] >> 16), w);
-            }
-        }
-    }
-}
-// dispatch: 16-bit weights only for 16-bit element types and only on request
-template <typename T, int D>
-__device__ __forceinline__ void gather_pass_any(const Tap *taps, unsigned livemask, const char *vbase, int slot,
-                                                float (&acc)[16 / sizeof(T)], bool w16) {
-    if constexpr (sizeof(T) == 2) {
-        if (w16) { gather_pass_w16<T, D>(taps, livemask, vbase, slot, acc); return; }
-    }
-    gather_pass<T, D>(taps, livemask, vbase, slot, acc);
-}
 
 // epilogue: sum the RPI slots, one rounding, 16-byte stores
 template <typename T, int D>
@@ -263,9 +214,9 @@ struct RowWalk {
             c.r = 0; c.tile += igrid;  // the rest of this tile's rows are past Lq as well
         }
     }
-    __device__ __forceinline__ RowCursor first(int ctas_per_sm, int nsm, int swizzle) const {
+    __device__ __forceinline__ RowCursor first(int ctas_per_sm, int nsm) const {   // swizzled when the grid is full
         long t0 = blockIdx.x;
-        if (swizzle && gridDim.x == (unsigned)(nsm * ctas_per_sm))
+        if (gridDim.x == (unsigned)(nsm * ctas_per_sm))
             t0 = (long)(blockIdx.x % nsm) * ctas_per_sm + blockIdx.x / nsm;
         RowCursor c; c.tile = (int)t0; c.r = 0; c.b = c.m = c.q = 0; c.ok = false;
         settle(c);
@@ -310,7 +261,7 @@ struct SamplerArgs {
     unsigned flags;
     int rows_per_warp, qtiles;
     long ntiles;
-    int ctas_per_sm, nsm, swizzle;
+    int ctas_per_sm, nsm;
     int walk_dq, walk_dm, walk_db;   // specialised kernel: grid-stride decomposed into (q-tile, head, batch) steps
 };
 
@@ -319,6 +270,5 @@ struct SamplerArgs {
 // without touching the error text when the configuration is outside its domain (the caller then takes the
 // generic kernel).
 int launch_sampler_v2(const SamplerArgs &a, int N, int D, int dtype, cudaStream_t st);
-int sampler_v2_set_tuning(int rows_per_warp, int wmode);
 
 }  // namespace mmfs

@@ -21,7 +21,6 @@ Plain library GEMMs (cuBLAS via torch) are used for the dense linears.
 from __future__ import annotations
 
 import math
-import os
 from dataclasses import dataclass, field
 from types import SimpleNamespace
 from typing import List, Optional, Tuple
@@ -109,17 +108,6 @@ class _CatWeight:
         return self.weight
 
 
-# Decode-step linears (at most 8 tokens in flight): ``ops.linear_skinny`` -- this repo's HBM-streaming kernel with the
-# RMSNorm / SwiGLU in front folded in -- or cuBLAS + the stand-alone norm / activation kernel.  cuBLAS is the default
-# (DESIGN.md section 4.7); MMFS_SKINNY_LINEARS=1 or ``llama_mmfs.SKINNY_DECODE_LINEARS = True`` switches.
-SKINNY_DECODE_LINEARS = os.environ.get("MMFS_SKINNY_LINEARS", "0") == "1"
-
-
-def _skinny(x, weight, prologue=0):
-    return (SKINNY_DECODE_LINEARS and not torch.is_grad_enabled() and x.is_cuda and
-            ops.linear_skinny_supported(x, weight, prologue))
-
-
 def _addmm_residual(residual, x, weight, inplace):
     """residual + x @ weight^T as one GEMM with the residual as the beta = 1 accumulator.  ``torch.addmm`` out of
     place first copies the residual into the result (a D2D memcpy of the whole stream per call); in place skips it."""
@@ -141,19 +129,9 @@ class LlamaMLP(nn.Module):
         self.up_proj = nn.Linear(hidden_size, intermediate_size, bias=False)
         self._gate_up = _CatWeight(self.gate_proj, self.up_proj)
 
-    def forward(self, x, residual=None, inplace=False, pre_norm=None):
-        """``inplace``: accumulate into ``residual``'s storage (beta = 1 GEMM epilogue, no copy of the stream).
-        ``pre_norm`` (extension): the LlamaRMSNorm in front of the block; ``x`` is then the un-normalised stream."""
-        w_gu = self._gate_up.get()
-        inter, hidden = self.down_proj.in_features, self.down_proj.out_features
-        if pre_norm is not None and residual is not None and inplace and _skinny(x, w_gu, 1) and \
-                ops.linear_skinny_shape_ok(x.shape[:-1].numel(), hidden, inter):           # down_proj's own limits
-            gu = ops.linear_skinny(x, w_gu, norm_weight=pre_norm.weight, eps=pre_norm.variance_epsilon)
-            ops.linear_skinny(gu, self.down_proj.weight, residual=residual, out=residual, swiglu=True)
-            return residual
-        if pre_norm is not None:
-            x = pre_norm(x)
-        gu = F.linear(x, w_gu)                                 # [gate | up] in one GEMM
+    def forward(self, x, residual=None, inplace=False):
+        """``inplace``: accumulate into ``residual``'s storage (beta = 1 GEMM epilogue, no copy of the stream)."""
+        gu = F.linear(x, self._gate_up.get())                 # [gate | up] in one GEMM
         act = ops.swiglu(gu)
         if residual is None:
             return self.down_proj(act)
@@ -216,23 +194,16 @@ class LlamaAttention(nn.Module):
         return self._rope[2], self._rope[3]
 
     def forward(self, hidden_states, attention_mask=None, position_ids=None, past_key_value=None,
-                output_attentions=False, use_cache=False, residual=None, inplace=False, pre_norm=None):
+                output_attentions=False, use_cache=False, residual=None, inplace=False):
         """``attention_mask``: (B, T_kv) key-padding mask, 1 = attend (what LlamaModel.forward receives,
         modeling_llama_mmfs.py:625) or None.  Causality is implicit (decoder).  Returns
         (attn_output [+ residual], None, present_key_value) like the reference (:217-280); the cache
-        holds (key, value) in (B, T, H, hd) layout.  ``pre_norm`` (extension): the input LlamaRMSNorm;
-        ``hidden_states`` is then the un-normalised stream (a decode step folds the norm into the q/k/v kernel)."""
+        holds (key, value) in (B, T, H, hd) layout."""
         if output_attentions:
             raise NotImplementedError("attention probabilities are never materialised by the fused kernel")
         B, T, _ = hidden_states.shape
         H, hd = self.num_heads, self.head_dim
-        w_qkv = self._qkv.get()
-        skinny = _skinny(hidden_states, w_qkv, 1 if pre_norm is not None else 0)
-        if skinny:
-            qkv = ops.linear_skinny(hidden_states, w_qkv, norm_weight=None if pre_norm is None else pre_norm.weight,
-                                    eps=0.0 if pre_norm is None else pre_norm.variance_epsilon).view(B, T, 3, H, hd)
-        else:
-            qkv = F.linear(hidden_states if pre_norm is None else pre_norm(hidden_states), w_qkv).view(B, T, 3, H, hd)
+        qkv = F.linear(hidden_states, self._qkv.get()).view(B, T, 3, H, hd)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
         static = isinstance(past_key_value, StaticKV)
         past = 0 if past_key_value is None else (past_key_value.length if static else past_key_value[0].shape[1])
@@ -266,10 +237,7 @@ class LlamaAttention(nn.Module):
             else:
                 key_mask = attention_mask
         ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)       # (B, T, H*hd)
-        if skinny and residual is not None and inplace and _skinny(ctx, self.o_proj.weight):
-            out = ops.linear_skinny(ctx, self.o_proj.weight, residual=residual, out=residual)
-        else:
-            out = self.o_proj(ctx) if residual is None else _addmm_residual(residual, ctx, self.o_proj.weight, inplace)
+        out = self.o_proj(ctx) if residual is None else _addmm_residual(residual, ctx, self.o_proj.weight, inplace)
         return out, None, present
 
 
@@ -374,13 +342,13 @@ class LlamaDecoderLayer(nn.Module):
         # guarantees ``hidden_states`` is a private contiguous buffer (LlamaModel.forward clones the embeddings once).
         residual = hidden_states.contiguous()
         inplace = inplace and not torch.is_grad_enabled()
-        hidden_states, _, present = self.self_attn(residual, attention_mask=attention_mask, position_ids=position_ids,
-                                                   past_key_value=past_key_value, use_cache=use_cache, residual=residual,
-                                                   inplace=inplace, pre_norm=self.input_layernorm)
+        hidden_states, _, present = self.self_attn(self.input_layernorm(residual), attention_mask=attention_mask,
+                                                   position_ids=position_ids, past_key_value=past_key_value,
+                                                   use_cache=use_cache, residual=residual, inplace=inplace)
         if self.llama_cross_attn is not None and vision_hidden_states is not None:
             hidden_states = self.llama_cross_attn(hidden_states, vision_hidden_states, cross_attention_mask,
                                                   residual=hidden_states, inplace=inplace)
-        hidden_states = self.mlp(hidden_states, residual=hidden_states, inplace=inplace, pre_norm=self.post_attention_layernorm)
+        hidden_states = self.mlp(self.post_attention_layernorm(hidden_states), residual=hidden_states, inplace=inplace)
         outputs = (hidden_states,)
         if use_cache:
             outputs += (present,)

@@ -55,7 +55,7 @@ def _check_inputs(value, spatial_shapes, level_start_index, sampling_loc, attn_w
 
 
 def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight,
-                           im2col_step: int = 64, strict: bool = False, w16: bool = False) -> torch.Tensor:
+                           im2col_step: int = 64, strict: bool = False) -> torch.Tensor:
     """Drop-in for ``MSDA.ms_deform_attn_forward`` (ops/src/ms_deform_attn.h:20-39).
 
     Returns a new tensor (N, Lq, M*D) with value's dtype/device (cu:55,78).  All N samples go
@@ -73,7 +73,7 @@ def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_lo
             value.data_ptr(), spatial_shapes.data_ptr(), level_start_index.data_ptr(),
             sampling_loc.data_ptr(), attn_weight.data_ptr(), out.data_ptr(),
             N, S, M, D, L, Lq, P, _DTYPE_CODE[value.dtype],
-            (_lib.MSDA_STRICT if strict else 0) | (_lib.MSDA_W16 if w16 else 0), stream)
+            _lib.MSDA_STRICT if strict else 0, stream)
     _lib.check(rc, "ms_deform_attn_forward")
     return out
 

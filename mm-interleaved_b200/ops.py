@@ -182,62 +182,6 @@ def attention(q, k, v, key_mask=None, causal=True, past=0, scale=None, force_gen
     return out.view(B, Tq, H * hd)
 
 
-_SKINNY_SCRATCH = {}   # device -> zeroed fp32 scratch (tickets + partial tiles), shared by every call on the device
-
-
-def linear_skinny_shape_ok(M: int, N: int, K: int) -> bool:
-    """At most 8 rows, N % 32 == 0, K % 512 == 0, the x rows + at least two 32 KB stages of the copy ring inside shared
-    memory (``csrc/linear_skinny_sm100.cu``): 8 rows up to K = 9216, 4 rows up to K = 18432."""
-    return (1 <= M <= 8 and N % 32 == 0 and N <= 32 << 16 and K % 512 == 0 and
-            2 * 32768 + M * (K * 2 + 64) + 16912 <= 227 * 1024)
-
-
-def linear_skinny_supported(x: torch.Tensor, weight: torch.Tensor, prologue: int = 0) -> bool:
-    """Whether ``linear_skinny`` takes this call: CUDA, f16 / bf16, contiguous, ``linear_skinny_shape_ok``."""
-    N, K = weight.shape
-    M = x.numel() // (K * (2 if prologue == 2 else 1))
-    return (x.is_cuda and x.dtype in (torch.float16, torch.bfloat16) and weight.dtype == x.dtype and x.is_contiguous()
-            and weight.is_contiguous() and linear_skinny_shape_ok(M, N, K))
-
-
-def linear_skinny(x: torch.Tensor, weight: torch.Tensor, residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
-                  norm_weight: Optional[torch.Tensor] = None, eps: float = 0.0, swiglu: bool = False) -> torch.Tensor:
-    """Decode-step linear ``prologue(x) @ weight^T (+ residual)`` for at most 8 rows (see ``mmfs_linear_skinny`` in
-    include/mmfs_b200.h).  ``norm_weight``: fold LlamaRMSNorm(x) in front; ``swiglu``: x is ``[gate | up]`` rows of
-    2K columns and the operand is silu(gate) * up.  ``out`` may be ``residual`` itself (in-place residual stream)."""
-    prologue = 1 if norm_weight is not None else (2 if swiglu else 0)
-    N, K = weight.shape
-    M = x.numel() // (K * (2 if swiglu else 1))
-    _require(linear_skinny_supported(x, weight, prologue), "linear_skinny: unsupported shape / dtype (see linear_skinny_supported)")
-    inference_only("linear_skinny", x, weight)
-    if out is None:
-        out = torch.empty(tuple(x.shape[:-1]) + (N,), dtype=x.dtype, device=x.device)
-    _require(out.is_contiguous() and out.numel() == M * N and out.dtype == x.dtype, "linear_skinny: out must be contiguous (M, N)")
-    if residual is not None:
-        _require(residual.is_contiguous() and residual.numel() == M * N and residual.dtype == x.dtype,
-                 "linear_skinny: residual must be contiguous (M, N)")
-    if norm_weight is not None:
-        _require(norm_weight.is_contiguous() and norm_weight.numel() == K and norm_weight.dtype == x.dtype,
-                 "linear_skinny: norm_weight must be (K,) in x.dtype")
-    lib = _lib.lib()
-    need = lib.mmfs_linear_skinny_scratch_floats(N)
-    key = (x.device.type, x.device.index)
-    scratch = _SKINNY_SCRATCH.get(key)
-    if scratch is None or scratch.numel() < need:
-        # zero once: every call leaves its tickets zero.  (Allocated outside any graph capture by the warm-up steps a
-        # capture is preceded by; a capture that allocates here records the zero fill, which is harmless.)
-        scratch = torch.zeros((max(need, 1 << 20),), dtype=torch.float32, device=x.device)
-        _SKINNY_SCRATCH[key] = scratch
-    with torch.cuda.device(x.device):
-        rc = lib.mmfs_linear_skinny(x.data_ptr(), weight.data_ptr(), out.data_ptr(),
-                                    residual.data_ptr() if residual is not None else None,
-                                    norm_weight.data_ptr() if norm_weight is not None else None, scratch.data_ptr(),
-                                    M, N, K, prologue, float(eps), _DTYPE_CODE[x.dtype], _stream())
-    _lib.check(rc, "linear_skinny")
-    launch_counter[0] += 1
-    return out
-
-
 def conv2d_supported(x: torch.Tensor, weight: torch.Tensor, stride: int, padding: int) -> bool:
     """Whether ``conv2d`` can take this layer (else the caller keeps it on cuDNN: conv_in / conv_out of the UNet)."""
     if x.dtype not in (torch.bfloat16, torch.float16) or not x.is_cuda or x.dim() != 4:

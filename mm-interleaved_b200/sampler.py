@@ -27,14 +27,14 @@ def _common(shapes, starts, qproj, rtable, relpos, refpts, scale_ratios, M, n_lv
 
 
 def mmfs_sampler_forward(value, shapes, starts, qproj, rtable, relpos, refpts, scale_ratios,
-                         n_levels: int, n_points: int, want_null_mass: bool = False, strict: bool = False, w16: bool = False,
+                         n_levels: int, n_points: int, want_null_mass: bool = False, strict: bool = False,
                          exact_weights: bool = False, generic: bool = False):
     """Fused relpos lookup + mask + null-slot softmax + location arithmetic + deformable gather.
     Returns the sampled features (N, Lq, M*D) [and the null mass (N, Lq, M) fp32].
 
     16-bit tensors with D = 64, P = 8 and 3 or 4 levels run the specialised kernel (csrc/mmfs_sampler_v2_sm100.cu),
     whose tap weights are rounded to the element type by default; ``exact_weights`` keeps them fp32 there,
-    ``generic`` forces the generic kernel (where ``w16`` is the opt-in for 16-bit weights)."""
+    ``generic`` forces the generic kernel (fp32 tap weights)."""
     from .ops import inference_only
     inference_only("mmfs_sampler_forward", value, qproj, rtable)
     _require(value.is_cuda and value.is_contiguous() and value.dim() == 4, "value must be contiguous CUDA (N,S,M,D)")
@@ -52,7 +52,7 @@ def mmfs_sampler_forward(value, shapes, starts, qproj, rtable, relpos, refpts, s
             null_mass.data_ptr() if want_null_mass else None,
             N, S, M, D, n_img, n_levels, Lq, n_points, relpos.shape[2], refpts.shape[0], refpts.shape[2],
             rtable.shape[0], _DTYPE_CODE[value.dtype],
-            (_lib.MSDA_STRICT if strict else 0) | (_lib.MSDA_W16 if w16 else 0) |
+            (_lib.MSDA_STRICT if strict else 0) |
             (_lib.SAMPLER_EXACT_WEIGHTS if exact_weights else 0) | (_lib.SAMPLER_GENERIC if generic else 0),
             torch.cuda.current_stream().cuda_stream)
     _lib.check(rc, "mmfs_sampler_forward")
@@ -78,10 +78,3 @@ def mmfs_sampler_locw(shapes, starts, qproj, rtable, relpos, refpts, scale_ratio
             rtable.shape[0], _DTYPE_CODE[qproj.dtype], torch.cuda.current_stream().cuda_stream)
     _lib.check(rc, "mmfs_sampler_locw")
     return loc, attn, null_mass
-
-
-def set_sampler_tuning(rows_per_warp: int = 0, wmode: int = 1, ctas_per_sm: int = 0) -> None:
-    """Benchmarks / tests: rows per warp per tile (0 = automatic), the weight mode of the specialised kernel and the
-    occupancy variant it is compiled for (0 = keep, 3 or 4 resident CTAs per SM)."""
-    _lib.check(_lib.lib().mmfs_sampler_set_tuning(int(rows_per_warp), int(wmode) | (int(ctas_per_sm) << 4)),
-               "mmfs_sampler_set_tuning")

@@ -16,7 +16,7 @@ def header_symbols():
     return sorted(set(re.findall(r"\b(mmfs_[a-z0-9_]+)\s*\(", text)))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_at_abi_2():
     from mm_interleaved_b200 import _lib
     lib = _lib.lib()
     syms = header_symbols()
@@ -24,10 +24,10 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(lib, s), f"{s} declared in include/mmfs_b200.h but not exported"
         assert s in _lib.SIGNATURES, f"{s} has no ctypes signature"
-    assert lib.mmfs_abi_version() == 1
+    assert lib.mmfs_abi_version() == 2
 
 
-def test_argument_validation_without_gpu():
+def test_msda_forward_argument_validation_without_gpu():
     from mm_interleaved_b200 import _lib
     lib = _lib.lib()
     # null pointers / bad dims are rejected before any CUDA call
@@ -40,8 +40,6 @@ def test_argument_validation_without_gpu():
     # empty batch is a no-op success (the reference returns an empty tensor)
     rc = lib.mmfs_msda_forward(None, None, None, None, None, None, 0, 4, 1, 8, 1, 1, 1, _lib.F32, 0, None)
     assert rc == _lib.OK
-    assert lib.mmfs_msda_set_tuning(-1, 0) == _lib.EINVAL
-    assert lib.mmfs_msda_set_tuning(0, 0) == _lib.OK
 
 
 def test_python_shim_mirrors_reference_errors():

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the MSDA forward kernel over the BASELINE shapes and tuning variants.
+"""Micro-benchmark of the MSDA forward kernel over the BASELINE shapes.
 CUDA-event timing on the launching stream, L2 flushed between iterations.  Internal tool
 (bench.py is the contract); results land in gpurun_out/msda_sweep.json."""
 import json
@@ -48,7 +48,6 @@ def time_kernel(fn, iters=20, flush=None):
 
 
 def main():
-    lib = m._lib.lib()
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")
     res = []
     for name, (N, shapes, M, D, Lq, P) in SHAPES.items():
@@ -71,18 +70,14 @@ def main():
                     loc = ref[None, :, None, None, None, :] + (loc - 0.5) * (12.0 / side if loc_mode == "clustered" else 0.5)
                 args = [v.to("cuda", dtype), s.cuda(), st.cuda(), loc.to("cuda", dtype).contiguous(), a.to("cuda", dtype)]
                 ab = algo_bytes(N, shapes, M, D, Lq, P, 2 if dtype == torch.bfloat16 else 4)
-                variants = [(0, 0)] if dtype == torch.float32 else [(0, 0), (0, 1), (1, 0), (2, 0), (4, 0), (16, 0)]
-                for wpc, mapping in variants:
-                    lib.mmfs_msda_set_tuning(wpc, mapping)
-                    fn = lambda: m.ms_deform_attn_forward(*args, 64)
-                    med_cold, best_cold = time_kernel(fn, flush=flush)
-                    med_warm, best_warm = time_kernel(fn, flush=None)
-                    r = dict(shape=name, loc=loc_mode, dtype=str(dtype).split(".")[-1], rpw=wpc, mapping=mapping,
-                             algo_MB=ab / 1e6, cold_us=med_cold * 1e6, warm_us=med_warm * 1e6,
-                             cold_GBs=ab / med_cold / 1e9, warm_GBs=ab / med_warm / 1e9)
-                    res.append(r)
-                    print(json.dumps(r), flush=True)
-                lib.mmfs_msda_set_tuning(0, 0)
+                fn = lambda: m.ms_deform_attn_forward(*args, 64)
+                med_cold, best_cold = time_kernel(fn, flush=flush)
+                med_warm, best_warm = time_kernel(fn, flush=None)
+                r = dict(shape=name, loc=loc_mode, dtype=str(dtype).split(".")[-1],
+                         algo_MB=ab / 1e6, cold_us=med_cold * 1e6, warm_us=med_warm * 1e6,
+                         cold_GBs=ab / med_cold / 1e9, warm_GBs=ab / med_warm / 1e9)
+                res.append(r)
+                print(json.dumps(r), flush=True)
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     json.dump(res, open(os.path.join(ROOT, "gpurun_out", "msda_sweep.json"), "w"), indent=1)
 

@@ -14,9 +14,7 @@ from mm_interleaved_b200.mmfs import relative_image_index  # noqa: E402
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 4
 reps = int(sys.argv[2]) if len(sys.argv) > 2 else 10
 masked = (sys.argv[3] if len(sys.argv) > 3 else "masked") == "masked"
-mode = sys.argv[4] if len(sys.argv) > 4 else "v2"          # v2 (default kernel) | exact | generic | generic_w16
-rpw = int(sys.argv[5]) if len(sys.argv) > 5 else 0
-occ = int(sys.argv[6]) if len(sys.argv) > 6 else 0
+mode = sys.argv[4] if len(sys.argv) > 4 else "v2"          # v2 (default kernel) | exact | generic
 wl = InterleavedCfg3(0, 1, B)
 wl.make_host_inputs(pin=False)
 ids = wl.host[0].cuda()
@@ -35,9 +33,7 @@ starts = torch.cat((shapes.new_zeros((1,)), shapes.prod(1).cumsum(0)[:-1]))
 ref = torch.full((1, Lq, 1, 2), 0.5, device="cuda")
 scale = torch.tensor([2.0, 1.0, 0.5], device="cuda")
 flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device="cuda")
-from mm_interleaved_b200.sampler import set_sampler_tuning  # noqa: E402
-set_sampler_tuning(rpw, 1, occ)
-kw = dict(v2={}, exact=dict(exact_weights=True), generic=dict(generic=True), generic_w16=dict(generic=True, w16=True))[mode]
+kw = dict(v2={}, exact=dict(exact_weights=True), generic=dict(generic=True))[mode]
 fn = lambda: m.mmfs_sampler_forward(value, shapes, starts, qproj, rtable, relpos, ref, scale, n_lvl, P, **kw)
 for _ in range(3):
     fn()
@@ -50,4 +46,4 @@ for _ in range(reps):
     ts.append(e0.elapsed_time(e1))
 t = sorted(ts)[len(ts) // 2] * 1e-3
 ab = msda_algorithmic_bytes(B, n_img * 1344, M, D, 12, Lq, P, 2)
-print(f"fused sampler B={B} masked={masked} mode={mode} rpw={rpw}: {t * 1e6:.1f} us  {ab / t / 1e9:.0f} GB/s (sec. 8d bytes)  visible frac {cross.mean().item():.2f}  out {out.float().abs().mean().item():.4f}")
+print(f"fused sampler B={B} masked={masked} mode={mode}: {t * 1e6:.1f} us  {ab / t / 1e9:.0f} GB/s (sec. 8d bytes)  visible frac {cross.mean().item():.2f}  out {out.float().abs().mean().item():.4f}")

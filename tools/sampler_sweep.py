@@ -1,6 +1,5 @@
 """Fused MMFS sampler on the cfg-3 layer shape (B = 4 sequences, 2048 tokens, 4 images): generic kernel vs the
-specialised kernel (fp32 / 16-bit tap weights) over rows-per-warp settings; CUDA events, L2 flushed between runs,
-median of `reps`.  Prints one line per setting and a final JSON list."""
+specialised kernel (fp32 / 16-bit tap weights); CUDA events, L2 flushed between runs, median of `reps`.  Prints one line per setting and a final JSON list."""
 import json
 import os
 import sys
@@ -13,7 +12,6 @@ import mm_interleaved_b200 as m  # noqa: E402
 from benchmarks.workloads import InterleavedCfg3, msda_algorithmic_bytes  # noqa: E402
 from mm_interleaved_b200.mm_interleaved import cross_attention_mask_from_ids  # noqa: E402
 from mm_interleaved_b200.mmfs import _relative_image_index  # noqa: E402
-from mm_interleaved_b200.sampler import set_sampler_tuning  # noqa: E402
 
 reps = int(sys.argv[1]) if len(sys.argv) > 1 else 20
 B = 4
@@ -38,26 +36,21 @@ rows = []
 for masked in (True, False):
     cross = cross_attention_mask_from_ids(ids, n_img, 1, wl.SOI_ID) if masked else torch.ones((B, Lq, n_img), device="cuda")
     relpos = _relative_image_index(cross, Lq)
-    for mode, rpws in (("generic", (0,)), ("generic_w16", (0,)), ("exact", (0,)), ("exact_occ4", (0,)), ("v2", (0, 1, 2, 4, 8)),
-                       ("v2_occ4", (0, 1, 2, 4, 8))):
-        kw = dict(v2={}, v2_occ4={}, exact=dict(exact_weights=True), exact_occ4=dict(exact_weights=True), generic=dict(generic=True),
-                  generic_w16=dict(generic=True, w16=True))[mode]
-        for rpw in rpws:
-            set_sampler_tuning(rpw, 1, 4 if mode.endswith("occ4") else 3)
-            fn = lambda: m.mmfs_sampler_forward(value, shapes, starts, qproj, rtable, relpos, ref, scale, n_lvl, P, **kw)
-            for _ in range(3):
-                fn()
-            ts = []
-            for _ in range(reps):
-                flush.zero_()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(); out = fn(); e1.record()
-                torch.cuda.synchronize()
-                ts.append(e0.elapsed_time(e1))
-            t = sorted(ts)[len(ts) // 2] * 1e-3
-            row = dict(masked=masked, visible_frac=round(float(cross.mean()), 3), mode=mode, rows_per_warp=rpw,
-                       us=round(t * 1e6, 1), gbs_8d=round(ab / t / 1e9, 1), frac_hbm=round(ab / t / 1e9 / 6584.5, 4))
-            rows.append(row)
-            print(row, flush=True)
-set_sampler_tuning(0, 1, 3)
+    for mode in ("generic", "exact", "v2"):
+        kw = dict(v2={}, exact=dict(exact_weights=True), generic=dict(generic=True))[mode]
+        fn = lambda: m.mmfs_sampler_forward(value, shapes, starts, qproj, rtable, relpos, ref, scale, n_lvl, P, **kw)
+        for _ in range(3):
+            fn()
+        ts = []
+        for _ in range(reps):
+            flush.zero_()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(); out = fn(); e1.record()
+            torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1))
+        t = sorted(ts)[len(ts) // 2] * 1e-3
+        row = dict(masked=masked, visible_frac=round(float(cross.mean()), 3), mode=mode,
+                   us=round(t * 1e6, 1), gbs_8d=round(ab / t / 1e9, 1), frac_hbm=round(ab / t / 1e9 / 6584.5, 4))
+        rows.append(row)
+        print(row, flush=True)
 print(json.dumps(rows))
