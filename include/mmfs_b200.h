@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define MMFS_B200_ABI_VERSION 2
+#define MMFS_B200_ABI_VERSION 3
 
 /* status codes */
 #define MMFS_OK            0
@@ -224,20 +224,15 @@ int mmfs_attn_decode(const void *q, const void *k, const void *v, void *out, con
  * those cases to mmfs_attn_generic).  Replaces LlamaAttention.forward's eager attention
  * (decoders/modeling_llama_mmfs.py:246-264), CLIPXAttention.forward's xformers call
  * (encoders/vit_adapter/xattn.py:70-72) and the SD-UNet attention (decoders/sd.py:64-65).
+ * With more (batch, query tile, head) items than resident CTAs (1 per SM at hd 128, 2 at hd 64) the kernel runs
+ * PERSISTENT: the resident CTAs walk the items handed out by an atomic counter, with barriers and tensor maps set up
+ * once and the K / V ring running on across items.  work_counter: one device uint32 of scratch, private to the call
+ * until it completes; the call zeroes it on `stream` when it runs persistent (the caller need not).
  */
 int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
                       int B, int H, int Tq, int Tkv, int hd,
                       long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
-                      float scale, int causal, int past, int dtype, void *stream);
-
-/* The same op as a PERSISTENT kernel: the resident CTAs (1 per SM at hd 128, 2 at hd 64) walk the (batch, query tile,
- * head) items handed out by an atomic counter, with barriers and tensor maps set up once and the K / V ring running on
- * across items.  Taken when there are more items than resident CTAs (else the call runs the kernel above).
- * work_counter: one device uint32 that is ZERO when the kernel starts and private to the call until it completes. */
-int mmfs_attn_forward_persistent(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
-                                 int B, int H, int Tq, int Tkv, int hd,
-                                 long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
-                                 float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream);
+                      float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream);
 
 /*
  * 2-D convolution as an implicit GEMM on the tensor cores (wgmma, TMA-shifted input boxes, no im2col buffer).

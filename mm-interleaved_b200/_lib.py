@@ -45,8 +45,7 @@ SIGNATURES = {
     "mmfs_conv2d_nhwc": (_I, [_P] * 6 + [_I] * 10 + [_P]),
     "mmfs_attn_decode_scratch_floats": (_L, [_I] * 4),
     "mmfs_attn_decode": (_I, [_P] * 6 + [_I] * 4 + [_L] * 6 + [_F, _I, _I, _I, _P]),
-    "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P]),
-    "mmfs_attn_forward_persistent": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
+    "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
 }
 
 
@@ -63,8 +62,8 @@ def lib() -> ctypes.CDLL:
             fn = getattr(handle, name)  # AttributeError if the ABI is incomplete
             fn.restype = res
             fn.argtypes = args
-        if handle.mmfs_abi_version() != 2:
-            raise RuntimeError(f"libmmfs_b200.so ABI {handle.mmfs_abi_version()} != 2")
+        if handle.mmfs_abi_version() != 3:
+            raise RuntimeError(f"libmmfs_b200.so ABI {handle.mmfs_abi_version()} != 3")
         _lib = handle
     return _lib
 

@@ -286,24 +286,21 @@ static int make_map_uncached(CUtensorMap *map, const void *ptr, int dtype, int B
 }
 
 template <typename T, int HD>
-static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const AttnParams &p, unsigned *sched,
-                       cudaStream_t st) {
-    const int dev = current_device();
+static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const AttnParams &p,
+                       unsigned *work_counter, cudaStream_t st) {
     const int n_q = (p.Tq + kBM - 1) / kBM;
     const long n_work = (long)n_q * p.H * p.B;
     if (n_work >= (1L << 30)) { set_error("attn_forward: %ld work items", n_work); return MMFS_EUNSUPPORTED; }
     constexpr size_t smem = (size_t)(HD / 64) * (kBM * 128 + 4 * kBN * 128) + 14 * 8 + 2 * sizeof(int);
-    auto kern = attn_fwd_kernel<T, HD>;
-    static bool attr_set[kMaxDevices] = {};          // the attribute is per device
-    if (dev < 0 || dev >= kMaxDevices || !attr_set[dev]) {
-        MMFS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev >= 0 && dev < kMaxDevices) attr_set[dev] = true;
-    }
-    // more items than resident CTAs: persistent, otherwise one item per CTA
+    constexpr auto kern = attn_fwd_kernel<T, HD>;
+    const int rc = ensure_dynamic_smem<kern>(smem);
+    if (rc != MMFS_OK) return rc;
+    // more items than resident CTAs: persistent over the items the zeroed counter hands out, otherwise one item per CTA
     const int resident = attn_ctas_per_sm<HD>() * num_sms();
-    const bool persistent = sched != nullptr && n_work > resident;
+    const bool persistent = n_work > resident;
+    if (persistent) MMFS_CUDA(cudaMemsetAsync(work_counter, 0, sizeof(unsigned), st));
     const int grid = persistent ? resident : (int)n_work;
-    kern<<<grid, kAttnThreads, smem, st>>>(mq, mk, mv, p, persistent ? sched : nullptr, (int)n_work);
+    kern<<<grid, kAttnThreads, smem, st>>>(mq, mk, mv, p, persistent ? work_counter : nullptr, (int)n_work);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -312,13 +309,14 @@ static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUten
 
 using namespace mmfs;
 
-static int attn_forward_impl(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
-                             int B, int H, int Tq, int Tkv, int hd,
-                             long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
-                             float scale, int causal, int past, int dtype, unsigned *sched, void *stream) {
+extern "C" int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
+                                 int B, int H, int Tq, int Tkv, int hd,
+                                 long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
+                                 float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream) {
     MMFS_CHECK_ARG(B >= 0 && H > 0 && Tq >= 0 && Tkv > 0, "attn_forward: bad shape");
     if (B == 0 || Tq == 0) return MMFS_OK;
-    MMFS_CHECK_ARG(q && k && v && out, "attn_forward: null pointer argument");
+    MMFS_CHECK_ARG(q && k && v && out && work_counter, "attn_forward: null pointer argument");
+    MMFS_CHECK_ARG((uintptr_t)work_counter % 4 == 0, "attn_forward: work_counter must be 4-byte aligned");
     if (!(hd == 64 || hd == 128) || !(dtype == MMFS_BF16 || dtype == MMFS_F16)) {
         set_error("attn_forward: tensor-core path needs hd in {64,128} and bf16/f16 (got hd=%d dtype=%d)", hd, dtype);
         return MMFS_EUNSUPPORTED;
@@ -337,24 +335,8 @@ static int attn_forward_impl(const void *q, const void *k, const void *v, void *
     p.out = out; p.key_mask = key_mask; p.B = B; p.H = H; p.Tq = Tq; p.Tkv = Tkv; p.causal = causal; p.past = past;
     p.o_bs = o_bs; p.o_ts = o_ts; p.scale_log2e = scale * 1.4426950408889634f;
     cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == MMFS_BF16)
-        return hd == 64 ? launch_attn<__nv_bfloat16, 64>(mq, mk, mv, p, sched, st) : launch_attn<__nv_bfloat16, 128>(mq, mk, mv, p, sched, st);
-    return hd == 64 ? launch_attn<__half, 64>(mq, mk, mv, p, sched, st) : launch_attn<__half, 128>(mq, mk, mv, p, sched, st);
-}
-
-extern "C" int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
-                                 int B, int H, int Tq, int Tkv, int hd,
-                                 long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
-                                 float scale, int causal, int past, int dtype, void *stream) {
-    return attn_forward_impl(q, k, v, out, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts, scale, causal,
-                             past, dtype, nullptr, stream);
-}
-
-extern "C" int mmfs_attn_forward_persistent(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
-                                            int B, int H, int Tq, int Tkv, int hd,
-                                            long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
-                                            float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream) {
-    MMFS_CHECK_ARG(work_counter != nullptr && (uintptr_t)work_counter % 4 == 0, "attn_forward_persistent: work_counter must be a zeroed device uint32");
-    return attn_forward_impl(q, k, v, out, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts, scale, causal,
-                             past, dtype, work_counter, stream);
+    return dispatch_dtype<kF16Types>(dtype, "attn_forward", [&](auto tag) {
+        using T = typename decltype(tag)::type;
+        return hd == 64 ? launch_attn<T, 64>(mq, mk, mv, p, work_counter, st) : launch_attn<T, 128>(mq, mk, mv, p, work_counter, st);
+    });
 }

@@ -459,8 +459,7 @@ static int launch_attn_generic(const void *q, const void *k, const void *v, void
                                int B, int H, int Tq, int Tkv, int hd, long q_bs, long q_ts, long k_bs, long k_ts,
                                long v_bs, long v_ts, long o_bs, long o_ts, float scale, int causal, int past, cudaStream_t st) {
     const long n_rows = (long)B * H * Tq;
-    const long blocks = (n_rows + kAttnWarps - 1) / kAttnWarps;
-    const int grid = (int)(blocks < (long)num_sms() * 16 ? blocks : (long)num_sms() * 16);
+    const int grid = capped_grid((n_rows + kAttnWarps - 1) / kAttnWarps, 16);
     const size_t smem = (size_t)kAttnWarps * (hd + kAttnChunk) * sizeof(float);
     attn_generic_kernel<T><<<grid, 32 * kAttnWarps, smem, st>>>((const T *)q, (const T *)k, (const T *)v, (T *)out, key_mask,
                                                               n_rows, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts,
@@ -481,12 +480,10 @@ extern "C" int mmfs_attn_generic(const void *q, const void *k, const void *v, vo
     if (B == 0 || Tq == 0) return MMFS_OK;
     MMFS_CHECK_ARG(q && k && v && out, "attn_generic: null pointer argument");
     cudaStream_t st = (cudaStream_t)stream;
-    switch (dtype) {
-        case MMFS_F32: return launch_attn_generic<float>(q, k, v, out, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts, scale, causal, past, st);
-        case MMFS_F16: return launch_attn_generic<__half>(q, k, v, out, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts, scale, causal, past, st);
-        case MMFS_BF16: return launch_attn_generic<__nv_bfloat16>(q, k, v, out, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts, scale, causal, past, st);
-        default: set_error("attn_generic: dtype %d unsupported", dtype); return MMFS_EINVAL;
-    }
+    return dispatch_dtype<kF32Types>(dtype, "attn_generic", [&](auto tag) {
+        return launch_attn_generic<typename decltype(tag)::type>(q, k, v, out, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts,
+                                                                 v_bs, v_ts, o_bs, o_ts, scale, causal, past, st);
+    });
 }
 
 extern "C" long mmfs_attn_decode_scratch_floats(int B, int H, int Tkv, int hd) {
@@ -510,9 +507,8 @@ extern "C" int mmfs_attn_decode(const void *q, const void *k, const void *v, voi
     const int last_key = causal ? (past < Tkv - 1 ? past : Tkv - 1) : Tkv - 1;     // the single query row sits at position `past`
     MMFS_CHECK_ARG(last_key >= 0, "attn_decode: negative past");
     cudaStream_t st = (cudaStream_t)stream;
-    switch (dtype) {
-        case MMFS_F32: return launch_attn_decode<float>(q, k, v, out, key_mask, scratch, B, H, Tkv, hd, q_bs, k_bs, k_ts, v_bs, v_ts, o_bs, scale, last_key, st);
-        case MMFS_F16: return launch_attn_decode<__half>(q, k, v, out, key_mask, scratch, B, H, Tkv, hd, q_bs, k_bs, k_ts, v_bs, v_ts, o_bs, scale, last_key, st);
-        default: return launch_attn_decode<__nv_bfloat16>(q, k, v, out, key_mask, scratch, B, H, Tkv, hd, q_bs, k_bs, k_ts, v_bs, v_ts, o_bs, scale, last_key, st);
-    }
+    return dispatch_dtype<kF32Types>(dtype, "attn_decode", [&](auto tag) {
+        return launch_attn_decode<typename decltype(tag)::type>(q, k, v, out, key_mask, scratch, B, H, Tkv, hd, q_bs, k_bs, k_ts,
+                                                                v_bs, v_ts, o_bs, scale, last_key, st);
+    });
 }

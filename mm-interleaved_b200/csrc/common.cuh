@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../../include/mmfs_b200.h"
 
 namespace mmfs {
@@ -41,6 +43,47 @@ inline size_t dtype_size(int dtype) {
 int num_sms();            // of the CURRENT device
 int current_device();     // cudaGetDevice, -1 on failure
 constexpr int kMaxDevices = 64;
+
+// ---- launch policy shared by the entry points -------------------------------------------------------------------
+// Element-type dispatch: returns f(DtypeTag<T>{}) for the element type T of `dtype` when the code is in the set
+// Accepted (bits 1 << MMFS_*); only the accepted types are instantiated.  Any other code sets
+// "<what>: dtype <code> unsupported" and returns Bad.
+template <typename T> struct DtypeTag { using type = T; };
+constexpr unsigned kF16Types = (1u << MMFS_F16) | (1u << MMFS_BF16);
+constexpr unsigned kF32Types = (1u << MMFS_F32) | kF16Types;
+constexpr unsigned kAllTypes = kF32Types | (1u << MMFS_F64);
+
+template <unsigned Accepted, int Bad = MMFS_EINVAL, typename F>
+int dispatch_dtype(int dtype, const char *what, F &&f) {
+    switch (dtype) {
+        case MMFS_F32: if constexpr ((Accepted >> MMFS_F32) & 1u) return f(DtypeTag<float>{}); break;
+        case MMFS_F16: if constexpr ((Accepted >> MMFS_F16) & 1u) return f(DtypeTag<__half>{}); break;
+        case MMFS_BF16: if constexpr ((Accepted >> MMFS_BF16) & 1u) return f(DtypeTag<__nv_bfloat16>{}); break;
+        case MMFS_F64: if constexpr ((Accepted >> MMFS_F64) & 1u) return f(DtypeTag<double>{}); break;
+    }
+    set_error("%s: dtype %d unsupported", what, dtype);
+    return Bad;
+}
+
+// Opts Kernel in to `bytes` of dynamic shared memory on the current device.  The attribute is per kernel and per
+// device and is only ever raised: sizes within the 48 KiB default or within what was set before make no driver call.
+template <auto Kernel>
+int ensure_dynamic_smem(size_t bytes) {
+    static size_t set[kMaxDevices] = {};
+    if (bytes <= 48 * 1024) return MMFS_OK;
+    const int dev = current_device();
+    const bool tracked = dev >= 0 && dev < kMaxDevices;
+    if (tracked && bytes <= set[dev]) return MMFS_OK;
+    MMFS_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    if (tracked) set[dev] = bytes;
+    return MMFS_OK;
+}
+
+// Grid of a grid-stride kernel: `blocks`, capped at per_sm CTAs per SM of the current device.
+inline int capped_grid(long blocks, int per_sm) {
+    const long cap = (long)num_sms() * per_sm;
+    return (int)(blocks < cap ? blocks : cap);
+}
 
 // ---- element <-> opmath conversions ---------------------------------------------------
 template <typename T> struct OpMath { using type = float; };
@@ -133,6 +176,33 @@ __device__ __forceinline__ uint16_t ldg_stream_u16(const void *p) {
 }
 __device__ __forceinline__ void stg_v4(void *p, const uint4 &v) {
     asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+
+// ---- mbarrier and bulk async copy (TMA engine) --------------------------------------------------------------------
+__device__ __forceinline__ uint32_t s_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+__device__ __forceinline__ void bar_init(uint64_t *bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s_addr(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void bar_expect_tx(uint64_t *bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s_addr(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bar_arrive(uint64_t *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_addr(bar)) : "memory");
+}
+__device__ __forceinline__ void bar_wait(uint64_t *bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "W_%=:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra D_%=;\n\t"
+        "bra W_%=;\n\t"
+        "D_%=:\n\t}" ::"r"(s_addr(bar)), "r"(parity) : "memory");
+}
+// `bytes` (a multiple of 16) from global to shared memory, completing on `bar`
+__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::
+                 "r"(s_addr(dst)), "l"(src), "r"(bytes), "r"(s_addr(bar)) : "memory");
 }
 
 }  // namespace mmfs

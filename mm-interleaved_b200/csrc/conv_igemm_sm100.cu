@@ -190,23 +190,12 @@ extern "C" int mmfs_conv2d_nhwc(const void *x, const void *w, const void *bias, 
     const size_t smem = (size_t)kConvStages * (128 * 128 + kConvBN * 128) + 2 * kConvStages * 8;
     dim3 grid((unsigned)(p.tiles_w * p.tiles_h * (B / TB)), (unsigned)(Cout / kConvBN));
     cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == MMFS_BF16) {
-        static bool attr[kMaxDevices] = {};            // the attribute is per device
-        const int dev = current_device();
-        if (dev < 0 || dev >= kMaxDevices || !attr[dev]) {
-            MMFS_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            if (dev >= 0 && dev < kMaxDevices) attr[dev] = true;
-        }
-        conv_igemm_kernel<__nv_bfloat16><<<grid, kConvThreads, smem, st>>>(mx, mw, p);
-    } else {
-        static bool attr[kMaxDevices] = {};
-        const int dev = current_device();
-        if (dev < 0 || dev >= kMaxDevices || !attr[dev]) {
-            MMFS_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            if (dev >= 0 && dev < kMaxDevices) attr[dev] = true;
-        }
-        conv_igemm_kernel<__half><<<grid, kConvThreads, smem, st>>>(mx, mw, p);
-    }
-    MMFS_CUDA(cudaGetLastError());
-    return MMFS_OK;
+    return dispatch_dtype<kF16Types>(dtype, "conv2d_nhwc", [&](auto tag) {
+        constexpr auto kern = conv_igemm_kernel<typename decltype(tag)::type>;
+        const int rc = ensure_dynamic_smem<kern>(smem);
+        if (rc != MMFS_OK) return rc;
+        kern<<<grid, kConvThreads, smem, st>>>(mx, mw, p);
+        MMFS_CUDA(cudaGetLastError());
+        return MMFS_OK;
+    });
 }

@@ -154,8 +154,9 @@ static int gn_launch(const void *x, const void *gamma, const void *beta, void *y
     ppb = min(ppb, HW);
     const int chunks = (HW + ppb - 1) / ppb;             // <= kGnMaxChunks
     const size_t smem_stats = (size_t)lanes * C * 2 * sizeof(float);
-    auto kern = gn_stats_kernel<T>;
-    if (smem_stats > 48 * 1024) MMFS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_stats));
+    constexpr auto kern = gn_stats_kernel<T>;
+    const int rc = ensure_dynamic_smem<kern>(smem_stats);
+    if (rc != MMFS_OK) return rc;
     dim3 grid(chunks, B);
     kern<<<grid, threads, smem_stats, st>>>((const T *)x, stats, HW, C, G, ppb, cvecs, lanes);
     gn_apply_kernel<T><<<grid, threads, 2 * G * sizeof(float), st>>>((const T *)x, (const T *)gamma, (const T *)beta, stats, (T *)y,
@@ -177,9 +178,7 @@ extern "C" int mmfs_groupnorm_nhwc(const void *x, const void *gamma, const void 
         return MMFS_EUNSUPPORTED;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    switch (dtype) {
-        case MMFS_F32: return gn_launch<float>(x, gamma, beta, y, stats, B, HW, C, G, eps, silu, st);
-        case MMFS_F16: return gn_launch<__half>(x, gamma, beta, y, stats, B, HW, C, G, eps, silu, st);
-        default: return gn_launch<__nv_bfloat16>(x, gamma, beta, y, stats, B, HW, C, G, eps, silu, st);
-    }
+    return dispatch_dtype<kF32Types>(dtype, "groupnorm", [&](auto tag) {
+        return gn_launch<typename decltype(tag)::type>(x, gamma, beta, y, stats, B, HW, C, G, eps, silu, st);
+    });
 }

@@ -354,65 +354,71 @@ __global__ void __launch_bounds__(256) swiglu_kernel(const T *__restrict__ gu, T
 }
 
 template <typename T>
-static int launch_all(int which, const void *a, const void *b, const void *c, void *d, const void *e, const void *f,
-                      long n0, int i0, int i1, int i2, int i3, int i4, int i5, float eps, cudaStream_t st) {
-    (void)i5;
-    switch (which) {
-        case 0:   // rmsnorm: a=x b=w d=y n0=rows i0=cols
-            if (i0 % (16 / (int)sizeof(T)) == 0 && i0 / (16 / (int)sizeof(T)) <= kRmsThreads * kRmsChunks)
-                rmsnorm_reg_kernel<T><<<(unsigned)n0, kRmsThreads, 0, st>>>((const T *)a, (const T *)b, (T *)d, i0, eps);
-            else
-                rmsnorm_kernel<T><<<(unsigned)n0, 256, 0, st>>>((const T *)a, (const T *)b, (T *)d, i0, eps);
-            break;
-        case 1: { // layernorm: a=x b=w c=bias d=y
-            constexpr int VEC = 16 / (int)sizeof(T);
-            const bool vec_ok = (i0 % VEC == 0) && (i0 / VEC <= 32 * kLnChunks) &&
-                                (((uintptr_t)a | (uintptr_t)d | (uintptr_t)b | (uintptr_t)c) % 16 == 0);
-            if (vec_ok) {
-                const int nvec = i0 / VEC;
-                const unsigned grid = (unsigned)((n0 + 7) / 8);
-#define MMFS_LN(CH) layernorm_warp_kernel<T, CH><<<grid, 256, 0, st>>>((const T *)a, (const T *)b, (const T *)c, (T *)d, n0, i0, eps)
-                if (nvec <= 32) MMFS_LN(1); else if (nvec <= 64) MMFS_LN(2); else if (nvec <= 128) MMFS_LN(4); else MMFS_LN(8);
-#undef MMFS_LN
-            } else
-                layernorm_kernel<T><<<(unsigned)n0, 256, 0, st>>>((const T *)a, (const T *)b, (const T *)c, (T *)d, i0, eps);
-            break;
-        }
-        case 2: { // rope: d=q (in place), a=k (in place, cast away const), e=cos f=sin c=pos; n0=tokens i0=H i1=hd i2=q_stride i3=k_stride i4=pos_per_batch i5=T
-            const int per_tok = i0 * 2 * ((i1 / 2) / (16 / (int)sizeof(T)));
-            const int threads = per_tok >= 256 ? 256 : ((per_tok + 31) / 32) * 32;
-            const int grid = (int)(n0 < (long)num_sms() * 32 ? n0 : (long)num_sms() * 32);
-            rope_qk_kernel<T><<<grid, threads, 0, st>>>((T *)d, (T *)const_cast<void *>(a), (const float *)e, (const float *)f,
-                                                     (const int64_t *)c, n0, i0, i1, i2, i3, i4, i5);
-            break;
-        }
-        case 3: { // swiglu / geglu: a=gate_up d=out n0=rows i0=I i1=variant (0 silu [gate|up], 1 gelu [value|gate])
-            const int nvec = i0 / (16 / (int)sizeof(T));
-            const int threads = nvec >= 512 ? 256 : (nvec >= 64 ? 64 : 32);
-            const int gx = (int)(n0 < (long)num_sms() * 64 ? n0 : (long)num_sms() * 64);
-            int gy = 1;                                   // fewer CTAs than SMs: slice the columns (two vectors per thread)
-            if (gx < num_sms()) { gy = (nvec + 2 * threads - 1) / (2 * threads); if (gy > 64) gy = 64; if (gy < 1) gy = 1; }
-            const dim3 grid(gx, gy);
-            if (i1 == 1)
-                swiglu_kernel<T, 1, true><<<grid, threads, 0, st>>>((const T *)a, (T *)d, n0, i0);
-            else
-                swiglu_kernel<T, 0, false><<<grid, threads, 0, st>>>((const T *)a, (T *)d, n0, i0);
-            break;
-        }
-    }
+static int launch_rmsnorm(const void *x, const void *w, void *y, long rows, int cols, float eps, cudaStream_t st) {
+    if (cols % (16 / (int)sizeof(T)) == 0 && cols / (16 / (int)sizeof(T)) <= kRmsThreads * kRmsChunks)
+        rmsnorm_reg_kernel<T><<<(unsigned)rows, kRmsThreads, 0, st>>>((const T *)x, (const T *)w, (T *)y, cols, eps);
+    else
+        rmsnorm_kernel<T><<<(unsigned)rows, 256, 0, st>>>((const T *)x, (const T *)w, (T *)y, cols, eps);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
 
-static int dispatch(int dtype, int which, const void *a, const void *b, const void *c, void *d, const void *e, const void *f,
-                    long n0, int i0, int i1, int i2, int i3, int i4, int i5, float eps, void *stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    switch (dtype) {
-        case MMFS_F32: return launch_all<float>(which, a, b, c, d, e, f, n0, i0, i1, i2, i3, i4, i5, eps, st);
-        case MMFS_F16: return launch_all<__half>(which, a, b, c, d, e, f, n0, i0, i1, i2, i3, i4, i5, eps, st);
-        case MMFS_BF16: return launch_all<__nv_bfloat16>(which, a, b, c, d, e, f, n0, i0, i1, i2, i3, i4, i5, eps, st);
-        default: set_error("dtype %d not supported by this kernel", dtype); return MMFS_EINVAL;
-    }
+template <typename T>
+static int launch_layernorm(const void *x, const void *w, const void *b, void *y, long rows, int cols, float eps, cudaStream_t st) {
+    constexpr int VEC = 16 / (int)sizeof(T);
+    const bool vec_ok = (cols % VEC == 0) && (cols / VEC <= 32 * kLnChunks) &&
+                        (((uintptr_t)x | (uintptr_t)y | (uintptr_t)w | (uintptr_t)b) % 16 == 0);
+    if (vec_ok) {
+        const int nvec = cols / VEC;
+        const unsigned grid = (unsigned)((rows + 7) / 8);
+#define MMFS_LN(CH) layernorm_warp_kernel<T, CH><<<grid, 256, 0, st>>>((const T *)x, (const T *)w, (const T *)b, (T *)y, rows, cols, eps)
+        if (nvec <= 32) MMFS_LN(1); else if (nvec <= 64) MMFS_LN(2); else if (nvec <= 128) MMFS_LN(4); else MMFS_LN(8);
+#undef MMFS_LN
+    } else
+        layernorm_kernel<T><<<(unsigned)rows, 256, 0, st>>>((const T *)x, (const T *)w, (const T *)b, (T *)y, cols, eps);
+    MMFS_CUDA(cudaGetLastError());
+    return MMFS_OK;
+}
+
+template <typename T>
+static int launch_rope(void *q, void *k, const float *cos_t, const float *sin_t, const int64_t *pos, long n_tok, int T_len,
+                       int H, int hd, int qs, int ks, int ppb, cudaStream_t st) {
+    const int per_tok = H * 2 * ((hd / 2) / (16 / (int)sizeof(T)));
+    const int threads = per_tok >= 256 ? 256 : ((per_tok + 31) / 32) * 32;
+    rope_qk_kernel<T><<<capped_grid(n_tok, 32), threads, 0, st>>>((T *)q, (T *)k, cos_t, sin_t, pos, n_tok, H, hd, qs, ks, ppb,
+                                                                  T_len);
+    MMFS_CUDA(cudaGetLastError());
+    return MMFS_OK;
+}
+
+// swiglu: silu over [gate | up]; geglu: gelu over [value | gate]
+template <typename T>
+static int launch_glu(const void *in, void *out, long rows, int inter, bool geglu, cudaStream_t st) {
+    const int nvec = inter / (16 / (int)sizeof(T));
+    const int threads = nvec >= 512 ? 256 : (nvec >= 64 ? 64 : 32);
+    const int gx = capped_grid(rows, 64);
+    int gy = 1;                                   // fewer CTAs than SMs: slice the columns (two vectors per thread)
+    if (gx < num_sms()) { gy = (nvec + 2 * threads - 1) / (2 * threads); if (gy > 64) gy = 64; if (gy < 1) gy = 1; }
+    const dim3 grid(gx, gy);
+    if (geglu)
+        swiglu_kernel<T, 1, true><<<grid, threads, 0, st>>>((const T *)in, (T *)out, rows, inter);
+    else
+        swiglu_kernel<T, 0, false><<<grid, threads, 0, st>>>((const T *)in, (T *)out, rows, inter);
+    MMFS_CUDA(cudaGetLastError());
+    return MMFS_OK;
+}
+
+template <typename T>
+static int launch_rope_append(void *q, const void *k, const void *v, const float *cos_t, const float *sin_t, const int64_t *pos,
+                              void *kc, void *vc, const int64_t *slot_dev, long slot_host, long n_tok, int T_len, int H, int hd,
+                              int qs, int ks, int vs, long cbs, long cts, int ppb, cudaStream_t st) {
+    const int items = H * ((hd / 2) / (16 / (int)sizeof(T))) * 2 + H * hd / (16 / (int)sizeof(T));
+    const int threads = items >= 256 ? 256 : ((items + 31) / 32) * 32;
+    rope_append_kernel<T><<<capped_grid(n_tok, 32), threads, 0, st>>>((T *)q, (const T *)k, (const T *)v, cos_t, sin_t, pos, (T *)kc,
+                                                                      (T *)vc, slot_dev, slot_host, n_tok, H, hd, qs, ks, vs, cbs,
+                                                                      cts, ppb, T_len);
+    MMFS_CUDA(cudaGetLastError());
+    return MMFS_OK;
 }
 
 }  // namespace mmfs
@@ -425,7 +431,9 @@ extern "C" int mmfs_rmsnorm(const void *x, const void *weight, void *y, long row
     MMFS_CHECK_ARG(x && weight && y, "rmsnorm: null pointer argument");
     MMFS_CHECK_ARG(((uintptr_t)x | (uintptr_t)weight | (uintptr_t)y) % 16 == 0 && (cols * dtype_size(dtype)) % 16 == 0,
                    "rmsnorm: rows must be 16-byte aligned");
-    return dispatch(dtype, 0, x, weight, nullptr, y, nullptr, nullptr, rows, cols, 0, 0, 0, 0, 0, eps, stream);
+    return dispatch_dtype<kF32Types>(dtype, "rmsnorm", [&](auto tag) {
+        return launch_rmsnorm<typename decltype(tag)::type>(x, weight, y, rows, cols, eps, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int mmfs_layernorm(const void *x, const void *weight, const void *bias, void *y, long rows, int cols, float eps,
@@ -433,7 +441,9 @@ extern "C" int mmfs_layernorm(const void *x, const void *weight, const void *bia
     MMFS_CHECK_ARG(rows >= 0 && cols > 0, "layernorm: bad shape");
     if (rows == 0) return MMFS_OK;
     MMFS_CHECK_ARG(x && y, "layernorm: null pointer argument");
-    return dispatch(dtype, 1, x, weight, bias, y, nullptr, nullptr, rows, cols, 0, 0, 0, 0, 0, eps, stream);
+    return dispatch_dtype<kF32Types>(dtype, "layernorm", [&](auto tag) {
+        return launch_layernorm<typename decltype(tag)::type>(x, weight, bias, y, rows, cols, eps, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int mmfs_rope_qk(void *q, void *k, const float *cos_table, const float *sin_table, const int64_t *position_ids,
@@ -445,21 +455,10 @@ extern "C" int mmfs_rope_qk(void *q, void *k, const float *cos_table, const floa
     MMFS_CHECK_ARG((hd / 2) % (16 / (int)dtype_size(dtype)) == 0 && ((uintptr_t)q | (uintptr_t)k) % 16 == 0 &&
                    (q_stride * dtype_size(dtype)) % 16 == 0 && (k_stride * dtype_size(dtype)) % 16 == 0,
                    "rope_qk: head_dim/2 must be a multiple of the 16-byte vector and rows 16-byte aligned");
-    return dispatch(dtype, 2, k, nullptr, position_ids, q, cos_table, sin_table, n_tokens, H, hd, q_stride, k_stride,
-                    pos_per_batch, T_len, 0.f, stream);
-}
-
-template <typename T>
-static int launch_rope_append(void *q, const void *k, const void *v, const float *cos_t, const float *sin_t, const int64_t *pos,
-                              void *kc, void *vc, const int64_t *slot_dev, long slot_host, long n_tok, int T_len, int H, int hd,
-                              int qs, int ks, int vs, long cbs, long cts, int ppb, cudaStream_t st) {
-    const int items = H * ((hd / 2) / (16 / (int)sizeof(T))) * 2 + H * hd / (16 / (int)sizeof(T));
-    const int threads = items >= 256 ? 256 : ((items + 31) / 32) * 32;
-    const int grid = (int)(n_tok < (long)num_sms() * 32 ? n_tok : (long)num_sms() * 32);
-    rope_append_kernel<T><<<grid, threads, 0, st>>>((T *)q, (const T *)k, (const T *)v, cos_t, sin_t, pos, (T *)kc, (T *)vc, slot_dev,
-                                                 slot_host, n_tok, H, hd, qs, ks, vs, cbs, cts, ppb, T_len);
-    MMFS_CUDA(cudaGetLastError());
-    return MMFS_OK;
+    return dispatch_dtype<kF32Types>(dtype, "rope_qk", [&](auto tag) {
+        return launch_rope<typename decltype(tag)::type>(q, k, cos_table, sin_table, position_ids, n_tokens, T_len, H, hd, q_stride,
+                                                         k_stride, pos_per_batch, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int mmfs_rope_qk_append(void *q, const void *k, const void *v, const float *cos_table, const float *sin_table,
@@ -476,13 +475,11 @@ extern "C" int mmfs_rope_qk_append(void *q, const void *k, const void *v, const 
                        (q_stride * es) % 16 == 0 && (k_stride * es) % 16 == 0 && (v_stride * es) % 16 == 0 &&
                        (cache_bs * es) % 16 == 0 && (cache_ts * es) % 16 == 0,
                    "rope_qk_append: head_dim/2 must be a multiple of the 16-byte vector and all rows 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    switch (dtype) {
-        case MMFS_F32: return launch_rope_append<float>(q, k, v, cos_table, sin_table, position_ids, k_cache, v_cache, slot_dev, slot_host, n_tokens, T_len, H, hd, q_stride, k_stride, v_stride, cache_bs, cache_ts, pos_per_batch, st);
-        case MMFS_F16: return launch_rope_append<__half>(q, k, v, cos_table, sin_table, position_ids, k_cache, v_cache, slot_dev, slot_host, n_tokens, T_len, H, hd, q_stride, k_stride, v_stride, cache_bs, cache_ts, pos_per_batch, st);
-        case MMFS_BF16: return launch_rope_append<__nv_bfloat16>(q, k, v, cos_table, sin_table, position_ids, k_cache, v_cache, slot_dev, slot_host, n_tokens, T_len, H, hd, q_stride, k_stride, v_stride, cache_bs, cache_ts, pos_per_batch, st);
-        default: set_error("rope_qk_append: dtype %d unsupported", dtype); return MMFS_EINVAL;
-    }
+    return dispatch_dtype<kF32Types>(dtype, "rope_qk_append", [&](auto tag) {
+        return launch_rope_append<typename decltype(tag)::type>(q, k, v, cos_table, sin_table, position_ids, k_cache, v_cache,
+                                                                slot_dev, slot_host, n_tokens, T_len, H, hd, q_stride, k_stride,
+                                                                v_stride, cache_bs, cache_ts, pos_per_batch, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int mmfs_swiglu(const void *gate_up, void *out, long rows, int inter, int dtype, void *stream) {
@@ -491,7 +488,9 @@ extern "C" int mmfs_swiglu(const void *gate_up, void *out, long rows, int inter,
     MMFS_CHECK_ARG(gate_up && out, "swiglu: null pointer argument");
     MMFS_CHECK_ARG(((uintptr_t)gate_up | (uintptr_t)out) % 16 == 0 && (inter * dtype_size(dtype)) % 16 == 0,
                    "swiglu: rows must be 16-byte aligned");
-    return dispatch(dtype, 3, gate_up, nullptr, nullptr, out, nullptr, nullptr, rows, inter, 0, 0, 0, 0, 0, 0.f, stream);
+    return dispatch_dtype<kF32Types>(dtype, "swiglu", [&](auto tag) {
+        return launch_glu<typename decltype(tag)::type>(gate_up, out, rows, inter, false, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int mmfs_geglu(const void *value_gate, void *out, long rows, int inter, int dtype, void *stream) {
@@ -500,5 +499,7 @@ extern "C" int mmfs_geglu(const void *value_gate, void *out, long rows, int inte
     MMFS_CHECK_ARG(value_gate && out, "geglu: null pointer argument");
     MMFS_CHECK_ARG(((uintptr_t)value_gate | (uintptr_t)out) % 16 == 0 && (inter * dtype_size(dtype)) % 16 == 0,
                    "geglu: rows must be 16-byte aligned");
-    return dispatch(dtype, 3, value_gate, nullptr, nullptr, out, nullptr, nullptr, rows, inter, 1, 0, 0, 0, 0, 0.f, stream);
+    return dispatch_dtype<kF32Types>(dtype, "geglu", [&](auto tag) {
+        return launch_glu<typename decltype(tag)::type>(value_gate, out, rows, inter, true, (cudaStream_t)stream);
+    });
 }

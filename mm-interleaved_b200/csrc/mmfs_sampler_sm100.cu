@@ -232,27 +232,13 @@ static int launch_sampler(SamplerArgs a, int N, cudaStream_t st) {
     const size_t smem = (size_t)(L + (a.n_lvl + 3) / 4) * sizeof(int4) +
                         (size_t)kWarpsPerCta * (kTapsPerWarp * sizeof(Tap) + (size_t)(xs_elems + qs_elems) * 4 + 256);
     if (smem > 200 * 1024) { set_error("mmfs_sampler: n_img*n_lvl*P = %d too large", L * a.P); return MMFS_EUNSUPPORTED; }
-    auto kern = mmfs_sampler_kernel<T, D, EMIT>;
-    static size_t smem_set[kMaxDevices] = {};  // per instantiation and per device
-    const int dev = current_device();
-    if (smem > 48 * 1024 && (dev < 0 || dev >= kMaxDevices || smem > smem_set[dev])) {
-        MMFS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev >= 0 && dev < kMaxDevices) smem_set[dev] = smem;
-    }
-    int ctas_per_sm = 0;
-    MMFS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern, 32 * kWarpsPerCta, smem));
-    if (ctas_per_sm < 1) { set_error("mmfs_sampler: kernel does not fit on an SM"); return MMFS_EUNSUPPORTED; }
-    const int nsm = num_sms();
-    int rpw = 8;
-    while (rpw > 1 && (long)N * a.M * ((a.Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw)) < 2L * nsm * ctas_per_sm) rpw >>= 1;
-    a.rows_per_warp = rpw;
-    a.qtiles = (a.Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw);
-    a.ntiles = (long)N * a.M * a.qtiles;
-    if (a.ntiles > 0x3fffffffL) { set_error("mmfs_sampler: too many tiles"); return MMFS_EUNSUPPORTED; }
-    a.ctas_per_sm = ctas_per_sm; a.nsm = nsm;
-    const long full = (long)nsm * ctas_per_sm;
-    const unsigned grid = (unsigned)(a.ntiles < full ? a.ntiles : full);
-    kern<<<grid, 32 * kWarpsPerCta, smem, st>>>(a);
+    constexpr auto kern = mmfs_sampler_kernel<T, D, EMIT>;
+    int rc = ensure_dynamic_smem<kern>(smem);
+    if (rc != MMFS_OK) return rc;
+    RowWalkPlan w;
+    if ((rc = plan_row_walk(kern, smem, (long)N * a.M, a.Lq, 8, "mmfs_sampler", w)) != MMFS_OK) return rc;
+    a.rows_per_warp = w.rows_per_warp; a.qtiles = w.qtiles; a.ntiles = w.ntiles; a.ctas_per_sm = w.ctas_per_sm; a.nsm = w.nsm;
+    kern<<<w.grid, 32 * kWarpsPerCta, smem, st>>>(a);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -309,11 +295,9 @@ static int sampler_entry(const void *value, const int64_t *shapes, const int64_t
         const int rc = launch_sampler_v2(a, N, D, dtype, st);
         if (rc != MMFS_EUNSUPPORTED) return rc;
     }
-    switch (dtype) {
-        case MMFS_F32: return dispatch_sampler<float>(a, N, D, emit, st);
-        case MMFS_F16: return dispatch_sampler<__half>(a, N, D, emit, st);
-        default: return dispatch_sampler<__nv_bfloat16>(a, N, D, emit, st);
-    }
+    return dispatch_dtype<kF32Types>(dtype, "mmfs_sampler", [&](auto tag) {
+        return dispatch_sampler<typename decltype(tag)::type>(a, N, D, emit, st);
+    });
 }
 
 extern "C" int mmfs_sampler_forward(const void *value, const int64_t *shapes, const int64_t *starts,

@@ -185,21 +185,14 @@ static int launch_bwd_impl(const void *value, const int64_t *shapes, const int64
     if ((P & (P - 1)) == 0) { p_shift = 0; while ((1 << p_shift) < P) ++p_shift; }
     const size_t per_warp = ((kTapsPerWarp * sizeof(Tap) + 4 * kDotStride * 4 + 16 + 15) / 16) * 16;
     const size_t smem = (size_t)L * sizeof(int4) + kWarpsPerCta * per_warp;
-    auto kern = msda_bwd_rows_kernel<T, D, DET>;
-    if (smem > 48 * 1024) MMFS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int ctas = 0;
-    MMFS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, kern, 32 * kWarpsPerCta, smem));
-    if (ctas < 1) { set_error("msda_backward: kernel does not fit"); return MMFS_EUNSUPPORTED; }
-    const int nsm = num_sms();
-    int rpw = 8;
-    while (rpw > 1 && (long)N * M * ((Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw)) < 2L * nsm * ctas) rpw >>= 1;
-    const int qtiles = (Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw);
-    const long ntiles = (long)N * M * qtiles;
-    if (ntiles > 0x3fffffffL) { set_error("msda_backward: too many tiles"); return MMFS_EUNSUPPORTED; }
-    const long full = (long)nsm * ctas;
-    kern<<<(unsigned)(ntiles < full ? ntiles : full), 32 * kWarpsPerCta, smem, st>>>(
+    constexpr auto kern = msda_bwd_rows_kernel<T, D, DET>;
+    int rc = ensure_dynamic_smem<kern>(smem);
+    if (rc != MMFS_OK) return rc;
+    RowWalkPlan w;
+    if ((rc = plan_row_walk(kern, smem, (long)N * M, Lq, 8, "msda_backward", w)) != MMFS_OK) return rc;
+    kern<<<w.grid, 32 * kWarpsPerCta, smem, st>>>(
         (const T *)value, shapes, starts, (const T *)loc, (const T *)attn, (const T *)grad_out, gv, gl, ga, fixed_scale,
-        S, M, L, Lq, P, p_shift, rpw, qtiles, ntiles, ctas, nsm);
+        S, M, L, Lq, P, p_shift, w.rows_per_warp, w.qtiles, w.ntiles, w.ctas_per_sm, w.nsm);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -232,12 +225,10 @@ using namespace mmfs;
 static int backward_entry(const void *value, const int64_t *shapes, const int64_t *starts, const void *loc, const void *attn,
                           const void *grad_out, void *grad_value, float *grad_loc, float *grad_attn, const float *fixed_scale,
                           int N, int S, int M, int D, int L, int Lq, int P, int dtype, cudaStream_t st) {
-    switch (dtype) {
-        case MMFS_F32: return dispatch_bwd<float>(D, value, shapes, starts, loc, attn, grad_out, grad_value, grad_loc, grad_attn, fixed_scale, N, S, M, L, Lq, P, st);
-        case MMFS_F16: return dispatch_bwd<__half>(D, value, shapes, starts, loc, attn, grad_out, grad_value, grad_loc, grad_attn, fixed_scale, N, S, M, L, Lq, P, st);
-        case MMFS_BF16: return dispatch_bwd<__nv_bfloat16>(D, value, shapes, starts, loc, attn, grad_out, grad_value, grad_loc, grad_attn, fixed_scale, N, S, M, L, Lq, P, st);
-        default: set_error("msda_backward: dtype %d unsupported (f32/f16/bf16)", dtype); return MMFS_EUNSUPPORTED;
-    }
+    return dispatch_dtype<kF32Types, MMFS_EUNSUPPORTED>(dtype, "msda_backward", [&](auto tag) {
+        return dispatch_bwd<typename decltype(tag)::type>(D, value, shapes, starts, loc, attn, grad_out, grad_value, grad_loc,
+                                                          grad_attn, fixed_scale, N, S, M, L, Lq, P, st);
+    });
 }
 
 extern "C" int mmfs_msda_backward(const void *value, const int64_t *shapes, const int64_t *starts, const void *loc,
@@ -265,12 +256,12 @@ extern "C" int mmfs_msda_backward_deterministic(const void *value, const int64_t
     cudaStream_t st = (cudaStream_t)stream;
     const long n_go = (long)N * Lq * M * D, n_gv = (long)N * S * M * D;
     MMFS_CUDA(cudaMemsetAsync(scratch2, 0, 2 * sizeof(float), st));
-    absmax_kernel<<<(unsigned)((n_go + 1023) / 1024 < 1184 ? (n_go + 1023) / 1024 : 1184), 256, 0, st>>>(grad_out, n_go, dtype, reinterpret_cast<unsigned *>(scratch2));
+    absmax_kernel<<<capped_grid((n_go + 1023) / 1024, 8), 256, 0, st>>>(grad_out, n_go, dtype, reinterpret_cast<unsigned *>(scratch2));
     fixed_scale_kernel<<<1, 1, 0, st>>>(scratch2);
     const int rc = backward_entry(value, shapes, starts, loc, attn, grad_out, grad_value_fixed, grad_loc, grad_attn, scratch2,
                                   N, S, M, D, L, Lq, P, dtype, st);
     if (rc != MMFS_OK) return rc;
-    fixed_to_float_kernel<<<(unsigned)((n_gv + 1023) / 1024 < 2368 ? (n_gv + 1023) / 1024 : 2368), 256, 0, st>>>(grad_value_fixed, grad_value, n_gv, scratch2);
+    fixed_to_float_kernel<<<capped_grid((n_gv + 1023) / 1024, 16), 256, 0, st>>>(grad_value_fixed, grad_value, n_gv, scratch2);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }

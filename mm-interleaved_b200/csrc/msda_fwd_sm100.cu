@@ -56,8 +56,8 @@ msda_fwd_rows_kernel(const T *__restrict__ value, const int64_t *__restrict__ sh
     for (int l = threadIdx.x; l < L; l += blockDim.x)
         s_lvl[l] = make_int4((int)shapes[2 * l], (int)shapes[2 * l + 1], (int)starts[l], 0);
     if (lane == 0) {
-        mbar_init(&bar[0], 1);
-        mbar_init(&bar[1], 1);
+        bar_init(&bar[0], 1);
+        bar_init(&bar[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -79,7 +79,7 @@ msda_fwd_rows_kernel(const T *__restrict__ value, const int64_t *__restrict__ sh
         const T *asrc = attn + qm * (size_t)LP;
         if (bulk_ok) {   // bulk async copies (TMA engine): two instructions stage the whole row
             if (lane == 0) {
-                mbar_expect_tx(&bar[buf], loc_bytes + att_bytes);
+                bar_expect_tx(&bar[buf], loc_bytes + att_bytes);
                 bulk_g2s(dst, lsrc, loc_bytes, &bar[buf]);
                 bulk_g2s(dst + 2 * LP, asrc, att_bytes, &bar[buf]);
             }
@@ -100,7 +100,7 @@ msda_fwd_rows_kernel(const T *__restrict__ value, const int64_t *__restrict__ sh
         const int buf = n_staged & 1;
         const unsigned parity = (n_staged >> 1) & 1;
         if (nxt.ok) stage_row(nxt.b, nxt.m, nxt.q, buf ^ 1);
-        if (bulk_ok) mbar_wait(&bar[buf], parity); else __syncwarp();
+        if (bulk_ok) bar_wait(&bar[buf], parity); else __syncwarp();
         ++n_staged;
 
         const T *s_loc = stage + buf * stage_elems;
@@ -298,32 +298,19 @@ static int launch_rows(const void *value, const int64_t *shapes, const int64_t *
     const size_t smem = (size_t)L * sizeof(int4) +
                         (size_t)kWarpsPerCta * (16 + 2 * (size_t)stage_elems * sizeof(T) + kTapsPerWarp * sizeof(Tap));
     if (smem > 200 * 1024) { set_error("msda: L*P = %d too large for the staging buffers", LP); return MMFS_EUNSUPPORTED; }
-    auto kern = msda_fwd_rows_kernel<T, D>;
-    static size_t smem_set[kMaxDevices] = {};  // per (T, D) instantiation and per device
-    const int dev = current_device();
-    if (smem > 48 * 1024 && (dev < 0 || dev >= kMaxDevices || smem > smem_set[dev])) {
-        MMFS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev >= 0 && dev < kMaxDevices) smem_set[dev] = smem;
-    }
-    int ctas_per_sm = 0;
-    MMFS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern, 32 * kWarpsPerCta, smem));
-    if (ctas_per_sm < 1) { set_error("msda: kernel does not fit on an SM (smem %zu)", smem); return MMFS_EUNSUPPORTED; }
-    const int nsm = num_sms();
+    constexpr auto kern = msda_fwd_rows_kernel<T, D>;
+    int rc = ensure_dynamic_smem<kern>(smem);
+    if (rc != MMFS_OK) return rc;
     // rows per warp per tile: short tiles -- neighbouring q-tiles of one head still share the L1-resident value slab
     // through the per-SM tile swizzle, and short tiles balance the tail of the persistent grid.  Tiny problems
     // (decode, Lq = 1) use 1.
-    int rpw = 2;
-    while (rpw > 1 && (long)N * M * ((Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw)) < 2L * nsm * ctas_per_sm) rpw >>= 1;
-    const int qtiles = (Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw);
-    const long ntiles = (long)N * M * qtiles;
-    if (ntiles > 0x3fffffffL) { set_error("msda: too many tiles (%ld)", ntiles); return MMFS_EUNSUPPORTED; }
-    const long full = (long)nsm * ctas_per_sm;
-    const unsigned grid = (unsigned)(ntiles < full ? ntiles : full);
+    RowWalkPlan w;
+    if ((rc = plan_row_walk(kern, smem, (long)N * M, Lq, 2, "msda", w)) != MMFS_OK) return rc;
     const bool bulk_ok = ((uintptr_t)loc % 16 == 0) && ((uintptr_t)attn % 16 == 0) &&
                          ((2 * LP * sizeof(T)) % 16 == 0) && ((LP * sizeof(T)) % 16 == 0);
-    kern<<<grid, 32 * kWarpsPerCta, smem, st>>>(
-        (const T *)value, shapes, starts, (const T *)loc, (const T *)attn, (T *)out,
-        S, M, L, Lq, P, p_shift, flags, rpw, qtiles, ntiles, ctas_per_sm, nsm, stage_elems, bulk_ok ? 1 : 0);
+    kern<<<w.grid, 32 * kWarpsPerCta, smem, st>>>(
+        (const T *)value, shapes, starts, (const T *)loc, (const T *)attn, (T *)out, S, M, L, Lq, P, p_shift, flags,
+        w.rows_per_warp, w.qtiles, w.ntiles, w.ctas_per_sm, w.nsm, stage_elems, bulk_ok ? 1 : 0);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -333,8 +320,7 @@ static int launch_generic(const void *value, const int64_t *shapes, const int64_
                           const void *attn, void *out, int N, int S, int M, int D, int L, int Lq, int P,
                           unsigned flags, cudaStream_t st) {
     const long total = (long)N * Lq * M * D;
-    const long blocks = (total + 255) / 256;
-    const int grid = (int)(blocks < (long)num_sms() * 32 ? blocks : (long)num_sms() * 32);
+    const int grid = capped_grid((total + 255) / 256, 32);
     msda_fwd_generic_kernel<T><<<grid, 256, 0, st>>>((const T *)value, shapes, starts, (const T *)loc,
                                                        (const T *)attn, (T *)out, total, S, M, D, L, Lq, P, flags);
     MMFS_CUDA(cudaGetLastError());
@@ -351,8 +337,7 @@ static int dispatch_d(const void *value, const int64_t *shapes, const int64_t *s
     if (aligned16 && L * P <= kSmallLP && (D == 32 || D == 64 || D == 128)) {
         constexpr int VEC = 16 / (int)sizeof(T);
         const long total = (long)N * Lq * M * (D / VEC);
-        const long blocks = (total + 255) / 256;
-        const int grid = (int)(blocks < (long)num_sms() * 64 ? blocks : (long)num_sms() * 64);
+        const int grid = capped_grid((total + 255) / 256, 64);
         if (D == 32)
             msda_fwd_smallrow_kernel<T, 32><<<grid, 256, 0, st>>>((const T *)value, shapes, starts, (const T *)loc, (const T *)attn, (T *)out, total, S, M, L, Lq, P, flags);
         else if (D == 64)
@@ -400,13 +385,13 @@ extern "C" int mmfs_msda_forward(const void *value, const int64_t *shapes, const
     int rc = check_msda_args(value, shapes, starts, loc, attn, out, N, S, M, D, L, Lq, P, dtype);
     if (rc != MMFS_OK || N == 0 || Lq == 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    switch (dtype) {
-        case MMFS_F32: return dispatch_d<float>(value, shapes, starts, loc, attn, out, N, S, M, D, L, Lq, P, flags, st);
-        case MMFS_F16: return dispatch_d<__half>(value, shapes, starts, loc, attn, out, N, S, M, D, L, Lq, P, flags, st);
-        case MMFS_BF16: return dispatch_d<__nv_bfloat16>(value, shapes, starts, loc, attn, out, N, S, M, D, L, Lq, P, flags, st);
-        case MMFS_F64: return launch_generic<double>(value, shapes, starts, loc, attn, out, N, S, M, D, L, Lq, P, flags, st);
-    }
-    return MMFS_EINVAL;
+    return dispatch_dtype<kAllTypes>(dtype, "msda", [&](auto tag) {
+        using T = typename decltype(tag)::type;
+        if constexpr (std::is_same_v<T, double>)   // f64 has only the generic kernel
+            return launch_generic<T>(value, shapes, starts, loc, attn, out, N, S, M, D, L, Lq, P, flags, st);
+        else
+            return dispatch_d<T>(value, shapes, starts, loc, attn, out, N, S, M, D, L, Lq, P, flags, st);
+    });
 }
 
 extern "C" int mmfs_msda_index_stream(const int64_t *shapes, const int64_t *starts, const void *loc,
@@ -419,13 +404,11 @@ extern "C" int mmfs_msda_index_stream(const int64_t *shapes, const int64_t *star
     if (total == 0) return MMFS_OK;
     MMFS_CHECK_ARG(shapes && starts && loc && idx, "msda_index_stream: null pointer argument");
     cudaStream_t st = (cudaStream_t)stream;
-    const long blocks = (total + 255) / 256;
-    const int grid = (int)(blocks < (long)num_sms() * 32 ? blocks : (long)num_sms() * 32);
-    switch (dtype) {
-        case MMFS_F32: msda_index_stream_kernel<float><<<grid, 256, 0, st>>>(shapes, starts, (const float *)loc, idx, total, M, D, L, P); break;
-        case MMFS_F16: msda_index_stream_kernel<__half><<<grid, 256, 0, st>>>(shapes, starts, (const __half *)loc, idx, total, M, D, L, P); break;
-        default: msda_index_stream_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(shapes, starts, (const __nv_bfloat16 *)loc, idx, total, M, D, L, P); break;
-    }
-    MMFS_CUDA(cudaGetLastError());
-    return MMFS_OK;
+    const int grid = capped_grid((total + 255) / 256, 32);
+    return dispatch_dtype<kF32Types>(dtype, "msda_index_stream", [&](auto tag) {
+        using T = typename decltype(tag)::type;
+        msda_index_stream_kernel<T><<<grid, 256, 0, st>>>(shapes, starts, (const T *)loc, idx, total, M, D, L, P);
+        MMFS_CUDA(cudaGetLastError());
+        return MMFS_OK;
+    });
 }

@@ -61,30 +61,6 @@ __device__ __forceinline__ void fma2(float &a0, float &a1, float w0, float w1, f
     a1 = __fmaf_rn(w1, v1, a1);
 }
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// mbarrier + bulk async copy (TMA engine, SASS UBLKCP): one instruction stages a whole
-// sampling-location / attention-weight row of the next output row into shared memory.
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::
-                 "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
 // 512 bytes of zeros: taps that must not contribute (outside the map, invalid corner, masked
 // image) are pointed here with weight 0, so the gather loop needs no predicates and a
 // non-finite `value` entry can never leak through a 0 * inf product.
@@ -228,6 +204,39 @@ struct RowWalk {
         return c;
     }
 };
+
+// Persistent grid of a RowWalk kernel over n_heads = N * M heads of Lq queries: one wave of the resident CTAs, at most
+// one per tile.  Rows per warp start at `rows_per_warp` and halve (down to 1) until every resident CTA gets two tiles,
+// which balances the tail of small problems.  MMFS_EUNSUPPORTED when the kernel does not fit on an SM or the tile count
+// exceeds 2^30; the error text is set only when `what` names the caller.
+struct RowWalkPlan {
+    int ctas_per_sm, nsm, rows_per_warp, qtiles;
+    long ntiles;
+    unsigned grid;
+};
+
+template <typename K>
+int plan_row_walk(K kernel, size_t smem, long n_heads, int Lq, int rows_per_warp, const char *what, RowWalkPlan &p) {
+    p.ctas_per_sm = 0;
+    MMFS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p.ctas_per_sm, kernel, 32 * kWarpsPerCta, smem));
+    if (p.ctas_per_sm < 1) {
+        if (what) set_error("%s: kernel does not fit on an SM (smem %zu)", what, smem);
+        return MMFS_EUNSUPPORTED;
+    }
+    p.nsm = num_sms();
+    const long full = (long)p.nsm * p.ctas_per_sm;
+    int rpw = rows_per_warp;
+    while (rpw > 1 && n_heads * ((Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw)) < 2 * full) rpw >>= 1;
+    p.rows_per_warp = rpw;
+    p.qtiles = (Lq + kWarpsPerCta * rpw - 1) / (kWarpsPerCta * rpw);
+    p.ntiles = n_heads * p.qtiles;
+    if (p.ntiles > 0x3fffffffL) {
+        if (what) set_error("%s: too many tiles (%ld)", what, p.ntiles);
+        return MMFS_EUNSUPPORTED;
+    }
+    p.grid = (unsigned)(p.ntiles < full ? p.ntiles : full);
+    return MMFS_OK;
+}
 
 // ------------------------------------------------------------------------------------
 // Fused MMFS sampler: argument block + small numeric helpers shared by the generic kernel

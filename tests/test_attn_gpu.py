@@ -87,9 +87,10 @@ def test_unsupported_shapes_fall_to_the_bandwidth_kernel_and_errors_are_loud():
     q = torch.randn((1, 64, 2, 80), device=DEV, dtype=torch.bfloat16)
     assert not attn_tc.supported(q, q, q, 64, 64, 80)
     lib = _lib.lib()
+    counter = torch.empty((1,), dtype=torch.int32, device=DEV)
     rc = lib.mmfs_attn_forward(q.data_ptr(), q.data_ptr(), q.data_ptr(), q.data_ptr(), None, 1, 2, 64, 64, 80,
                                q.stride(0), q.stride(1), q.stride(0), q.stride(1), q.stride(0), q.stride(1), q.stride(0), q.stride(1),
-                               0.1, 0, 0, _lib.BF16, None)
+                               0.1, 0, 0, _lib.BF16, counter.data_ptr(), None)
     assert rc == _lib.EUNSUPPORTED
 
 

@@ -16,7 +16,7 @@ def header_symbols():
     return sorted(set(re.findall(r"\b(mmfs_[a-z0-9_]+)\s*\(", text)))
 
 
-def test_library_exports_every_declared_symbol_at_abi_2():
+def test_library_exports_every_declared_symbol_at_abi_3():
     from mm_interleaved_b200 import _lib
     lib = _lib.lib()
     syms = header_symbols()
@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol_at_abi_2():
     for s in syms:
         assert hasattr(lib, s), f"{s} declared in include/mmfs_b200.h but not exported"
         assert s in _lib.SIGNATURES, f"{s} has no ctypes signature"
-    assert lib.mmfs_abi_version() == 2
+    assert lib.mmfs_abi_version() == 3
 
 
 def test_msda_forward_argument_validation_without_gpu():
