@@ -240,11 +240,22 @@ int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, co
  * utils/monkey_patch/sd_unet_forward_monkey_patch.py:235-366; 3x3 stride 1/2 and 1x1, NHWC).
  *   x (B,H,W,Cin) NHWC; w (Cout,KH,KW,Cin); out (B,Ho,Wo,Cout) NHWC; optional fused epilogue terms: bias (Cout),
  *   add_bc (B,Cout) [the ResNet block's time-embedding projection], residual (like out).
- * Requires bf16/f16, Cin % 64 == 0, Cout % 160 == 0, stride <= 2, output tileable by 8x16 (or 8x8 with even B) pixel
- * patches: MMFS_EUNSUPPORTED otherwise (callers keep those few layers -- conv_in / conv_out -- on the library path).
+ * Requires bf16/f16, Cin % 64 == 0, Cout % 160 == 0 or Cout % 128 == 0, stride <= 2, output tileable by 8x16 (or 8x8
+ * with even B) pixel patches: MMFS_EUNSUPPORTED otherwise (callers keep those few layers -- conv_in / conv_out -- on the
+ * library path).
  */
 int mmfs_conv2d_nhwc(const void *x, const void *w, const void *bias, const void *add_bc, const void *residual, void *out,
                      int B, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dtype, void *stream);
+
+/*
+ * Nearest 2x upsample followed by a 3x3 / pad-1 convolution (diffusers' Upsample2D with use_conv), without the
+ * upsampled intermediate: each of the four output parities is a 2x2 convolution over the low-resolution input.
+ *   x (B,H,W,Cin) NHWC; w_phases (4,Cout,2,2,Cin): the 3x3 filter folded per parity p = 2*py + px (rows: py = 0 ->
+ *   {w0, w1+w2}, py = 1 -> {w0+w1, w2}; columns alike); bias (Cout) or NULL; out (B,2H,2W,Cout) NHWC.
+ * Same requirements as mmfs_conv2d_nhwc on (Cin, Cout, dtype, alignment), with the H x W grid tileable.
+ */
+int mmfs_conv2d_up2x_nhwc(const void *x, const void *w_phases, const void *bias, void *out, int B, int H, int W, int Cin,
+                          int Cout, int dtype, void *stream);
 
 /*
  * GroupNorm (+ SiLU when silu != 0) on NHWC activations: the nn.GroupNorm(32) in front of every UNet convolution

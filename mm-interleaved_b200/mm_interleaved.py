@@ -194,13 +194,14 @@ TextHead = TextDecoder   # round-1 name
 class StableDiffusion(nn.Module):
     """``StableDiffusion`` (decoders/sd.py:23-218) on this repo's modules: ``unet`` (SD-2.1-base UNet with the patched
     forward, unet_sd.py), ``mmfs_module`` (MMFSNet) and ``noise_scheduler`` (scheduler.py: DDPM on the SD-2.1-base
-    schedule, sd.py:48-50) -- same attribute / state-dict names as the reference.  The VAE is a diffusers object this
-    repository does not rebuild: ``vae_decode`` (a callable latents -> image in [-1, 1], e.g. ``AutoencoderKL.decode``)
-    may be attached; without it ``generate_images`` returns the denoised latents (the pipeline's
+    schedule, sd.py:48-50) -- same attribute / state-dict names as the reference.  ``vae`` (e.g. the SD-2.1 decoder
+    ``vae_sd.AutoencoderKL``) is registered as ``self.vae`` -- state-dict keys ``vae.*`` as in a reference checkpoint --
+    and ``vae_decode`` defaults to its ``decode``; any callable latents -> image in [-1, 1] may be given as
+    ``vae_decode`` instead.  Without either, ``generate_images`` returns the denoised latents (the pipeline's
     ``output_type="latent"`` result, sd.py:196-211)."""
 
     def __init__(self, unet=None, mmfs_module=None, image_size=512, base_seed=0, use_random_seed=False,
-                 noise_scheduler=None, vae_decode=None, vae_scaling_factor=0.18215, **unet_kwargs):
+                 noise_scheduler=None, vae_decode=None, vae_scaling_factor=0.18215, vae=None, **unet_kwargs):
         super().__init__()
         from . import unet_sd
         from .scheduler import DDPMScheduler, SD21_BASE_SCHEDULER
@@ -208,6 +209,9 @@ class StableDiffusion(nn.Module):
         self.mmfs_module = mmfs_module
         self.image_size, self.base_seed, self.use_random_seed = image_size, base_seed, use_random_seed
         self.noise_scheduler = noise_scheduler if noise_scheduler is not None else DDPMScheduler(**SD21_BASE_SCHEDULER)
+        self.vae = vae
+        if vae is not None and vae_decode is None:
+            vae_decode = vae.decode
         self.vae_decode, self.vae_scaling_factor = vae_decode, vae_scaling_factor
         self._unet_graphs = None        # enable_cuda_graphs(): {input shapes -> unet_sd.GraphedUNet}, kept across calls
 
@@ -256,11 +260,13 @@ class StableDiffusion(nn.Module):
 class ImageDecoder(nn.Module):
     """``ImageDecoder`` (decoders/decoder_image.py:9-156): ``perceiver_resampler`` (Q-Former, 77 queries of width 1024
     over the per-image LLM context), ``neg_prompt_embeds`` and ``decoder`` = ``StableDiffusion`` (UNet + MMFSNet +
-    scheduler).  State-dict names follow the reference (``decoder.unet.*``, ``decoder.mmfs_module.*``)."""
+    scheduler, and the VAE decoder when ``vae`` is given).  State-dict names follow the reference (``decoder.unet.*``,
+    ``decoder.mmfs_module.*``, ``decoder.vae.*``).  ``vae``: ``True`` builds the SD-2.1 decoder (vae_sd.py), a dict
+    builds ``vae_sd.AutoencoderKL(**vae)``, a module is used as it is; it applies when ``decoder`` is not given."""
 
     def __init__(self, perceiver_config=None, seq_len=77, embed_dim=1024, unet=None, mmfs_module=None, image_size=512,
                  base_seed=0, sd_base_seed=None, sd_use_random_seed=False, mmfs_input_channel=1024, mmfs_feat_levels=4,
-                 uncond_prob=0.1, decoder: Optional[nn.Module] = None, **_):
+                 uncond_prob=0.1, decoder: Optional[nn.Module] = None, vae=None, **_):
         super().__init__()
         from .visual_tokenizer import PerceiverResampler
         self.uncond_prob = uncond_prob
@@ -273,9 +279,12 @@ class ImageDecoder(nn.Module):
                 unet = unet_sd.UNet2DConditionModel()
                 mmfs_module = MMFSNet(mmfs_input_channel, tuple(unet.block_out_channels), 2,
                                       downsample_factor=512 // image_size, n_levels=mmfs_feat_levels)
+            if vae is True or isinstance(vae, dict):
+                from .vae_sd import AutoencoderKL
+                vae = AutoencoderKL(**(vae if isinstance(vae, dict) else {}))
             decoder = StableDiffusion(unet=unet, mmfs_module=mmfs_module, image_size=image_size,
                                       base_seed=base_seed if sd_base_seed is None else sd_base_seed,
-                                      use_random_seed=sd_use_random_seed)
+                                      use_random_seed=sd_use_random_seed, vae=None if vae is False else vae)
         self.decoder = decoder
 
     # round-1 attribute names
@@ -733,8 +742,9 @@ class MMInterleaved(InterleavedForward):
 
     Differences a caller can see: weights are not fetched by the constructor (``llm_model_path`` is only read for its
     ``config.json``; the reference's ``load_model_weights`` fills the parameters afterwards); ``forward`` computes the
-    text loss (and returns the logits) -- the image-decoder training loss needs the diffusers VAE and is not built;
-    ``generate_images`` returns latents as ``image`` unless a ``vae_decode`` callable is attached to
+    text loss (and returns the logits) -- the image-decoder training loss needs the VAE encoder and is not built;
+    ``generate_images`` returns latents as ``image`` unless the image decoder has a VAE (``image_decoder_config``
+    with ``vae=True`` builds the SD-2.1 decoder, vae_sd.py) or a ``vae_decode`` callable is attached to
     ``image_decoder.decoder``.  Extension keyword: ``llm_config`` (a ``LlamaMMFSConfig`` / dict) replaces
     ``llm_model_path``; ``max_num_image`` in a batch skips the one host sync on ``num_image_per_seq.max()``."""
 

@@ -190,7 +190,7 @@ def conv2d_supported(x: torch.Tensor, weight: torch.Tensor, stride: int, padding
     Cout, _, KH, KW = weight.shape
     Ho, Wo = (H + 2 * padding - KH) // stride + 1, (W + 2 * padding - KW) // stride + 1
     tile = (Wo % 16 == 0 and Ho % 8 == 0) or (Wo == 8 and Ho == 8 and B % 2 == 0)
-    return Cin % 64 == 0 and Cout % 160 == 0 and stride in (1, 2) and tile
+    return Cin % 64 == 0 and (Cout % 160 == 0 or Cout % 128 == 0) and stride in (1, 2) and tile
 
 
 def conv2d(x: torch.Tensor, weight_khwc: torch.Tensor, bias=None, stride: int = 1, padding: int = 0, add_bc=None,
@@ -215,6 +215,47 @@ def conv2d(x: torch.Tensor, weight_khwc: torch.Tensor, bias=None, stride: int = 
             add_bc.data_ptr() if add_bc is not None else None, residual.data_ptr() if residual is not None else None,
             out.data_ptr(), B, H, W, Cin, Cout, KH, KW, stride, padding, _DTYPE_CODE[x.dtype], _stream())
     _lib.check(rc, "conv2d")
+    launch_counter[0] += 1
+    return out
+
+
+def fold_up2x_weights(weight: torch.Tensor) -> torch.Tensor:
+    """A 3x3 filter (Cout, Cin, 3, 3) folded for ``conv2d_up2x``: (4, Cout, 2, 2, Cin), phase p = 2 py + px.
+
+    ``conv3x3(up2x(x), pad 1)`` at output pixel (2i + py, 2j + px) reads the low-resolution rows {i-1, i, i} (py = 0)
+    or {i, i, i+1} (py = 1), so along rows the taps fold to {w0, w1 + w2} at offsets {-1, 0} or {w0 + w1, w2} at
+    {0, +1}, and the same along columns.  Summed in fp32 (fp64 stays fp64) and rounded to the filter's dtype once."""
+    acc = torch.float64 if weight.dtype == torch.float64 else torch.float32
+    fold = torch.tensor([[[1, 0, 0], [0, 1, 1]], [[1, 1, 0], [0, 0, 1]]], dtype=acc, device=weight.device)   # (py, tap, k)
+    w = torch.einsum("pak,ockl,qbl->pqoabc", fold, weight.to(acc), fold)         # (py, px, Cout, 2, 2, Cin)
+    return w.reshape(4, *w.shape[2:]).to(weight.dtype).contiguous()
+
+
+def conv2d_up2x_supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
+    """Whether ``conv2d_up2x`` can take ``conv3x3(interpolate(x, 2, "nearest"))`` for this (B, Cin, H, W) input and
+    (Cout, Cin, 3, 3) filter."""
+    if x.dtype not in (torch.bfloat16, torch.float16) or not x.is_cuda or x.dim() != 4 or tuple(weight.shape[2:]) != (3, 3):
+        return False
+    B, Cin, H, W = x.shape
+    Cout = weight.shape[0]
+    tile = (W % 16 == 0 and H % 8 == 0) or (W == 8 and H == 8 and B % 2 == 0)
+    return Cin % 64 == 0 and (Cout % 160 == 0 or Cout % 128 == 0) and tile
+
+
+def conv2d_up2x(x: torch.Tensor, weight_phases: torch.Tensor, bias=None) -> torch.Tensor:
+    """Nearest 2x upsample + 3x3 / pad-1 convolution in one kernel (csrc/conv_igemm_sm100.cu, phase form): four 2x2
+    convolutions over the low-resolution input, the 4x-size upsampled tensor is never formed.  ``x`` (B, Cin, H, W)
+    channels_last; ``weight_phases`` from ``fold_up2x_weights``; returns (B, Cout, 2H, 2W) channels_last."""
+    B, Cin, H, W = x.shape
+    Cout = weight_phases.shape[1]
+    inference_only("conv2d_up2x", x, weight_phases, bias)
+    _require(x.is_contiguous(memory_format=torch.channels_last) and weight_phases.is_contiguous(), "conv2d_up2x: x must be channels_last")
+    _require(tuple(weight_phases.shape) == (4, Cout, 2, 2, Cin), "conv2d_up2x: weights must be (4, Cout, 2, 2, Cin)")
+    out = torch.empty((B, Cout, 2 * H, 2 * W), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+    with torch.cuda.device(x.device):
+        rc = _lib.lib().mmfs_conv2d_up2x_nhwc(x.data_ptr(), weight_phases.data_ptr(), bias.data_ptr() if bias is not None else None,
+                                              out.data_ptr(), B, H, W, Cin, Cout, _DTYPE_CODE[x.dtype], _stream())
+    _lib.check(rc, "conv2d_up2x")
     launch_counter[0] += 1
     return out
 

@@ -80,17 +80,20 @@ class TimestepEmbedding(nn.Module):
 
 
 class ResnetBlock2D(nn.Module):
+    """diffusers ``ResnetBlock2D``; ``temb_channels=None`` (the VAE decoder) has no ``time_emb_proj`` and no temb."""
+
     def __init__(self, in_channels, out_channels, temb_channels=1280, groups=32, eps=1e-5):
         super().__init__()
         self.norm1 = nn.GroupNorm(groups, in_channels, eps=eps)
         self.conv1 = nn.Conv2d(in_channels, out_channels, 3, padding=1)
-        self.time_emb_proj = nn.Linear(temb_channels, out_channels)
+        self.time_emb_proj = nn.Linear(temb_channels, out_channels) if temb_channels is not None else None
         self.norm2 = nn.GroupNorm(groups, out_channels, eps=eps)
         self.conv2 = nn.Conv2d(out_channels, out_channels, 3, padding=1)
         self.conv_shortcut = nn.Conv2d(in_channels, out_channels, 1) if in_channels != out_channels else None
 
-    def forward(self, x, temb):
-        h = _conv(self.conv1, _gn(self.norm1, x, True), add_bc=self.time_emb_proj(F.silu(temb)))
+    def forward(self, x, temb=None):
+        add = self.time_emb_proj(F.silu(temb)) if self.time_emb_proj is not None else None
+        h = _conv(self.conv1, _gn(self.norm1, x, True), add_bc=add)
         skip = x if self.conv_shortcut is None else _conv(self.conv_shortcut, x)
         return _conv(self.conv2, _gn(self.norm2, h, True), residual=skip)
 
