@@ -30,7 +30,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
-from ._cache import SourceCache
+from ._cache import SourceCache, WeightCache
 from .mmfs import MMFS
 
 
@@ -96,16 +96,11 @@ class _CatWeight:
 
     def __init__(self, *linears):
         self.linears = linears
-        self.key = None
-        self.weight = None
+        self._cache = WeightCache()
 
     def get(self):
-        key = tuple((l.weight.data_ptr(), l.weight._version, l.weight.dtype, l.weight.device) for l in self.linears)
-        if key != self.key:
-            with torch.no_grad():
-                self.weight = torch.cat([l.weight for l in self.linears], 0).contiguous()
-            self.key = key
-        return self.weight
+        ws = [l.weight for l in self.linears]
+        return self._cache.get(ws, lambda: torch.cat(ws, 0).contiguous())
 
 
 def _addmm_residual(residual, x, weight, inplace):
@@ -258,6 +253,7 @@ class LlamaMMFSAttention(nn.Module):
         self.norm1 = LlamaRMSNorm(config.hidden_size, eps=config.rms_norm_eps)
         self.norm2 = LlamaRMSNorm(self.vision_hidden_size, eps=config.rms_norm_eps)
         self._vision_cache = SourceCache()   # RMSNorm(vision features), identity-checked (see _cache.py)
+        self._gated = WeightCache()
         self._geom_cache = {}       # (device, n_img) -> (shapes, starts); (device, Lq) -> reference points
 
     def _geometry(self, device, n_img, hw, len_q):
@@ -277,12 +273,12 @@ class LlamaMMFSAttention(nn.Module):
 
     def _gated_output(self):
         """``output_proj`` pre-multiplied by tanh(gate) (:334 applies the gate to the block output), inference only."""
-        w, b, g = self.attn.output_proj.weight, self.attn.output_proj.bias, self.gate
-        key = (w.data_ptr(), w._version, b._version, g._version, w.dtype, w.device)
-        if getattr(self, "_gated", None) is None or self._gated[0] != key:
-            t = g.detach().float().tanh()
-            self._gated = (key, (w.detach().float() * t).to(w.dtype), (b.detach().float() * t).to(b.dtype))
-        return self._gated[1], self._gated[2]
+        w, b, g = ps = self.attn.output_proj.weight, self.attn.output_proj.bias, self.gate
+
+        def build():
+            t = g.float().tanh()
+            return (w.float() * t).to(w.dtype), (b.float() * t).to(b.dtype)
+        return self._gated.get(ps, build)
 
     def project_vision(self, vision_hidden_states):
         """value_proj(RMSNorm(vision)) as (B, n_img*hw, M, D): the image-only part of this layer (:353, mmfs.py:165-172)."""
@@ -298,13 +294,8 @@ class LlamaMMFSAttention(nn.Module):
         else:
             # RMSNorm(vision) depends only on the images: reuse it while the SAME tensor object is passed again (the
             # decode steps of one generate call); modeling_llama_mmfs.py:353 recomputes it per layer per token
-            w2 = self.norm2.weight
-            vextra = (w2.data_ptr(), w2._version)
-            v = None if torch.is_grad_enabled() else self._vision_cache.get(vision_hidden_states, vextra)
-            if v is None:
-                v = self.norm2(vision_hidden_states)
-                if not torch.is_grad_enabled():
-                    self._vision_cache.put(vision_hidden_states, v, vextra)
+            v = self._vision_cache.get_or_build((vision_hidden_states, self.norm2.weight),
+                                                lambda: self.norm2(vision_hidden_states), cache=not torch.is_grad_enabled())
             _, n_img, hw, _ = v.shape
         shapes, starts, ref = self._geometry(h.device, n_img, hw, h.shape[1])
         if not torch.is_grad_enabled():

@@ -15,6 +15,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from ._cache import WeightCache
 from .llama_mmfs import LlamaMMFSConfig, LlamaModel
 
 # special-token convention of the reference (mm_interleaved.py:33-39; custom_datasets/wds_utils.py:186-215 appends
@@ -150,25 +151,25 @@ class TextDecoder(nn.Module):
         self.orig_txt_vocab_size = orig_vocab_size
         self.head = nn.Linear(hidden_size, vocab_size, bias=True)
         self.head_new = nn.Linear(hidden_size, vocab_size - orig_vocab_size, bias=True)
+        self._fused_cache = WeightCache()
 
     _PAD = 128   # a vocabulary of 32002+ rows is not a multiple of 8: cuBLAS drops to an unaligned legacy kernel (5x slower)
 
     def _fused(self):
         """head + head_new folded into one matrix / bias, rows zero-padded to a multiple of 128 (inference only)."""
-        ps = (self.head.weight, self.head_new.weight, self.head.bias, self.head_new.bias)
-        key = tuple((w.data_ptr(), w._version, w.dtype, w.device) for w in ps)
-        if getattr(self, "_fused_cache", None) is None or self._fused_cache[0] != key:
-            V, C = self.head.weight.shape
-            Vp = (V + self._PAD - 1) // self._PAD * self._PAD
-            with torch.no_grad():
-                w = self.head.weight.new_zeros((Vp, C))
-                w[:V] = self.head.weight
-                w[self.orig_txt_vocab_size:V] += self.head_new.weight
-                b = self.head.bias.new_zeros((Vp,))
-                b[:V] = self.head.bias
-                b[self.orig_txt_vocab_size:V] += self.head_new.bias
-            self._fused_cache = (key, w, b)
-        return self._fused_cache[1], self._fused_cache[2]
+        head, new = self.head, self.head_new
+        return self._fused_cache.get((head.weight, new.weight, head.bias, new.bias), self._fold_heads)
+
+    def _fold_heads(self):
+        V, C = self.head.weight.shape
+        Vp = (V + self._PAD - 1) // self._PAD * self._PAD
+        w = self.head.weight.new_zeros((Vp, C))
+        w[:V] = self.head.weight
+        w[self.orig_txt_vocab_size:V] += self.head_new.weight
+        b = self.head.bias.new_zeros((Vp,))
+        b[:V] = self.head.bias
+        b[self.orig_txt_vocab_size:V] += self.head_new.bias
+        return w, b
 
     def logits(self, hidden_states):
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):

@@ -28,28 +28,20 @@ from torch import nn
 
 from . import msda as _msda
 from . import sampler as _sampler
-from ._cache import SourceCache
+from ._cache import SourceCache, WeightCache
 
 _FAST_HEAD_DIMS = (32, 64, 128)
 
 
-_RELPOS_CACHE = {}
+_relpos_cache = SourceCache()
 
 
 def relative_image_index(attention_mask: torch.Tensor, len_q: int) -> torch.Tensor:
     """uint8 (N, n_img, 1|Lq): newest visible image -> 1, older -> 2.., masked -> 0 (mmfs.py:154-163).
-    Every MMFS layer of a forward receives the same mask tensor, so the last result is kept (keyed on the
-    tensor's storage + version) instead of being recomputed per layer."""
-    key = (attention_mask.data_ptr(), attention_mask._version, tuple(attention_mask.shape), attention_mask.dtype,
-           attention_mask.device, len_q)
-    hit = _RELPOS_CACHE.get("last")
-    if hit is not None and hit[0] == key and hit[1]() is attention_mask:
-        return hit[2]
-    rel = _relative_image_index(attention_mask, len_q)
-    if not torch.is_grad_enabled() or not attention_mask.requires_grad:
-        import weakref
-        _RELPOS_CACHE["last"] = (key, weakref.ref(attention_mask), rel)
-    return rel
+    Every MMFS layer of a forward receives the same mask tensor, so the last result is kept instead of being
+    recomputed per layer."""
+    return _relpos_cache.get_or_build(attention_mask, lambda: _relative_image_index(attention_mask, len_q), len_q,
+                                      cache=not (torch.is_grad_enabled() and attention_mask.requires_grad))
 
 
 def _relative_image_index(attention_mask: torch.Tensor, len_q: int) -> torch.Tensor:
@@ -95,7 +87,8 @@ class MMFS(nn.Module):
         self.output_proj = nn.Linear(d_inner, d_out)
         self.query_relpos = nn.Embedding(max_num_image_per_seq, d_query)
         self._reset_parameters()
-        self._fused = None        # (versions, W_cat, b_cat, rtable)
+        self._fused = WeightCache()
+        self._ignore_nonzero = WeightCache()
         self._value_cache = SourceCache()  # value_proj(input_flatten), identity-checked (see _cache.py)
 
     def _reset_parameters(self):   # same initialisation scheme as mmfs.py:102-118
@@ -116,33 +109,28 @@ class MMFS(nn.Module):
     def _fused_weights(self):
         ps = (self.sampling_offsets.weight, self.sampling_offsets.bias, self.attention_weights.weight,
               self.attention_weights.bias, self.query_relpos.weight)
-        key = tuple((p.data_ptr(), p._version, p.dtype, p.device) for p in ps)
-        if self._fused is None or self._fused[0] != key:
-            with torch.no_grad():
-                w = torch.cat([ps[0], ps[2]], 0).contiguous()
-                b = torch.cat([ps[1], ps[3]], 0).contiguous()
-                rtable = F.linear(ps[4], w).contiguous()          # W @ relpos_embed[r], no bias
-            self._fused = (key, w, b, rtable)
-        return self._fused[1:]
+
+        def build():
+            w = torch.cat([ps[0], ps[2]], 0).contiguous()
+            b = torch.cat([ps[1], ps[3]], 0).contiguous()
+            return w, b, F.linear(ps[4], w).contiguous()          # W @ relpos_embed[r], no bias
+        return self._fused.get(ps, build)
+
+    def _needs_null_slot(self):
+        """Whether ``ignore_token`` has non-zero entries: one host sync per weight load, not per forward."""
+        return self._ignore_nonzero.get(self.ignore_token, lambda: bool(torch.count_nonzero(self.ignore_token)))
 
     def project_value(self, input_flatten, input_padding_mask=None, cache=True):
         """value_proj(input_flatten) as (N, n_img*hw, M, D), cached per input tensor (mmfs.py:165-172).  ``cache=False``:
         compute only (callers that keep the result themselves, e.g. ``MMFSNet.prepare``)."""
-        w, b = self.value_proj.weight, self.value_proj.bias
-        extra = (w.data_ptr(), w._version, b.data_ptr(), b._version)
-        cacheable = cache and input_padding_mask is None and not torch.is_grad_enabled()
-        if cacheable:
-            hit = self._value_cache.get(input_flatten, extra)
-            if hit is not None:
-                return hit
-        N, n_img, hw, _ = input_flatten.shape
-        value = self.value_proj(input_flatten)
-        if input_padding_mask is not None:
-            value = value.masked_fill(input_padding_mask[..., None], float(0))
-        value = value.reshape(N, n_img * hw, self.n_heads, value.shape[-1] // self.n_heads).contiguous()
-        if cacheable:
-            self._value_cache.put(input_flatten, value, extra)
-        return value
+        def build():
+            N, n_img, hw, _ = input_flatten.shape
+            value = self.value_proj(input_flatten)
+            if input_padding_mask is not None:
+                value = value.masked_fill(input_padding_mask[..., None], float(0))
+            return value.reshape(N, n_img * hw, self.n_heads, value.shape[-1] // self.n_heads).contiguous()
+        return self._value_cache.get_or_build((input_flatten, self.value_proj.weight, self.value_proj.bias), build,
+                                              cache=cache and input_padding_mask is None and not torch.is_grad_enabled())
 
     def forward(self, query, reference_points, input_flatten, input_spatial_shapes, input_level_start_index,
                 input_padding_mask=None, attention_mask=None, output_weight=None, output_bias=None, value=None):
@@ -180,10 +168,7 @@ class MMFS(nn.Module):
         shapes = input_spatial_shapes.contiguous()
         starts = input_level_start_index.contiguous()
         scale = self.scale_ratios.to(torch.float32).contiguous()
-        ign_key = (self.ignore_token.data_ptr(), self.ignore_token._version)
-        if self._ignore_nonzero is None or self._ignore_nonzero[0] != ign_key:   # one host sync per weight load
-            self._ignore_nonzero = (ign_key, bool(torch.count_nonzero(self.ignore_token)))
-        need_null = self._ignore_nonzero[1]
+        need_null = self._needs_null_slot()
 
         D = value.shape[-1]
         if D in _FAST_HEAD_DIMS:
@@ -200,11 +185,3 @@ class MMFS(nn.Module):
         if output_weight is not None:
             return F.linear(sampled, output_weight, output_bias)
         return self.output_proj(sampled)
-
-    _ignore_nonzero = None   # cache of (key, "ignore_token has non-zero entries")
-
-    def _load_from_state_dict(self, *args, **kwargs):
-        super()._load_from_state_dict(*args, **kwargs)
-        self._fused = None
-        self._value_cache.clear()
-        self._ignore_nonzero = None

@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
-from ._cache import SourceCache
+from ._cache import SourceCache, WeightCache
 from .mmfs import MMFS
 
 
@@ -43,28 +43,13 @@ def sincos_pos_embed_2d(embed_dim: int, grid_size: int) -> torch.Tensor:
     return torch.from_numpy(np.concatenate([enc(rows), enc(cols)], axis=1)).float()
 
 
-_RESIZE_CACHE = {}
-
-
 def resize_abs_pos(abs_pos: torch.Tensor, tgt_len: int) -> torch.Tensor:
     """``get_abs_pos`` (utils/pos_embed.py:16-40) for embeddings without a cls token: bicubic resize of the square grid.
-    The table is a frozen parameter, so the resized copy is cached (the reference re-interpolates on every forward)."""
+    The tables are frozen parameters, so callers cache the result on them (the reference re-interpolates per forward)."""
     src = int(math.sqrt(abs_pos.shape[0]))
     tgt = int(math.sqrt(tgt_len))
     if src == tgt:
         return abs_pos
-    key = (abs_pos.data_ptr(), abs_pos._version, abs_pos.dtype, abs_pos.device, tuple(abs_pos.shape), tgt)
-    if key in _RESIZE_CACHE:
-        return _RESIZE_CACHE[key]
-    if len(_RESIZE_CACHE) > 64:
-        _RESIZE_CACHE.clear()
-    out = _resize_abs_pos_uncached(abs_pos, src, tgt)
-    if not torch.is_grad_enabled() or not abs_pos.requires_grad:
-        _RESIZE_CACHE[key] = out
-    return out
-
-
-def _resize_abs_pos_uncached(abs_pos, src, tgt):
     x = abs_pos.float().reshape(1, src, src, -1).permute(0, 3, 1, 2)
     x = F.interpolate(x, size=(tgt, tgt), mode="bicubic", align_corners=False)
     return x.permute(0, 2, 3, 1).flatten(0, 2).to(abs_pos.dtype)
@@ -95,43 +80,38 @@ class MMFSBlock(nn.Module):
         self.conv = nn.Conv2d(query_dim, query_dim, kernel_size=1, stride=1)
         nn.init.zeros_(self.conv.weight)       # zero_module (:148-151)
         nn.init.zeros_(self.conv.bias)
-        self._cache = {}
+        self._geometry_cache = WeightCache()
         self._feat_cache = SourceCache()   # LayerNorm(ms_feat), identity-checked (see _cache.py)
-        self._fused_out = None
+        self._fused_out = WeightCache()
 
     def _reset_parameters(self):
         self.mmfs._reset_parameters()
 
     def _geometry(self, device, dtype, h, w, n_images, spatial_shapes):
-        key = (device, dtype, h, w, n_images, tuple(spatial_shapes), self.pos_embed._version)
-        if key not in self._cache:
+        def build():
             ss = torch.tensor(list(spatial_shapes) * n_images, dtype=torch.long)
             starts = torch.cat((ss.new_zeros((1,)), ss.prod(1).cumsum(0)[:-1]))
             pos = resize_abs_pos(self.pos_embed.detach(), h * w).to(device=device, dtype=dtype)
-            self._cache[key] = (pixel_reference_points(h, w, device), ss.to(device), starts.to(device), pos)
-        return self._cache[key]
+            return pixel_reference_points(h, w, device), ss.to(device), starts.to(device), pos
+        key = (device, dtype, h, w, n_images, tuple(spatial_shapes))
+        return self._geometry_cache.get(self.pos_embed, build, key)
 
     def _out_conv_fused(self):
         """conv1x1(output_proj(x)) = (Wc Wo) x + (Wc bo + bc): one GEMM."""
         ps = (self.mmfs.output_proj.weight, self.mmfs.output_proj.bias, self.conv.weight, self.conv.bias)
-        key = tuple((p.data_ptr(), p._version, p.dtype) for p in ps)
-        if self._fused_out is None or self._fused_out[0] != key:
-            with torch.no_grad():
-                wc = self.conv.weight.view(self.conv.weight.shape[0], -1).float()
-                w = (wc @ ps[0].float()).to(ps[0].dtype).contiguous()
-                b = (wc @ ps[1].float() + ps[3].float()).to(ps[0].dtype).contiguous()
-            self._fused_out = (key, w, b)
-        return self._fused_out[1], self._fused_out[2]
+
+        def build():
+            wc = self.conv.weight.view(self.conv.weight.shape[0], -1).float()
+            w = (wc @ ps[0].float()).to(ps[0].dtype).contiguous()
+            b = (wc @ ps[1].float() + ps[3].float()).to(ps[0].dtype).contiguous()
+            return w, b
+        return self._fused_out.get(ps, build)
 
     def normalised_features(self, ms_feat):
         n = self.feat_norm
-        extra = (n.weight.data_ptr(), n.weight._version, n.bias.data_ptr(), n.bias._version)
-        hit = None if torch.is_grad_enabled() else self._feat_cache.get(ms_feat, extra)
-        if hit is None:
-            hit = ops.layernorm(ms_feat.contiguous(), n.weight, n.bias, n.eps)
-            if not torch.is_grad_enabled():
-                self._feat_cache.put(ms_feat, hit, extra)
-        return hit
+        return self._feat_cache.get_or_build((ms_feat, n.weight, n.bias),
+                                             lambda: ops.layernorm(ms_feat.contiguous(), n.weight, n.bias, n.eps),
+                                             cache=not torch.is_grad_enabled())
 
     @torch.no_grad()
     def project_features(self, ms_feat):
@@ -220,11 +200,9 @@ class MMFSNet(nn.Module):
             return sample, new_res
         spatial_shapes = [(int(f.shape[-2]), int(f.shape[-1])) for f in mmfs_features]
         # constant across the denoise steps of one loop: the same list of tensor objects comes back every step
-        feats = None if torch.is_grad_enabled() else self._packed.get(list(mmfs_features))
-        if feats is None:
-            feats = torch.cat([f.flatten(3).transpose(2, 3) for f in mmfs_features], dim=2).contiguous()   # b n (h w) c
-            if not torch.is_grad_enabled():
-                self._packed.put(list(mmfs_features), feats)
+        def pack():
+            return torch.cat([f.flatten(3).transpose(2, 3) for f in mmfs_features], dim=2).contiguous()   # b n (h w) c
+        feats = self._packed.get_or_build(list(mmfs_features), pack, cache=not torch.is_grad_enabled())
         new_res = ()
         for res, blk in zip(down_block_res_samples, self.mmfs_down_blocks):
             new_res += (res + blk(res, feats, mmfs_mask, spatial_shapes),)

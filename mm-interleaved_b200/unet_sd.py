@@ -29,6 +29,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
+from ._cache import WeightCache
 
 USE_CONV_KERNEL = True      # tests flip this to compare against the cuDNN path on the same weights
 
@@ -41,20 +42,29 @@ def _gn(mod: nn.GroupNorm, x: torch.Tensor, silu: bool) -> torch.Tensor:
     return F.silu(h) if silu else h
 
 
-def _conv(mod: nn.Conv2d, x: torch.Tensor, add_bc: Optional[torch.Tensor] = None,
+class Conv2d(nn.Conv2d):
+    """``nn.Conv2d`` that keeps its filter in the layouts ``ops.conv2d`` (KHWC) and ``ops.conv2d_up2x`` (folded) read."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self._derived = WeightCache()
+
+    def weight_khwc(self) -> torch.Tensor:
+        return self._derived.get(self.weight, lambda: self.weight.permute(0, 2, 3, 1).contiguous(), key="khwc")
+
+    def weight_up2x(self) -> torch.Tensor:
+        return self._derived.get(self.weight, lambda: ops.fold_up2x_weights(self.weight), key="up2x")
+
+
+def _conv(mod: Conv2d, x: torch.Tensor, add_bc: Optional[torch.Tensor] = None,
           residual: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``mod(x) [+ add_bc[:, :, None, None]] [+ residual]`` -- on the wgmma implicit-GEMM kernel when the layer
     qualifies (ops.conv2d_supported), else on the library convolution."""
     stride, pad = mod.stride[0], mod.padding[0]
     if USE_CONV_KERNEL and x.is_contiguous(memory_format=torch.channels_last) and ops.conv2d_supported(x, mod.weight, stride, pad):
-        cache = getattr(mod, "_w_khwc", None)
-        if cache is None or cache[0] != (mod.weight.data_ptr(), mod.weight._version, mod.weight.dtype):
-            cache = ((mod.weight.data_ptr(), mod.weight._version, mod.weight.dtype),
-                     mod.weight.detach().permute(0, 2, 3, 1).contiguous())
-            mod._w_khwc = cache
         if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
             residual = residual.contiguous(memory_format=torch.channels_last)
-        return ops.conv2d(x, cache[1], mod.bias, stride, pad, add_bc=add_bc, residual=residual)
+        return ops.conv2d(x, mod.weight_khwc(), mod.bias, stride, pad, add_bc=add_bc, residual=residual)
     h = mod(x)
     if add_bc is not None:
         h = h + add_bc[:, :, None, None]
@@ -85,11 +95,11 @@ class ResnetBlock2D(nn.Module):
     def __init__(self, in_channels, out_channels, temb_channels=1280, groups=32, eps=1e-5):
         super().__init__()
         self.norm1 = nn.GroupNorm(groups, in_channels, eps=eps)
-        self.conv1 = nn.Conv2d(in_channels, out_channels, 3, padding=1)
+        self.conv1 = Conv2d(in_channels, out_channels, 3, padding=1)
         self.time_emb_proj = nn.Linear(temb_channels, out_channels) if temb_channels is not None else None
         self.norm2 = nn.GroupNorm(groups, out_channels, eps=eps)
-        self.conv2 = nn.Conv2d(out_channels, out_channels, 3, padding=1)
-        self.conv_shortcut = nn.Conv2d(in_channels, out_channels, 1) if in_channels != out_channels else None
+        self.conv2 = Conv2d(out_channels, out_channels, 3, padding=1)
+        self.conv_shortcut = Conv2d(in_channels, out_channels, 1) if in_channels != out_channels else None
 
     def forward(self, x, temb=None):
         add = self.time_emb_proj(F.silu(temb)) if self.time_emb_proj is not None else None
@@ -184,7 +194,7 @@ class Transformer2DModel(nn.Module):
 class Downsample2D(nn.Module):
     def __init__(self, channels):
         super().__init__()
-        self.conv = nn.Conv2d(channels, channels, 3, stride=2, padding=1)
+        self.conv = Conv2d(channels, channels, 3, stride=2, padding=1)
 
     def forward(self, x):
         return _conv(self.conv, x)
@@ -193,7 +203,7 @@ class Downsample2D(nn.Module):
 class Upsample2D(nn.Module):
     def __init__(self, channels):
         super().__init__()
-        self.conv = nn.Conv2d(channels, channels, 3, padding=1)
+        self.conv = Conv2d(channels, channels, 3, padding=1)
 
     def forward(self, x):
         return _conv(self.conv, F.interpolate(x, scale_factor=2.0, mode="nearest"))

@@ -62,16 +62,12 @@ class VAEAttention(nn.Module):
 
 class Upsample2D(unet_sd.Upsample2D):
     """Nearest 2x + 3x3 conv; on the fused phase-form kernel when the layer qualifies (ops.conv2d_up2x_supported),
-    else ``conv(interpolate(x))`` as in the UNet.  The folded weights are cached per weight version."""
+    else ``conv(interpolate(x))`` as in the UNet."""
 
     def forward(self, x):
         w = self.conv.weight
         if unet_sd.USE_CONV_KERNEL and x.is_contiguous(memory_format=torch.channels_last) and ops.conv2d_up2x_supported(x, w):
-            cache = getattr(self, "_w_phases", None)
-            if cache is None or cache[0] != (w.data_ptr(), w._version, w.dtype):
-                cache = ((w.data_ptr(), w._version, w.dtype), ops.fold_up2x_weights(w.detach()))
-                self._w_phases = cache
-            return ops.conv2d_up2x(x, cache[1], self.conv.bias)
+            return ops.conv2d_up2x(x, self.conv.weight_up2x(), self.conv.bias)
         return super().forward(x)
 
 

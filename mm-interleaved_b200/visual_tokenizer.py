@@ -28,6 +28,7 @@ from torch import nn
 
 from . import msda as _msda
 from . import ops
+from ._cache import WeightCache
 from .sd_mmfs import resize_abs_pos, sincos_pos_embed_2d
 
 
@@ -80,15 +81,11 @@ class CLIPAttention(nn.Module):
         self.v_proj = nn.Linear(self.embed_dim, self.embed_dim)
         self.q_proj = nn.Linear(self.embed_dim, self.embed_dim)
         self.out_proj = nn.Linear(self.embed_dim, self.embed_dim)
-        self._qkv = None
+        self._qkv = WeightCache()
 
     def _fused(self):
         ps = (self.q_proj.weight, self.k_proj.weight, self.v_proj.weight, self.q_proj.bias, self.k_proj.bias, self.v_proj.bias)
-        key = tuple((p.data_ptr(), p._version, p.dtype) for p in ps)
-        if self._qkv is None or self._qkv[0] != key:
-            with torch.no_grad():
-                self._qkv = (key, torch.cat(ps[:3], 0).contiguous(), torch.cat(ps[3:], 0).contiguous())
-        return self._qkv[1], self._qkv[2]
+        return self._qkv.get(ps, lambda: (torch.cat(ps[:3], 0).contiguous(), torch.cat(ps[3:], 0).contiguous()))
 
     def forward(self, x):
         """softmax(q k^T / sqrt(d)) v, no mask (CLIPXAttention.forward, xattn.py:47-141)."""
@@ -558,6 +555,7 @@ class VisualTokenizer(nn.Module):
         self.pos_ln = nn.LayerNorm(enc, eps=1e-6)
         pe = torch.cat([torch.zeros(1, enc), sincos_pos_embed_2d(enc, grid_size)], 0)       # cls_token=True (:27-31)
         self.pos_embed = nn.Parameter(pe, requires_grad=False)
+        self._abs_pos_cache = WeightCache()
         self.perceiver_resampler = PerceiverResampler(**perceiver_config)
         self.length = perceiver_config["num_queries"]
         self.post_ln = nn.LayerNorm(enc, eps=1e-6)
@@ -568,6 +566,13 @@ class VisualTokenizer(nn.Module):
             self.register_buffer("clip_mean", torch.tensor(CLIP_MEAN).view(1, 3, 1, 1))
             self.register_buffer("clip_std", torch.tensor(CLIP_STD).view(1, 3, 1, 1))
 
+    def abs_pos(self, n):
+        """``pos_embed`` without its cls row, resized to ``n`` positions.  Cached per length on the parameter itself
+        (the reference re-interpolates on every forward); not while the table is being trained."""
+        if torch.is_grad_enabled() and self.pos_embed.requires_grad:
+            return resize_abs_pos(self.pos_embed[1:], n)
+        return self._abs_pos_cache.get(self.pos_embed, lambda: resize_abs_pos(self.pos_embed[1:], n), key=n)
+
     def forward(self, image):
         if self.clip_normalize:
             image = (image - self.clip_mean.to(image.dtype)) / self.clip_std.to(image.dtype)
@@ -575,10 +580,10 @@ class VisualTokenizer(nn.Module):
         image_embed = out.last_hidden_state
         feats = []
         for f in out.hidden_states:                                                       # :74-82
-            pe = resize_abs_pos(self.pos_embed[1:], f.size(2) * f.size(3))
+            pe = self.abs_pos(f.size(2) * f.size(3))
             feats.append(f + pe.to(f.dtype).view(f.size(2), f.size(3), -1).permute(2, 0, 1))
         n = image_embed.size(1)
-        pe = torch.cat([self.pos_embed[:1], resize_abs_pos(self.pos_embed[1:], n - 1)], 0).to(image_embed.dtype)
+        pe = torch.cat([self.pos_embed[:1], self.abs_pos(n - 1)], 0).to(image_embed.dtype)
         q_in = _ln(self.pos_ln, self.pos_proj(image_embed)) + pe                          # :85-87
         image_embed = image_embed + pe
         q_in = _ln(self.post_ln, q_in)
