@@ -258,6 +258,16 @@ int mmfs_conv2d_up2x_nhwc(const void *x, const void *w_phases, const void *bias,
                           int Cout, int dtype, void *stream);
 
 /*
+ * 3x3 / stride-2 convolution after a one-sided zero pad of one row at the bottom and one column at the right (diffusers'
+ * Downsample2D with padding=0, the VAE encoder's downsampler): conv3x3(F.pad(x, (0, 1, 0, 1)), stride 2).
+ *   x (B,H,W,Cin) NHWC with H and W even; w (Cout,3,3,Cin); bias (Cout) or NULL; out (B,H/2,W/2,Cout) NHWC.
+ * Null pointers, non-positive or odd H / W: MMFS_EINVAL.  Same requirements as mmfs_conv2d_nhwc on (Cin, Cout, dtype,
+ * alignment), with the H/2 x W/2 output tileable.
+ */
+int mmfs_conv2d_down2x_nhwc(const void *x, const void *w, const void *bias, void *out, int B, int H, int W, int Cin,
+                            int Cout, int dtype, void *stream);
+
+/*
  * GroupNorm (+ SiLU when silu != 0) on NHWC activations: the nn.GroupNorm(32) in front of every UNet convolution
  * (same call sites as mmfs_conv2d_nhwc).  x, y (B, HW, C) NHWC; gamma/beta (C) or NULL; stats = caller-provided
  * scratch of 128*B*G floats (per-chunk partial sums; reduced in a fixed order, so results are run-to-run reproducible).  f32 / f16 / bf16; C % (16/sizeof) == 0 and C*sizeof <= 16 KiB.

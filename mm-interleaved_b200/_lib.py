@@ -44,6 +44,7 @@ SIGNATURES = {
     "mmfs_groupnorm_nhwc": (_I, [_P] * 5 + [_I] * 4 + [_F, _I, _I, _P]),
     "mmfs_conv2d_nhwc": (_I, [_P] * 6 + [_I] * 10 + [_P]),
     "mmfs_conv2d_up2x_nhwc": (_I, [_P] * 4 + [_I] * 6 + [_P]),
+    "mmfs_conv2d_down2x_nhwc": (_I, [_P] * 4 + [_I] * 6 + [_P]),
     "mmfs_attn_decode_scratch_floats": (_L, [_I] * 4),
     "mmfs_attn_decode": (_I, [_P] * 6 + [_I] * 4 + [_L] * 6 + [_F, _I, _I, _I, _P]),
     "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),

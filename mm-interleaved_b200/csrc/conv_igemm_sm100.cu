@@ -26,6 +26,9 @@
 // {w0 + w1, w2} at pad 0 -- read from (4, Cout, 2, 2, Cin) (ops.fold_up2x_weights).  blockIdx.z is the phase; the
 // tiles walk the (H, W) low-resolution grid and the epilogue stores pixel (ho, wo) to (2 ho + py, 2 wo + px) of the
 // (2H, 2W) output.  TMA's zero fill at X[-1] / X[H] is exactly the padding of the upsampled map.
+//
+// The VAE encoder's downsampler, conv3x3(F.pad(x, (0, 1, 0, 1)), stride 2), is the UP = false kernel at pad 0 / stride 2
+// with the (H/2, W/2) output grid given by its entry point: the one-sided pad is the zero fill of row H / column W.
 // Roofline: tensor (2*M*N*K flop).
 #include "tc_common.cuh"
 
@@ -178,11 +181,12 @@ int launch(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap &mx, const
     return MMFS_OK;
 }
 
-// UP: KH = KW = 2 and the (H, W) low-resolution grid of outputs per phase; the per-phase padding is set in the kernel
+// Output grid (Ho, Wo) from the caller: the (H, W) low-resolution grid per phase for UP (KH = KW = 2; the per-phase
+// padding is set in the kernel), the symmetric-padding size for mmfs_conv2d_nhwc, (H/2, W/2) for the one-sided pad
 template <bool UP>
 int launch_conv(const char *what, const void *x, const void *w, const void *bias, const void *add_bc, const void *residual,
-                void *out, int B, int H, int W, int Cin, int Cout, int KH, int KW, int stride, int pad, int dtype, void *stream) {
-    const int Ho = UP ? H : (H + 2 * pad - KH) / stride + 1, Wo = UP ? W : (W + 2 * pad - KW) / stride + 1;
+                void *out, int B, int H, int W, int Ho, int Wo, int Cin, int Cout, int KH, int KW, int stride, int pad,
+                int dtype, void *stream) {
     int TW, TH, TB;
     if (Wo % 16 == 0 && Ho % 8 == 0) { TW = 16; TH = 8; TB = 1; }
     else if (Wo == 8 && Ho == 8 && B % 2 == 0) { TW = 8; TH = 8; TB = 2; }
@@ -240,7 +244,9 @@ extern "C" int mmfs_conv2d_nhwc(const void *x, const void *w, const void *bias, 
                                 int dtype, void *stream) {
     MMFS_CHECK_ARG(B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && KH > 0 && KW > 0 && stride > 0 && pad >= 0, "conv2d_nhwc: bad dimension");
     MMFS_CHECK_ARG(x && w && out, "conv2d_nhwc: null pointer argument");
-    return launch_conv<false>("conv2d_nhwc", x, w, bias, add_bc, residual, out, B, H, W, Cin, Cout, KH, KW, stride, pad, dtype, stream);
+    const int Ho = (H + 2 * pad - KH) / stride + 1, Wo = (W + 2 * pad - KW) / stride + 1;
+    return launch_conv<false>("conv2d_nhwc", x, w, bias, add_bc, residual, out, B, H, W, Ho, Wo, Cin, Cout, KH, KW, stride,
+                              pad, dtype, stream);
 }
 
 // x (B, H, W, Cin) NHWC, w_phases (4, Cout, 2, 2, Cin) folded per output parity, out (B, 2H, 2W, Cout) NHWC; bias (Cout) may be null
@@ -248,5 +254,18 @@ extern "C" int mmfs_conv2d_up2x_nhwc(const void *x, const void *w_phases, const 
                                      int Cout, int dtype, void *stream) {
     MMFS_CHECK_ARG(B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "conv2d_up2x_nhwc: bad dimension");
     MMFS_CHECK_ARG(x && w_phases && out, "conv2d_up2x_nhwc: null pointer argument");
-    return launch_conv<true>("conv2d_up2x_nhwc", x, w_phases, bias, nullptr, nullptr, out, B, H, W, Cin, Cout, 2, 2, 1, 0, dtype, stream);
+    return launch_conv<true>("conv2d_up2x_nhwc", x, w_phases, bias, nullptr, nullptr, out, B, H, W, H, W, Cin, Cout, 2, 2, 1, 0,
+                             dtype, stream);
+}
+
+// x (B, H, W, Cin) NHWC, w (Cout, 3, 3, Cin), out (B, H/2, W/2, Cout) NHWC; bias (Cout) may be null.
+// conv3x3(pad(x, bottom 1, right 1), stride 2): diffusers' Downsample2D(padding=0).  Pad 0, stride 2: the last output
+// row reads input rows H-2 .. H, and row H (column W) is TMA's zero fill -- exactly the one-sided pad.
+extern "C" int mmfs_conv2d_down2x_nhwc(const void *x, const void *w, const void *bias, void *out, int B, int H, int W, int Cin,
+                                       int Cout, int dtype, void *stream) {
+    MMFS_CHECK_ARG(B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "conv2d_down2x_nhwc: bad dimension");
+    MMFS_CHECK_ARG(x && w && out, "conv2d_down2x_nhwc: null pointer argument");
+    MMFS_CHECK_ARG(H % 2 == 0 && W % 2 == 0, "conv2d_down2x_nhwc: odd H or W");
+    return launch_conv<false>("conv2d_down2x_nhwc", x, w, bias, nullptr, nullptr, out, B, H, W, H / 2, W / 2, Cin, Cout, 3, 3,
+                              2, 0, dtype, stream);
 }

@@ -199,16 +199,20 @@ class StableDiffusion(nn.Module):
     ``vae_sd.AutoencoderKL``) is registered as ``self.vae`` -- state-dict keys ``vae.*`` as in a reference checkpoint --
     and ``vae_decode`` defaults to its ``decode``; any callable latents -> image in [-1, 1] may be given as
     ``vae_decode`` instead.  Without either, ``generate_images`` returns the denoised latents (the pipeline's
-    ``output_type="latent"`` result, sd.py:196-211)."""
+    ``output_type="latent"`` result, sd.py:196-211).  ``forward`` (the denoising loss) needs a VAE with an encoder
+    (``vae_sd.AutoencoderKL(with_encoder=True)``); it encodes in chunks of ``vae_encode_mini_bs`` images (<= 0: one
+    chunk)."""
 
     def __init__(self, unet=None, mmfs_module=None, image_size=512, base_seed=0, use_random_seed=False,
-                 noise_scheduler=None, vae_decode=None, vae_scaling_factor=0.18215, vae=None, **unet_kwargs):
+                 noise_scheduler=None, vae_decode=None, vae_scaling_factor=0.18215, vae=None, vae_encode_mini_bs=32,
+                 **unet_kwargs):
         super().__init__()
         from . import unet_sd
         from .scheduler import DDPMScheduler, SD21_BASE_SCHEDULER
         self.unet = unet if unet is not None else unet_sd.UNet2DConditionModel(**unet_kwargs)
         self.mmfs_module = mmfs_module
         self.image_size, self.base_seed, self.use_random_seed = image_size, base_seed, use_random_seed
+        self.vae_encode_mini_bs = vae_encode_mini_bs
         self.noise_scheduler = noise_scheduler if noise_scheduler is not None else DDPMScheduler(**SD21_BASE_SCHEDULER)
         self.vae = vae
         if vae is not None and vae_decode is None:
@@ -257,17 +261,63 @@ class StableDiffusion(nn.Module):
         image = self.vae_decode(lat.float() / self.vae_scaling_factor)                       # sd.py:212-215
         return (image / 2 + 0.5).clamp(0, 1).float()
 
+    def _encode_latents(self, image, dtype, generator=None):
+        """sd.py:220-238: posterior samples of ``vae_encode_mini_bs`` images at a time, cast to ``dtype``, times the
+        scaling factor.  The VAE encodes in its own dtype (the reference casts it to fp32)."""
+        n = self.vae_encode_mini_bs if self.vae_encode_mini_bs > 0 else image.shape[0]
+        parts = [self.vae.encode(image[i:i + n]).latent_dist.sample(generator).to(dtype) for i in range(0, image.shape[0], n)]
+        return torch.cat(parts, dim=0) * self.vae_scaling_factor
+
+    def forward(self, image, text_embeds, return_outputs=False, mmfs_features=None, mmfs_mask=None,
+                generator: Optional[torch.Generator] = None):
+        """The denoising loss of sd.py:240-316 (inference kernels: an evaluation loss, call under ``torch.no_grad()``).
+        ``image`` (B, 3, S, S) in [0, 1] with S = ``image_size``; returns the per-element
+        ``mse(unet(noisy, t), target)`` in fp32, shaped like the latents, or with ``return_outputs`` the reference's
+        ``dict(loss, pred, target)`` plus ``latents`` and ``timesteps``.
+
+        Random draws, in this order: the posterior noise of each encode chunk, the diffusion noise (like the latents, in
+        the UNet's dtype), one timestep in [0, num_train_timesteps) per image -- from ``generator`` when given, else from
+        the global generator, as the reference does.  Differences from the reference: the image is normalised out of
+        place (the reference's ``image.sub_(0.5).div_(0.5)`` rewrites the caller's tensor), and the UNet runs eagerly on
+        the (B,) timesteps with no classifier-free-guidance batch."""
+        h, w = image.shape[-2:]
+        assert h == self.image_size and w == self.image_size, f"{tuple(image.shape)=} {self.image_size=}"
+        if getattr(self.vae, "encoder", None) is None:
+            raise RuntimeError("StableDiffusion.forward needs a VAE with an encoder (vae_sd.AutoencoderKL(with_encoder=True))")
+        dtype = next(self.unet.parameters()).dtype
+        latents = self._encode_latents((image - 0.5) / 0.5, dtype, generator)
+        noise = torch.randn(latents.shape, generator=generator, device=latents.device, dtype=latents.dtype)
+        timesteps = torch.randint(0, self.noise_scheduler.num_train_timesteps, (latents.shape[0],), generator=generator,
+                                  device=latents.device)
+        noisy = self.noise_scheduler.add_noise(latents, noise, timesteps)
+        pt = self.noise_scheduler.prediction_type
+        if pt == "epsilon":
+            target = noise
+        elif pt == "v_prediction":
+            target = self.noise_scheduler.get_velocity(latents, noise, timesteps)
+        else:
+            raise ValueError(f"Unknown prediction type {pt}")
+        if noisy.is_cuda:
+            noisy = noisy.contiguous(memory_format=torch.channels_last)
+        pred = self.unet(noisy, timesteps, text_embeds, mmfs_features=mmfs_features, mmfs_mask=mmfs_mask,
+                         mmfs_module=self.mmfs_module)
+        loss = F.mse_loss(pred.float(), target.float(), reduction="none")
+        if not return_outputs:
+            return loss
+        return dict(loss=loss, pred=pred, target=target, latents=latents, timesteps=timesteps)
+
 
 class ImageDecoder(nn.Module):
     """``ImageDecoder`` (decoders/decoder_image.py:9-156): ``perceiver_resampler`` (Q-Former, 77 queries of width 1024
     over the per-image LLM context), ``neg_prompt_embeds`` and ``decoder`` = ``StableDiffusion`` (UNet + MMFSNet +
     scheduler, and the VAE decoder when ``vae`` is given).  State-dict names follow the reference (``decoder.unet.*``,
     ``decoder.mmfs_module.*``, ``decoder.vae.*``).  ``vae``: ``True`` builds the SD-2.1 decoder (vae_sd.py), a dict
-    builds ``vae_sd.AutoencoderKL(**vae)``, a module is used as it is; it applies when ``decoder`` is not given."""
+    builds ``vae_sd.AutoencoderKL(**vae)`` (``{"with_encoder": True}`` adds the encoder that ``forward``, the image
+    loss, needs), a module is used as it is; it applies when ``decoder`` is not given."""
 
     def __init__(self, perceiver_config=None, seq_len=77, embed_dim=1024, unet=None, mmfs_module=None, image_size=512,
                  base_seed=0, sd_base_seed=None, sd_use_random_seed=False, mmfs_input_channel=1024, mmfs_feat_levels=4,
-                 uncond_prob=0.1, decoder: Optional[nn.Module] = None, vae=None, **_):
+                 uncond_prob=0.1, decoder: Optional[nn.Module] = None, vae=None, vae_encode_mini_bs=32, **_):
         super().__init__()
         from .visual_tokenizer import PerceiverResampler
         self.uncond_prob = uncond_prob
@@ -285,12 +335,35 @@ class ImageDecoder(nn.Module):
                 vae = AutoencoderKL(**(vae if isinstance(vae, dict) else {}))
             decoder = StableDiffusion(unet=unet, mmfs_module=mmfs_module, image_size=image_size,
                                       base_seed=base_seed if sd_base_seed is None else sd_base_seed,
-                                      use_random_seed=sd_use_random_seed, vae=None if vae is False else vae)
+                                      use_random_seed=sd_use_random_seed, vae=None if vae is False else vae,
+                                      vae_encode_mini_bs=vae_encode_mini_bs)
         self.decoder = decoder
 
     # round-1 attribute names
     unet = property(lambda self: self.decoder.unet)
     mmfs_module = property(lambda self: self.decoder.mmfs_module)
+
+    def forward(self, image_tensors, context_features, context_attention_mask=None, image_loss_mask=None,
+                mmfs_features=None, mmfs_mask=None, generator: Optional[torch.Generator] = None):
+        """decoder_image.py:69-120: the image loss of B_I images, a scalar.  Q-Former over the per-image context; with
+        probability ``uncond_prob`` an image's prompt is replaced by ``neg_prompt_embeds`` (in eval mode too, as in the
+        reference; that ``rand`` is drawn before the diffusion loss's draws, from ``generator`` when given); the
+        per-element SD loss is zeroed for images whose context has <= 2 tokens (``<bos>``, ``<soi>``) and where
+        ``image_loss_mask`` is 0, then averaged over every element, zeroed ones included."""
+        assert image_tensors.shape[0] == context_features.shape[0]
+        if context_attention_mask is None:
+            raise ValueError("ImageDecoder.forward needs context_attention_mask")
+        assert bool(torch.all(context_attention_mask.sum(dim=1) > 0)), "an image has an empty context"
+        ctx = self.perceiver_resampler(encoder_hidden_states=context_features,
+                                       encoder_attention_mask=context_attention_mask)[0]
+        if self.uncond_prob > 0.0:
+            u = torch.rand(ctx[:, :1, :1].shape, generator=generator, device=ctx.device, dtype=ctx.dtype)
+            ctx = torch.where(u < self.uncond_prob, self.neg_prompt_embeds.to(ctx.dtype), ctx)
+        loss = self.decoder(image_tensors, ctx, mmfs_features=mmfs_features, mmfs_mask=mmfs_mask, generator=generator)
+        loss = loss * (context_attention_mask.sum(dim=1) > 2).to(loss.device).view(-1, 1, 1, 1)
+        if image_loss_mask is not None:
+            loss = loss * image_loss_mask.to(loss.device).view(-1, 1, 1, 1)
+        return loss.mean()
 
     @torch.no_grad()
     def generate_images(self, context_features, context_attention_mask=None, mmfs_features=None, mmfs_mask=None, **kwargs):
@@ -743,8 +816,9 @@ class MMInterleaved(InterleavedForward):
 
     Differences a caller can see: weights are not fetched by the constructor (``llm_model_path`` is only read for its
     ``config.json``; the reference's ``load_model_weights`` fills the parameters afterwards); ``forward`` computes the
-    text loss (and returns the logits) -- the image-decoder training loss needs the VAE encoder and is not built;
-    ``generate_images`` returns latents as ``image`` unless the image decoder has a VAE (``image_decoder_config``
+    text loss (and returns the logits), and adds the image-decoder loss ``loss_img`` when the image decoder's VAE has
+    an encoder (``image_decoder_config={"vae": {"with_encoder": True}}``) -- evaluation losses only, there is no
+    backward; ``generate_images`` returns latents as ``image`` unless the image decoder has a VAE (``image_decoder_config``
     with ``vae=True`` builds the SD-2.1 decoder, vae_sd.py) or a ``vae_decode`` callable is attached to
     ``image_decoder.decoder``.  Extension keyword: ``llm_config`` (a ``LlamaMMFSConfig`` / dict) replaces
     ``llm_model_path``; ``max_num_image`` in a batch skips the one host sync on ``num_image_per_seq.max()``."""
@@ -838,10 +912,15 @@ class MMInterleaved(InterleavedForward):
     def forward(self, text_ids, image_tensors=None, image_tensors_dec=None, num_image_per_seq=None, attention_mask=None,
                 gt_text_ids=None, nearest_bos_idxs=None, ignore_prompt_token_offset=0, loss_img_weight=None,
                 loss_txt_weight=None, meta=None, image_loss_mask=None, **kwargs):
-        """mm_interleaved.py:408-518 up to the text loss.  Returns ``loss_txt`` / ``loss`` like the reference plus
-        ``text_logits`` (B, T, V) (extension; ``return_loss=False`` stops there -- the "step" of SURVEY.md 8d).
+        """mm_interleaved.py:408-518.  Returns ``loss_txt`` / ``loss`` like the reference plus ``text_logits`` (B, T, V)
+        (extension; ``return_loss=False`` stops there -- the "step" of SURVEY.md 8d).  When the image decoder's VAE has
+        an encoder, the image loss is added as in the reference: ``ImageDecoder.forward`` on ``image_tensors_dec`` (else
+        ``image_tensors``) with the per-image contexts and previous-image MMFS features (from ``nearest_bos_idxs``),
+        ``loss_img`` = its detached mean and ``loss = loss_txt * w_txt + loss_img * w_img``; ``multiscale_features``
+        then leaves the output, as there.  ``generator`` (keyword) seeds the image loss's random draws.
         Inference-only kernels: call under ``torch.no_grad()``."""
         return_loss = kwargs.pop("return_loss", True)
+        generator = kwargs.pop("generator", None)
         out = self._prepare_mm_embeds(text_ids, image_tensors, num_image_per_seq, meta, kwargs.pop("max_num_image", None))
         mm = self.mm_decoder(inputs_embeds=out.pop("mm_embeds"), attention_mask=attention_mask,
                              vision_hidden_states=out.pop("mmfs_features_mm"),
@@ -855,7 +934,24 @@ class MMInterleaved(InterleavedForward):
         loss_txt = F.cross_entropy(logits[:, :-1].float().transpose(1, 2), gt.contiguous(), reduction="mean")   # :458-463
         w = self.loss_txt_weight if loss_txt_weight is None else loss_txt_weight
         out.update(loss_txt=loss_txt.detach(), loss=loss_txt * w, text_logits=logits)
+        if self._has_image_loss():                                                                    # :478-515
+            st = self.special_token_dict
+            ms = out.pop("multiscale_features")
+            ctx, ctx_mask = context_features_for_image_decoder(mm.last_hidden_state, text_ids, st["soi_token_id"],
+                                                               self.context_feat_proj, self.seq_len, ms[0].shape[0],
+                                                               nearest_bos_idxs=nearest_bos_idxs)
+            mmfs_features, mmfs_mask = mmfs_features_for_image_decoder(ms, text_ids, st["soi_token_id"], nearest_bos_idxs)
+            loss_img = self.image_decoder(image_tensors=image_tensors if image_tensors_dec is None else image_tensors_dec,
+                                          context_features=ctx, context_attention_mask=ctx_mask,
+                                          image_loss_mask=image_loss_mask, mmfs_features=mmfs_features,
+                                          mmfs_mask=mmfs_mask, generator=generator).mean()
+            wi = self.loss_img_weight if loss_img_weight is None else loss_img_weight
+            out.update(loss_img=loss_img.detach(), loss=out["loss"] + loss_img * wi)
         return out
+
+    def _has_image_loss(self) -> bool:
+        sd = getattr(self.image_decoder, "decoder", None)
+        return getattr(getattr(sd, "vae", None), "encoder", None) is not None
 
     @torch.no_grad()
     def generate_texts(self, text_ids, image_tensors=None, num_image_per_seq=None, attention_mask=None, meta=None, **kwargs):

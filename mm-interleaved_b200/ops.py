@@ -260,6 +260,39 @@ def conv2d_up2x(x: torch.Tensor, weight_phases: torch.Tensor, bias=None) -> torc
     return out
 
 
+def conv2d_down2x_supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
+    """Whether ``conv2d_down2x`` can take ``conv3x3(F.pad(x, (0, 1, 0, 1)), stride 2)`` for this (B, Cin, H, W) input and
+    (Cout, Cin, 3, 3) filter."""
+    if x.dtype not in (torch.bfloat16, torch.float16) or not x.is_cuda or x.dim() != 4 or tuple(weight.shape[2:]) != (3, 3):
+        return False
+    B, Cin, H, W = x.shape
+    Cout = weight.shape[0]
+    if H % 2 or W % 2:
+        return False
+    Ho, Wo = H // 2, W // 2
+    tile = (Wo % 16 == 0 and Ho % 8 == 0) or (Wo == 8 and Ho == 8 and B % 2 == 0)
+    return Cin % 64 == 0 and (Cout % 160 == 0 or Cout % 128 == 0) and tile
+
+
+def conv2d_down2x(x: torch.Tensor, weight_khwc: torch.Tensor, bias=None) -> torch.Tensor:
+    """diffusers' ``Downsample2D(padding=0)`` -- one zero row at the bottom and one zero column at the right, then a 3x3 /
+    stride-2 convolution -- in the implicit-GEMM kernel (csrc/conv_igemm_sm100.cu), the padded copy never formed.  ``x``
+    (B, Cin, H, W) channels_last with H, W even; ``weight_khwc`` (Cout, 3, 3, Cin) contiguous; returns (B, Cout, H/2, W/2)
+    channels_last."""
+    B, Cin, H, W = x.shape
+    Cout = weight_khwc.shape[0]
+    inference_only("conv2d_down2x", x, weight_khwc, bias)
+    _require(x.is_contiguous(memory_format=torch.channels_last) and weight_khwc.is_contiguous(), "conv2d_down2x: x must be channels_last")
+    _require(tuple(weight_khwc.shape) == (Cout, 3, 3, Cin), "conv2d_down2x: weights must be (Cout, 3, 3, Cin)")
+    out = torch.empty((B, Cout, H // 2, W // 2), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+    with torch.cuda.device(x.device):
+        rc = _lib.lib().mmfs_conv2d_down2x_nhwc(x.data_ptr(), weight_khwc.data_ptr(), bias.data_ptr() if bias is not None else None,
+                                                out.data_ptr(), B, H, W, Cin, Cout, _DTYPE_CODE[x.dtype], _stream())
+    _lib.check(rc, "conv2d_down2x")
+    launch_counter[0] += 1
+    return out
+
+
 def group_norm_supported(x: torch.Tensor) -> bool:
     if not x.is_cuda or x.dim() != 4 or x.dtype not in _DTYPE_CODE or x.dtype == torch.float64:
         return False

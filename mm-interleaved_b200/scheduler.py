@@ -71,6 +71,24 @@ class _SchedulerBase:
     def _prev(self, t: int) -> int:
         return t - self.num_train_timesteps // self.num_inference_steps
 
+    def _noise_coefficients(self, timesteps, sample):
+        """(sqrt(abar_t), sqrt(1 - abar_t)) per sample, shaped to broadcast over (C, H, W); ``alphas_cumprod`` is moved
+        to the sample's device AND dtype first, as in diffusers 0.20 (a 16-bit sample rounds abar_t to 16 bit)."""
+        acp = self.alphas_cumprod.to(device=sample.device, dtype=sample.dtype)[timesteps.to(sample.device)]
+        shape = (-1,) + (1,) * (sample.dim() - 1)
+        return (acp ** 0.5).flatten().view(shape), ((1 - acp) ** 0.5).flatten().view(shape)
+
+    def add_noise(self, original_samples, noise, timesteps):
+        """Forward diffusion ``sqrt(abar_t) x + sqrt(1 - abar_t) eps``, one timestep per sample (diffusers 0.20's
+        ``add_noise``)."""
+        a, b = self._noise_coefficients(timesteps, original_samples)
+        return a * original_samples + b * noise
+
+    def get_velocity(self, sample, noise, timesteps):
+        """The v-prediction target ``sqrt(abar_t) eps - sqrt(1 - abar_t) x``, one timestep per sample."""
+        a, b = self._noise_coefficients(timesteps, sample)
+        return a * noise - b * sample
+
     def _x0(self, model_output, sample, a_t):
         if self.prediction_type == "epsilon":
             return (sample - (1 - a_t) ** 0.5 * model_output) / a_t ** 0.5

@@ -1,6 +1,9 @@
 """SD-2.1 VAE decode timing: a bf16 decode of (8, 4, 64, 64) latents (eight 512 x 512 images) at SD-2.1 widths.
+With ``--encode``, the encoder half instead (see ``encode_bench``): eight 512 x 512 images encoded in bf16 on this
+repo's kernels, on cuDNN (``unet_sd.USE_CONV_KERNEL = False``) and in fp32; the three downsample shapes against
+``F.pad`` + cuDNN; cuDNN's ``conv_in`` (Cin = 3) alone; one ``ImageDecoder.forward`` (the image loss) with B_I = 8.
 
-    python tools/vae_bench.py [--batch 8] [--iters 10] [--warmup 3] [--out DIR]
+    python tools/vae_bench.py [--encode] [--batch 8] [--iters 10] [--warmup 3] [--out DIR]
 
 * whole decode, CUDA events after warm-up, median (and min / max) of ``--iters`` decodes, for three paths of the same
   module and weights: bf16 on this repo's kernels; bf16 on cuDNN (``unet_sd.USE_CONV_KERNEL = False``: every
@@ -89,17 +92,108 @@ def conv_shapes(model, z):
     return counts
 
 
+def _median(t):
+    return {"median_ms": statistics.median(t), "min_ms": min(t), "max_ms": max(t)}
+
+
+def encode_bench(args, info):
+    """``--encode``: the encoder half and the image-decoder loss step it feeds."""
+    from mm_interleaved_b200.mm_interleaved import ImageDecoder
+    torch.manual_seed(0)
+    model = AutoencoderKL(with_encoder=True).eval().to("cuda", torch.bfloat16).to(memory_format=CL)
+    x = torch.rand((args.batch, 3, 512, 512), device="cuda") * 2 - 1
+    res = {"gpu": info, "mode": "encode", "batch": args.batch, "iters": args.iters,
+           "cudnn_allow_tf32": torch.backends.cudnn.allow_tf32, "matmul_allow_tf32": torch.backends.cuda.matmul.allow_tf32}
+    with torch.no_grad():
+        enc = {"own_bf16": time_ms(lambda: model.encode(x), args.iters, args.warmup)}
+        mean_own = model.encode(x).latent_dist.mean.float()
+        unet_sd.USE_CONV_KERNEL = False
+        try:
+            enc["cudnn_bf16"] = time_ms(lambda: model.encode(x), args.iters, args.warmup)
+            mean_lib = model.encode(x).latent_dist.mean.float()
+        finally:
+            unet_sd.USE_CONV_KERNEL = True
+        m32 = AutoencoderKL(with_encoder=True).eval().to("cuda")
+        m32.load_state_dict({k: v.float() for k, v in model.state_dict().items()})
+        enc["cudnn_fp32"] = time_ms(lambda: m32.encode(x), args.iters, args.warmup)
+        mean_32 = m32.encode(x).latent_dist.mean
+        del m32
+        res["encode"] = {k: _median(v) for k, v in enc.items()}
+        scale = mean_32.abs().max()
+        res["mean_err_vs_fp32"] = {"own_bf16_max_rel": float((mean_own - mean_32).abs().max() / scale),
+                                   "cudnn_bf16_max_rel": float((mean_lib - mean_32).abs().max() / scale)}
+
+        rows = []
+        for C, H in ((128, 512), (256, 256), (512, 128)):            # the three downsamplers, eight images
+            xd = torch.randn((args.batch, C, H, H), device="cuda", dtype=torch.bfloat16).contiguous(memory_format=CL)
+            w = (torch.randn((C, C, 3, 3), device="cuda") / (C * 9) ** 0.5).to(torch.bfloat16)
+            bias = torch.zeros(C, device="cuda", dtype=torch.bfloat16)
+            wk, wcl = w.permute(0, 2, 3, 1).contiguous(), w.contiguous(memory_format=CL)
+            flop = 2.0 * args.batch * (H // 2) ** 2 * C * C * 9
+            own_ms = kernel_ms(lambda: ops.conv2d_down2x(xd, wk, bias))
+            lib_ms = kernel_ms(lambda: F.conv2d(F.pad(xd, (0, 1, 0, 1)), wcl, bias, stride=2))
+            rows.append({"C": C, "H": H, "own_ms": own_ms, "own_tflops": flop / own_ms / 1e9,
+                         "pad_cudnn_ms": lib_ms, "pad_cudnn_tflops": flop / lib_ms / 1e9})
+            del xd, w, wk, wcl
+        res["down2x"] = rows
+        conv_in = model.encoder.conv_in
+        xin = x.to(torch.bfloat16).contiguous(memory_format=CL)
+        res["conv_in_cudnn_ms"] = kernel_ms(lambda: conv_in(xin))
+        del model
+
+        torch.manual_seed(1)
+        dec = ImageDecoder(perceiver_config=dict(num_queries=77, hidden_size=1024, encoder_hidden_size=5120,
+                                                 cross_attention_frequency=1, num_hidden_layers=1, num_attention_heads=16),
+                           seq_len=77, embed_dim=1024, image_size=512, vae={"with_encoder": True}).eval()
+        dec = dec.to("cuda", torch.bfloat16)
+        dec.decoder.unet.to(memory_format=CL)
+        B = args.batch
+        images = torch.rand((B, 3, 512, 512), device="cuda")
+        ctx = torch.randn((B, 40, 5120), device="cuda", dtype=torch.bfloat16)
+        ctx_mask = torch.ones((B, 40), dtype=torch.long, device="cuda")
+        feats = [torch.randn((B, 1, 1024, s, s), device="cuda", dtype=torch.bfloat16) for s in (64, 32, 16, 8)]
+        fmask = torch.ones((B, 1), dtype=torch.long, device="cuda")
+        step = lambda: dec(images, ctx, ctx_mask, mmfs_features=feats, mmfs_mask=fmask,
+                           generator=torch.Generator(device="cuda").manual_seed(0))
+        res["image_decoder_forward"] = _median(time_ms(step, args.iters, args.warmup))
+        res["image_decoder_forward"]["loss"] = float(step())
+
+    print(f"encode of ({args.batch}, 3, 512, 512) images, median of {args.iters}:")
+    for name, d in res["encode"].items():
+        print(f"  {name:11s} {d['median_ms']:9.2f} ms  (min {d['min_ms']:.2f}, max {d['max_ms']:.2f})")
+    print(f"  posterior mean max |err| / max|fp32|: own bf16 {res['mean_err_vs_fp32']['own_bf16_max_rel']:.3e}, "
+          f"cuDNN bf16 {res['mean_err_vs_fp32']['cudnn_bf16_max_rel']:.3e}")
+    print("downsample (one-sided pad + 3x3 / stride 2), one launch:")
+    for r in rows:
+        print(f"  {r['C']:4d}ch {r['H']}^2 -> {r['H'] // 2}^2  own {r['own_ms']:8.3f} ms {r['own_tflops']:6.1f} TF/s  "
+              f"pad + cuDNN {r['pad_cudnn_ms']:8.3f} ms {r['pad_cudnn_tflops']:6.1f} TF/s")
+    print(f"conv_in (3 -> 128, 512^2, cuDNN bf16): {res['conv_in_cudnn_ms']:.3f} ms")
+    d = res["image_decoder_forward"]
+    print(f"ImageDecoder.forward, B_I = {args.batch}: {d['median_ms']:.2f} ms (min {d['min_ms']:.2f}, max {d['max_ms']:.2f})")
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--encode", action="store_true", help="time the encoder and the image-decoder loss instead")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("vae_bench.py needs a CUDA device")
     info = gpu_info()
     print("gpu:", info)
+    if args.encode:
+        res = encode_bench(args, info)
+        line = json.dumps(res)
+        print(line)
+        if args.out:
+            os.makedirs(args.out, exist_ok=True)
+            with open(os.path.join(args.out, "vae_bench_encode.json"), "w") as f:
+                f.write(line + "\n")
+        return
     torch.manual_seed(0)
     model = AutoencoderKL().eval().to("cuda", torch.bfloat16).to(memory_format=CL)
     z = torch.randn((args.batch, 4, 64, 64), device="cuda") * 4
