@@ -275,6 +275,32 @@ int mmfs_conv2d_down2x_nhwc(const void *x, const void *w, const void *bias, void
 int mmfs_groupnorm_nhwc(const void *x, const void *gamma, const void *beta, void *y, float *stats, int B, int HW, int C,
                         int G, float eps, int silu, int dtype, void *stream);
 
+/* modes of mmfs_decode_select */
+#define MMFS_SELECT_GREEDY 0
+#define MMFS_SELECT_SAMPLE 1
+
+/*
+ * One decode step's token choice for B rows of fp32 logits (B, V), row stride ld >= V, V <= 131072; one CTA per row.
+ * Replaces, in HF's order (transformers 4.31, generation/logits_process.py): RepetitionPenaltyLogitsProcessor (every
+ * distinct id of out_ids[b, :step] gets s * p if s < 0 else s / p; skipped when p == 1), MinLengthLogitsProcessor
+ * (every eos id -inf while step < min_length), then either the arg-max (MMFS_SELECT_GREEDY; first index wins ties, like
+ * torch.argmax) or TemperatureLogitsWarper + TopPLogitsWarper + the multinomial draw (MMFS_SELECT_SAMPLE): tokens whose
+ * ascending cumulative softmax mass is <= 1 - top_p are dropped, the most likely token is always kept, and tokens tied
+ * exactly at the threshold are all kept (HF's sort keeps an arbitrary subset of them); the id is drawn by inverse CDF
+ * over the kept set in vocabulary order with u = uniforms[b] when uniforms != NULL, else from Philox4x32-10 keyed by
+ * (*seed, b, step).  Then the bookkeeping of the eager loop: a row with finished[b] set emits pad_id, finished[b] |=
+ * (id in eos_ids), and the id is written to out_ids[b, step] and next_ids[b].
+ *   out_ids (B, max_new) int64; step: DEVICE int64 (nothing is written unless 0 <= step < max_new); finished (B) uint8;
+ *   next_ids (B) int64; eos_ids (n_eos) int64 device, NULL iff n_eos == 0; params: DEVICE fp32 {repetition_penalty,
+ *   temperature, top_p}; seed: DEVICE int64, may be NULL in greedy mode or with uniforms; uniforms (B) fp32 or NULL.
+ * The per-call values (step, params, seed) are read on the device, so one captured CUDA graph serves any of them.
+ * Sampling sums the softmax mass in 2^-40 fixed point with integer atomics: the choice is run-to-run reproducible.
+ */
+int mmfs_decode_select(const float *logits, long ld, int64_t *out_ids, const int64_t *step, uint8_t *finished,
+                       int64_t *next_ids, const int64_t *eos_ids, int n_eos, long pad_id, int min_length,
+                       const float *params, const int64_t *seed, const float *uniforms, int B, int V, int max_new,
+                       int mode, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

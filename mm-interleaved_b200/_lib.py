@@ -16,6 +16,7 @@ F32, F16, BF16, F64 = 0, 1, 2, 3
 MSDA_STRICT = 1
 SAMPLER_EXACT_WEIGHTS = 4
 SAMPLER_GENERIC = 8
+SELECT_GREEDY, SELECT_SAMPLE = 0, 1
 
 _lib = None
 
@@ -48,6 +49,7 @@ SIGNATURES = {
     "mmfs_attn_decode_scratch_floats": (_L, [_I] * 4),
     "mmfs_attn_decode": (_I, [_P] * 6 + [_I] * 4 + [_L] * 6 + [_F, _I, _I, _I, _P]),
     "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
+    "mmfs_decode_select": (_I, [_P, _L] + [_P] * 5 + [_I, _L, _I] + [_P] * 3 + [_I] * 4 + [_P]),
 }
 
 

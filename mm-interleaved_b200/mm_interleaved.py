@@ -386,18 +386,23 @@ class ImageDecoder(nn.Module):
         return out
 
 
-class _GraphedGreedyDecoder:
-    """Static state + one CUDA graph of a greedy decode step for ``InterleavedForward`` (see ``enable_decode_graphs``).
+class _GraphedDecoder:
+    """Static state + one CUDA graph of a decode step for ``InterleavedForward`` (see ``enable_decode_graphs``).
 
     Everything that changes from token to token lives in DEVICE tensors the graph updates itself -- the slot the new
     key/value row goes to, the key mask over the whole static cache, the position ids, the step counter, the finished
     flags, the output ids -- so generating N tokens is N ``graph.replay()`` calls with no host synchronisation.  The
     image-side tensors of the cross-attention layers are a ``PreparedVision`` over static storage, refilled eagerly once
-    per call (a graph replay bypasses Python, so nothing inside the graph may depend on a tensor-identity cache)."""
+    per call (a graph replay bypasses Python, so nothing inside the graph may depend on a tensor-identity cache).
 
-    def __init__(self, owner, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new):
+    ``mode``: None = plain greedy (processors + arg-max in torch ops); ``"greedy"`` (with a repetition penalty) and
+    ``"sample"`` (temperature + top-p) choose the token with ``ops.decode_select``, which reads the penalty,
+    temperature, top_p and seed from device buffers written once per call, so one graph serves any of their values."""
+
+    def __init__(self, owner, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, mode=None):
         from .llama_mmfs import PreparedVision
         self.owner, self.B, self.t_max, self.max_new, self.min_length = owner, B, t_max, max_new, int(min_length)
+        self.mode, self.pad_id = mode, int(pad_id)
         model = owner.mm_decoder
         n_img = feats_shape[1]
         self.past = model.static_cache(B, t_max, dtype=dtype, device=device)
@@ -418,6 +423,10 @@ class _GraphedGreedyDecoder:
         self.pad = torch.tensor(int(pad_id), dtype=torch.long, device=device)
         self.neg_inf = torch.tensor(float("-inf"), dtype=torch.float32, device=device)
         self.zero = torch.zeros((), dtype=torch.float32, device=device)
+        if mode is not None:
+            self.params = torch.ones((3,), dtype=torch.float32, device=device)   # penalty, temperature, top_p
+            self.seed = torch.zeros((1,), dtype=torch.long, device=device)
+            self.next_ids = torch.zeros((B, 1), dtype=torch.long, device=device)
         self.graph = None
         self.launches = 0
 
@@ -427,20 +436,27 @@ class _GraphedGreedyDecoder:
             c.length = self.t_max - 1 if on else length
 
     def _step(self):
-        """One token: processors + arg-max on the pending logits, bookkeeping, decoder forward on the chosen token."""
+        """One token: processors + arg-max / draw on the pending logits, bookkeeping, decoder forward on the chosen token."""
+        from . import ops
         o = self.owner
-        scores = self.logits
-        if self.eos is not None and self.min_length > 0:                   # HF MinLengthLogitsProcessor
-            bias = torch.where(self.step < self.min_length, self.neg_inf, self.zero)
-            scores = scores.index_add(1, self.eos, bias.expand(self.B, self.eos.numel()).contiguous())
-        nxt = scores.argmax(-1)
-        if self.eos is not None:
-            nxt = torch.where(self.finished, self.pad, nxt)
-            self.finished.logical_or_((nxt[:, None] == self.eos[None, :]).any(dim=1))
-        self.out_ids.index_copy_(1, self.step, nxt[:, None])
+        if self.mode is None:
+            scores = self.logits
+            if self.eos is not None and self.min_length > 0:               # HF MinLengthLogitsProcessor
+                bias = torch.where(self.step < self.min_length, self.neg_inf, self.zero)
+                scores = scores.index_add(1, self.eos, bias.expand(self.B, self.eos.numel()).contiguous())
+            nxt = scores.argmax(-1)
+            if self.eos is not None:
+                nxt = torch.where(self.finished, self.pad, nxt)
+                self.finished.logical_or_((nxt[:, None] == self.eos[None, :]).any(dim=1))
+            self.out_ids.index_copy_(1, self.step, nxt[:, None])
+            fed = nxt[:, None]
+        else:                                                              # processors, choice and bookkeeping: one kernel
+            ops.decode_select(self.logits, self.out_ids, self.step, self.finished, self.next_ids, self.params, eos=self.eos,
+                              pad_id=self.pad_id, min_length=self.min_length, sample=self.mode == "sample", seed=self.seed)
+            fed = self.next_ids
         self.key_mask.index_fill_(1, self.cur, 1)                          # the fed token's cache slot becomes visible
         self.pos.add_(1)
-        hid = o.mm_decoder(inputs_embeds=o.mm_decoder.embed_tokens(nxt[:, None]), attention_mask=self.key_mask,
+        hid = o.mm_decoder(inputs_embeds=o.mm_decoder.embed_tokens(fed), attention_mask=self.key_mask,
                            position_ids=self.pos, past_key_values=self.past, vision_hidden_states=self.pv,
                            cross_attention_mask=self.cross_last, use_cache=True, return_dict=True).last_hidden_state
         self.logits.copy_(o.text_decoder.logits(hid)[:, -1].float())
@@ -458,12 +474,19 @@ class _GraphedGreedyDecoder:
         self.cross_last.copy_(cross[:, -1:, :])
         self.logits.copy_(logits0)
 
-    def generate(self, mm_embeds, cross, feats, attention_mask, position_ids):
+    def generate(self, mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty=1.0, temperature=1.0,
+                 top_p=1.0, generator=None):
         from . import ops
         o = self.owner
         B, L, _ = mm_embeds.shape
         if L + self.max_new > self.t_max:
             raise RuntimeError("prompt + new tokens exceed the captured cache length")
+        if self.mode is not None:                                           # per-call values the graph reads on the device
+            self.params[0].fill_(float(repetition_penalty))
+            self.params[1].fill_(float(temperature))
+            self.params[2].fill_(float(top_p))
+            if self.mode == "sample":                                       # one seed per call, drawn on the device
+                self.seed.random_(generator=generator)
         o.mm_decoder.prepare_vision(feats, out=self.pv)                     # eager, into the static buffers the graph reads
         self._set_graph_mode(False, 0)
         out = o.mm_decoder(inputs_embeds=mm_embeds, attention_mask=attention_mask, position_ids=position_ids,
@@ -521,28 +544,38 @@ class InterleavedForward(nn.Module):
         self.seq_len = seq_len
         self.image_decoder = image_decoder                                                # ImageDecoder or None
         self._decode_graphs = None                                                        # enable_decode_graphs()
+        self._decode_graph_sampling = False
 
-    def enable_decode_graphs(self, enabled: bool = True) -> "InterleavedForward":
+    def enable_decode_graphs(self, enabled: bool = True, sampling: bool = False) -> "InterleavedForward":
         """Greedy ``generate_texts`` then replays ONE captured CUDA graph per generated token (embedding -> 40 layers ->
         head -> logits processors -> arg-max -> state update, ~1000 kernels) instead of launching them from Python; the
         graph, its static KV cache and input buffers are kept per (batch, cache length, image count) and reused by
-        later calls (SURVEY.md 8 f3; causal_lm_cascade.py:171-204 is the loop it replaces)."""
+        later calls (SURVEY.md 8 f3; causal_lm_cascade.py:171-204 is the loop it replaces).  Greedy decoding with a
+        ``repetition_penalty`` is graphed too (``ops.decode_select``), token-identical to the eager loop.
+
+        ``sampling=True`` also graphs ``use_nucleus_sampling`` (temperature + top-p).  Its draws come from the kernel's
+        counter-based generator (Philox4x32-10 keyed by a per-call seed taken from the caller's ``generator``, by
+        row and by step): a seeded call reproduces itself, but the tokens are NOT those of the eager loop, whose
+        ``torch.multinomial`` consumes the generator differently.  Without it, sampled decoding runs eagerly."""
         self._decode_graphs = {} if enabled else None
+        self._decode_graph_sampling = bool(enabled and sampling)
         return self
 
     @torch.no_grad()
-    def _graphed_greedy(self, mm_embeds, cross, feats, attention_mask, position_ids, max_new_tokens, eos_ids, pad_id, min_length):
+    def _graphed_decode(self, mm_embeds, cross, feats, attention_mask, position_ids, max_new_tokens, eos_ids, pad_id,
+                        min_length, mode, repetition_penalty, temperature, top_p, generator):
         B, L, _ = mm_embeds.shape
         t_max = ((L + max_new_tokens + 255) // 256) * 256                  # cache-length bucket: one graph serves nearby prompts
         key = (B, t_max, tuple(feats.shape), mm_embeds.dtype, mm_embeds.device, tuple(eos_ids), int(pad_id), int(min_length),
-               int(max_new_tokens))
+               int(max_new_tokens), mode)
         dec = self._decode_graphs.get(key)
         if dec is None:
             if len(self._decode_graphs) >= 4:
                 self._decode_graphs.pop(next(iter(self._decode_graphs)))
-            dec = self._decode_graphs[key] = _GraphedGreedyDecoder(self, B, t_max, feats.shape, mm_embeds.dtype, mm_embeds.device,
-                                                                   eos_ids, pad_id, min_length, max_new_tokens)
-        return dec.generate(mm_embeds, cross, feats, attention_mask, position_ids)
+            dec = self._decode_graphs[key] = _GraphedDecoder(self, B, t_max, feats.shape, mm_embeds.dtype, mm_embeds.device,
+                                                             eos_ids, pad_id, min_length, max_new_tokens, mode)
+        return dec.generate(mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty, temperature, top_p,
+                            generator)
 
     def prepare(self, text_ids, visual_output, num_image_per_seq, max_num_image: int):
         st = self.special_token_dict
@@ -603,7 +636,12 @@ class InterleavedForward(nn.Module):
         is suppressed while fewer than ``min_length`` tokens were generated), several ``eos_token_id`` values (the
         reference passes [eos, soi]), and ``use_nucleus_sampling`` = temperature + top-p sampling.  ``num_beams > 1``
         runs HF-style beam search (``_beam_search`` below; the reference's captioning default is 5 beams) and returns
-        (B * num_return_sequences, <= max_new_tokens) padded ids; otherwise (B, max_new_tokens) ids."""
+        (B * num_return_sequences, <= max_new_tokens) padded ids; otherwise (B, max_new_tokens) ids.
+
+        Under ``enable_decode_graphs()`` greedy decoding (with or without the penalty) replays one CUDA graph per token
+        with the eager loop's tokens; nucleus sampling is graphed only after ``enable_decode_graphs(True,
+        sampling=True)``, and then draws from the kernel's Philox stream instead of ``torch.multinomial`` (same
+        distribution, different tokens for a given ``generator`` seed).  Beam search always runs eagerly."""
         if num_beams > 1:
             if use_nucleus_sampling:
                 raise NotImplementedError("beam-sample (num_beams > 1 with sampling) is not implemented")
@@ -616,11 +654,12 @@ class InterleavedForward(nn.Module):
         eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
         mm_embeds, cross, feats = self.prepare(text_ids, visual_output, num_image_per_seq, max_num_image)
         position_ids = (attention_mask.long().cumsum(-1) - 1).masked_fill(attention_mask == 0, 1)   # causal_lm_cascade.py:181-183
-        graphed = (self._decode_graphs is not None and static_cache and not use_nucleus_sampling and
-                   repetition_penalty == 1.0 and text_ids.is_cuda and max_new_tokens > 0)
+        graphed = (self._decode_graphs is not None and static_cache and text_ids.is_cuda and max_new_tokens > 0 and
+                   (not use_nucleus_sampling or self._decode_graph_sampling))
         if graphed:
-            return self._graphed_greedy(mm_embeds, cross, feats, attention_mask, position_ids, max_new_tokens, eos_ids,
-                                        pad_token_id, min_length)
+            mode = "sample" if use_nucleus_sampling else ("greedy" if repetition_penalty != 1.0 else None)
+            return self._graphed_decode(mm_embeds, cross, feats, attention_mask, position_ids, max_new_tokens, eos_ids,
+                                        pad_token_id, min_length, mode, repetition_penalty, temperature, top_p, generator)
         # the image-only half of the 10 cross-attention layers, once per call (PreparedVision)
         feats = self.mm_decoder.prepare_vision(feats)
         # pre-allocated per-layer caches appended in place (the reference's cat-per-token re-copies every layer's cache)

@@ -109,6 +109,51 @@ def rope_qk_append_(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cos: torc
     launch_counter[0] += 1
 
 
+def decode_select(logits: torch.Tensor, out_ids: torch.Tensor, step: torch.Tensor, finished: torch.Tensor,
+                  next_ids: torch.Tensor, params: torch.Tensor, eos: Optional[torch.Tensor] = None, pad_id: int = 0,
+                  min_length: int = 0, sample: bool = False, seed: Optional[torch.Tensor] = None,
+                  uniforms: Optional[torch.Tensor] = None) -> None:
+    """One decode step's token choice in one kernel (csrc/decode_select_sm100.cu): HF's repetition penalty and
+    min-length processors on the fp32 ``logits`` (B, V), then the arg-max or (``sample``) temperature + top-p sampling,
+    then the finished / pad bookkeeping; the id is written to ``out_ids[:, step]`` and ``next_ids``.  ``step`` (1,)
+    int64, ``params`` (3,) fp32 ``[repetition_penalty, temperature, top_p]`` and ``seed`` (1,) int64 are read on the
+    device (a captured graph serves any of their values); ``finished`` (B,) bool / uint8 is updated in place;
+    ``uniforms`` (B,) fp32 replaces the Philox draw when given."""
+    inference_only("decode_select", logits)
+    _require(logits.is_cuda and logits.dim() == 2 and logits.dtype == torch.float32 and logits.stride(1) == 1,
+             "decode_select: logits must be a CUDA fp32 (B, V) tensor with unit column stride")
+    B, V = logits.shape
+    dev = logits.device
+    _require(out_ids.device == dev and out_ids.dtype == torch.int64 and out_ids.dim() == 2 and out_ids.shape[0] == B
+             and out_ids.is_contiguous(), "decode_select: out_ids must be contiguous int64 (B, max_new) on the logits' device")
+    _require(step.device == dev and step.dtype == torch.int64 and step.numel() == 1, "decode_select: step must be a (1,) int64 device tensor")
+    _require(finished.device == dev and finished.dtype in (torch.bool, torch.uint8) and finished.numel() == B
+             and finished.is_contiguous(), "decode_select: finished must be contiguous bool / uint8 with B entries")
+    _require(next_ids.device == dev and next_ids.dtype == torch.int64 and next_ids.numel() == B and next_ids.is_contiguous(),
+             "decode_select: next_ids must be contiguous int64 with B entries")
+    _require(params.device == dev and params.dtype == torch.float32 and params.numel() == 3 and params.is_contiguous(),
+             "decode_select: params must be a contiguous (3,) fp32 device tensor [repetition_penalty, temperature, top_p]")
+    if eos is not None:
+        _require(eos.device == dev and eos.dtype == torch.int64 and eos.dim() == 1 and eos.is_contiguous(),
+                 "decode_select: eos must be a contiguous 1-D int64 device tensor")
+    if seed is not None:
+        _require(seed.device == dev and seed.dtype == torch.int64 and seed.numel() == 1, "decode_select: seed must be a (1,) int64 device tensor")
+    _require(not sample or seed is not None or uniforms is not None, "decode_select: sampling needs a seed or uniforms")
+    if uniforms is not None:
+        _require(uniforms.device == dev and uniforms.dtype == torch.float32 and uniforms.numel() == B and uniforms.is_contiguous(),
+                 "decode_select: uniforms must be contiguous fp32 with B entries")
+    seed_ptr = seed.data_ptr() if seed is not None else None
+    with torch.cuda.device(dev):
+        rc = _lib.lib().mmfs_decode_select(logits.data_ptr(), logits.stride(0), out_ids.data_ptr(), step.data_ptr(),
+                                           finished.data_ptr(), next_ids.data_ptr(), eos.data_ptr() if eos is not None else None,
+                                           eos.numel() if eos is not None else 0, int(pad_id), int(min_length),
+                                           params.data_ptr(), seed_ptr, uniforms.data_ptr() if uniforms is not None else None,
+                                           B, V, out_ids.shape[1], _lib.SELECT_SAMPLE if sample else _lib.SELECT_GREEDY,
+                                           _stream())
+    _lib.check(rc, "decode_select")
+    launch_counter[0] += 1
+
+
 def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
     """act_fn(gate) * up on a (..., 2*I) tensor holding [gate | up] (LlamaMLP, :188-189)."""
     inference_only("swiglu", gate_up)
