@@ -301,6 +301,47 @@ int mmfs_decode_select(const float *logits, long ld, int64_t *out_ids, const int
                        const float *params, const int64_t *seed, const float *uniforms, int B, int V, int max_new,
                        int mode, void *stream);
 
+/*
+ * One step of beam search for B sequences of num_beams rows each (R = B * num_beams rows of fp32 logits, row stride
+ * ld >= V, V <= 131072): the scoring and BeamSearchScorer.process of HF beam_search (transformers 4.31,
+ * early_stopping=False), in two launches (rows, then sequences).  Per row: log_softmax, RepetitionPenaltyLogitsProcessor
+ * on the log-probs of every distinct id of history[r, :step] (s * p if s < 0 else s * (1/p), the fp32 reciprocal, as
+ * mmfs_decode_select), MinLengthLogitsProcessor (eos ids -inf while step < min_length), + beam_scores[r], and the row's
+ * top K with K = max(2, 1 + n_eos) * num_beams.  Per sequence: the top K of its rows' union, ordered by higher score
+ * first and, on exactly equal scores, by the lower flat index row_in_group * V + token (torch.topk leaves that order
+ * unspecified); then, in rank order, an eos candidate of rank < num_beams becomes a hypothesis scored
+ * sum_logprobs / max(step, 1) ** length_penalty (double), an eos candidate of rank >= num_beams is skipped, non-eos
+ * candidates fill the num_beams next beams (slots left over get pad_id, score 0, parent b * num_beams).  A sequence is
+ * done once it holds num_beams hypotheses whose worst is >= best candidate / (step + 1) ** length_penalty.  A sequence
+ * already done emits pad_id, score 0 and parent b * num_beams and changes no hypothesis.  Writes beam_scores, next_ids
+ * and parent (absolute row index) per row, reorders history by parent and appends the new token at column step.
+ *   params: DEVICE double {repetition_penalty, length_penalty}; step: DEVICE int64 (nothing is done unless
+ *   0 <= step < max_new); history (R, max_new) int64; beam_scores (R) fp32; next_ids, parent (R) int64; done (B) uint8;
+ *   hypotheses, num_beams slots per sequence: hyp_scores (B, num_beams) double, hyp_ids (B, num_beams, max_new) int64,
+ *   hyp_meta (B, num_beams, 2) int64 {length, insertion serial}, length -1 = free slot.  A full set replaces its first
+ *   (lowest serial) lowest-scored hypothesis, so sorting by serial gives the eager loop's list order.
+ *   eos_ids (n_eos) int64 device, NULL iff n_eos == 0; scratch: R * K uint64 of device memory private to the call.
+ * Limits: num_beams <= 8, n_eos <= 4, K <= V; outside them MMFS_EINVAL.  The per-call values (step, params) are read
+ * on the device, so one captured CUDA graph serves any of them.
+ */
+int mmfs_beam_select(const float *logits, long ld, const int64_t *step, const double *params, float *beam_scores,
+                     int64_t *history, int64_t *next_ids, int64_t *parent, uint8_t *done, double *hyp_scores,
+                     int64_t *hyp_ids, int64_t *hyp_meta, const int64_t *eos_ids, int n_eos, long pad_id, int min_length,
+                     uint64_t *scratch, int B, int num_beams, int V, int max_new, void *stream);
+
+/*
+ * The KV-cache reorder of beam search, in place and over the generated positions only: for each of n_caches cache
+ * tensors (base pointer cache + i * cache_stride bytes) and each group of num_beams rows, row j gets the contents of
+ * row parent[j] (an absolute row index in the same group) at positions [*cur - *step, *cur); the prompt positions are
+ * identical across the beams of a sequence and are left alone.  Groups with done[g] set are skipped (done may be NULL).
+ * Row r, position p of cache i starts at cache + i * cache_stride + r * row_stride + p * pos_stride and holds row_bytes
+ * bytes.  cur, step: DEVICE int64; *step <= max_positions (the grid covers max_positions positions).  The pointer,
+ * strides and row_bytes must be multiples of 16 bytes; num_beams <= 8 and rows % num_beams == 0, else MMFS_EINVAL.
+ */
+int mmfs_kv_beam_reorder(void *cache, int n_caches, long cache_stride, int rows, long row_stride, long pos_stride,
+                         long row_bytes, int num_beams, const int64_t *parent, const int64_t *cur, const int64_t *step,
+                         const uint8_t *done, int max_positions, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -149,6 +149,14 @@ class StaticKV:
         # attends over the WHOLE buffer under the caller's key mask, and ``length`` stays pinned at max_len - 1.
         self.slot = None
 
+    @classmethod
+    def over(cls, k, v) -> "StaticKV":
+        """An empty cache over existing (B, T_max, H, hd) storage, e.g. views of one tensor holding every layer's k and v
+        (the graphed beam search reorders all of them in one launch)."""
+        c = cls.__new__(cls)
+        c.k, c.v, c.length, c.slot = k, v, 0, None
+        return c
+
 
 class PreparedVision:
     """Image-side state of the MMFS cross-attention layers for ONE batch of images: per layer, ``value`` =

@@ -397,38 +397,64 @@ class _GraphedDecoder:
 
     ``mode``: None = plain greedy (processors + arg-max in torch ops); ``"greedy"`` (with a repetition penalty) and
     ``"sample"`` (temperature + top-p) choose the token with ``ops.decode_select``, which reads the penalty,
-    temperature, top_p and seed from device buffers written once per call, so one graph serves any of their values."""
+    temperature, top_p and seed from device buffers written once per call, so one graph serves any of their values.
+    ``"beam"``: beam search over B * num_beams rows (``generate_beams``); the step is ``ops.beam_select`` (scores,
+    hypotheses, done flags, history) -> ``ops.kv_beam_reorder`` (the generated positions of every layer's K and V, held
+    in one tensor ``kv``) -> the decoder on the next tokens, with the repetition and length penalties in a device
+    buffer.  ``finished`` then holds the per-sequence done flags."""
 
-    def __init__(self, owner, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, mode=None):
-        from .llama_mmfs import PreparedVision
+    def __init__(self, owner, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, mode=None,
+                 num_beams=1):
+        from . import ops
+        from .llama_mmfs import PreparedVision, StaticKV
         self.owner, self.B, self.t_max, self.max_new, self.min_length = owner, B, t_max, max_new, int(min_length)
-        self.mode, self.pad_id = mode, int(pad_id)
+        self.mode, self.pad_id, self.nb = mode, int(pad_id), int(num_beams)
+        R = B * self.nb                                                     # decoder rows: one per beam
         model = owner.mm_decoder
         n_img = feats_shape[1]
-        self.past = model.static_cache(B, t_max, dtype=dtype, device=device)
-        self.pv = PreparedVision(feats_shape)
+        if mode == "beam":
+            H = model.config.num_attention_heads
+            self.kv = torch.zeros((2 * len(model.layers), R, t_max, H, model.config.hidden_size // H), dtype=dtype,
+                                  device=device)
+            self.past = [StaticKV.over(self.kv[2 * i], self.kv[2 * i + 1]) for i in range(len(model.layers))]
+        else:
+            self.past = model.static_cache(B, t_max, dtype=dtype, device=device)
+        self.pv = PreparedVision((R,) + tuple(feats_shape[1:]))
         probe = model.prepare_vision(torch.zeros(feats_shape, dtype=dtype, device=device))
         for idx, val in probe.values.items():
-            self.pv.values[idx] = torch.empty_like(val)
+            self.pv.values[idx] = val.new_empty((R,) + tuple(val.shape[1:]))
         V = owner.text_decoder.head.weight.shape[0]
-        self.logits = torch.zeros((B, V), dtype=torch.float32, device=device)
-        self.key_mask = torch.zeros((B, t_max), dtype=torch.uint8, device=device)
-        self.pos = torch.zeros((B, 1), dtype=torch.long, device=device)
+        self.logits = torch.zeros((R, V), dtype=torch.float32, device=device)
+        self.key_mask = torch.zeros((R, t_max), dtype=torch.uint8, device=device)
+        self.pos = torch.zeros((R, 1), dtype=torch.long, device=device)
         self.cur = torch.zeros((1,), dtype=torch.long, device=device)
         self.step = torch.zeros((1,), dtype=torch.long, device=device)
         self.finished = torch.zeros((B,), dtype=torch.bool, device=device)
         self.out_ids = torch.zeros((B, max_new), dtype=torch.long, device=device)
-        self.cross_last = torch.zeros((B, 1, n_img), dtype=torch.float32, device=device)
+        self.cross_last = torch.zeros((R, 1, n_img), dtype=torch.float32, device=device)
         self.eos = torch.tensor(eos_ids, dtype=torch.long, device=device) if eos_ids else None
         self.pad = torch.tensor(int(pad_id), dtype=torch.long, device=device)
         self.neg_inf = torch.tensor(float("-inf"), dtype=torch.float32, device=device)
         self.zero = torch.zeros((), dtype=torch.float32, device=device)
         if mode is not None:
+            self.next_ids = torch.zeros((R, 1), dtype=torch.long, device=device)
+        if mode in ("greedy", "sample"):
             self.params = torch.ones((3,), dtype=torch.float32, device=device)   # penalty, temperature, top_p
             self.seed = torch.zeros((1,), dtype=torch.long, device=device)
-            self.next_ids = torch.zeros((B, 1), dtype=torch.long, device=device)
+        if mode == "beam":
+            nb = self.nb
+            self.params = torch.ones((2,), dtype=torch.float64, device=device)   # repetition_penalty, length_penalty
+            self.beam_scores = torch.zeros((R,), dtype=torch.float32, device=device)
+            self.history = torch.zeros((R, max_new), dtype=torch.long, device=device)
+            self.parent = torch.zeros((R,), dtype=torch.long, device=device)
+            self.hyp_scores = torch.zeros((B, nb), dtype=torch.float64, device=device)
+            self.hyp_ids = torch.zeros((B, nb, max_new), dtype=torch.long, device=device)
+            self.hyp_meta = torch.zeros((B, nb, 2), dtype=torch.long, device=device)          # length (-1: free), serial
+            self.scratch = torch.zeros((R * ops.beam_candidates(nb, len(eos_ids)),), dtype=torch.long, device=device)
+            self.all_done = torch.zeros((1,), dtype=torch.bool).pin_memory()                 # written by every replay
         self.graph = None
         self.launches = 0
+        self.replays = 0
 
     def _set_graph_mode(self, on: bool, length: int = 0):
         for c in self.past:
@@ -450,6 +476,12 @@ class _GraphedDecoder:
                 self.finished.logical_or_((nxt[:, None] == self.eos[None, :]).any(dim=1))
             self.out_ids.index_copy_(1, self.step, nxt[:, None])
             fed = nxt[:, None]
+        elif self.mode == "beam":                                          # scorer, then the cache follows the parents
+            ops.beam_select(self.logits, self.step, self.params, self.beam_scores, self.history, self.next_ids,
+                            self.parent, self.finished, self.hyp_scores, self.hyp_ids, self.hyp_meta, self.scratch,
+                            self.nb, eos=self.eos, pad_id=self.pad_id, min_length=self.min_length)
+            ops.kv_beam_reorder(self.kv, self.parent, self.cur, self.step, self.nb, self.max_new, done=self.finished)
+            fed = self.next_ids
         else:                                                              # processors, choice and bookkeeping: one kernel
             ops.decode_select(self.logits, self.out_ids, self.step, self.finished, self.next_ids, self.params, eos=self.eos,
                               pad_id=self.pad_id, min_length=self.min_length, sample=self.mode == "sample", seed=self.seed)
@@ -462,6 +494,8 @@ class _GraphedDecoder:
         self.logits.copy_(o.text_decoder.logits(hid)[:, -1].float())
         self.step.add_(1)
         self.cur.add_(1)
+        if self.mode == "beam":                                            # read by the host two replays later
+            self.all_done.copy_(self.finished.all().view(1), non_blocking=True)
 
     def _reset(self, L, attention_mask, position_ids, cross, logits0):
         self.key_mask.zero_()
@@ -473,6 +507,43 @@ class _GraphedDecoder:
         self.out_ids.fill_(int(self.pad))
         self.cross_last.copy_(cross[:, -1:, :])
         self.logits.copy_(logits0)
+        if self.mode == "beam":
+            self.beam_scores.fill_(-1e9)
+            self.beam_scores[::self.nb] = 0.0                              # only the first beam of a sequence is live
+            self.history.fill_(self.pad_id)
+            self.hyp_scores.zero_()
+            self.hyp_meta.fill_(-1)
+
+    def _prefill_done(self, L, reset):
+        """After the prefill: zero the unused cache slots, capture the step graph once, reset the per-call state."""
+        from . import ops
+        o = self.owner
+        for c in self.past:                                                 # masked slots must hold finite numbers
+            c.k[:, L:].zero_()
+            c.v[:, L:].zero_()
+        self._set_graph_mode(True)
+        if self.graph is None:
+            reset()
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                for _ in range(2):                                          # lazy handles, weight-derived caches, RoPE tables
+                    reset()                                                 # every warm-up step is step 0
+                    self._step()
+            torch.cuda.current_stream().wait_stream(side)
+            reset()
+            before = ops.launch_counter[0]
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph):
+                self._step()
+            self.launches = ops.launch_counter[0] - before
+            # the graph reads the RoPE tables by address: keep the captured storage alive even if an eager decode grows
+            # (and so replaces) the shared tables later
+            self._captured_rope = [l.self_attn._rope for l in o.mm_decoder.layers]
+            for c in self.past:                                             # the warm-up steps wrote slots L, L+1
+                c.k[:, L:].zero_()
+                c.v[:, L:].zero_()
+        reset()
 
     def generate(self, mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty=1.0, temperature=1.0,
                  top_p=1.0, generator=None):
@@ -493,37 +564,59 @@ class _GraphedDecoder:
                            past_key_values=self.past, vision_hidden_states=self.pv, cross_attention_mask=cross,
                            use_cache=True, return_dict=True)               # prefill straight into the static cache
         logits0 = o.text_decoder.logits(out.last_hidden_state[:, -1:])[:, -1].float()
-        for c in self.past:                                                 # masked slots must hold finite numbers
-            c.k[:, L:].zero_()
-            c.v[:, L:].zero_()
-        self._set_graph_mode(True)
-        if self.graph is None:
-            self._reset(L, attention_mask, position_ids, cross, logits0)
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                for _ in range(2):                                          # lazy handles, weight-derived caches, RoPE tables
-                    self._reset(L, attention_mask, position_ids, cross, logits0)   # every warm-up step is step 0
-                    self._step()
-            torch.cuda.current_stream().wait_stream(side)
-            self._reset(L, attention_mask, position_ids, cross, logits0)
-            before = ops.launch_counter[0]
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self._step()
-            self.launches = ops.launch_counter[0] - before
-            # the graph reads the RoPE tables by address: keep the captured storage alive even if an eager decode grows
-            # (and so replaces) the shared tables later
-            self._captured_rope = [l.self_attn._rope for l in o.mm_decoder.layers]
-            for c in self.past:                                             # the warm-up steps wrote slots L, L+1
-                c.k[:, L:].zero_()
-                c.v[:, L:].zero_()
-        self._reset(L, attention_mask, position_ids, cross, logits0)
+        self._prefill_done(L, lambda: self._reset(L, attention_mask, position_ids, cross, logits0))
         for _ in range(self.max_new):
             self.graph.replay()
         ops.launch_counter[0] += self.launches * self.max_new
         self._set_graph_mode(False, L)
         return self.out_ids.clone()
+
+    def generate_beams(self, mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty=1.0,
+                       length_penalty=1.0):
+        """Beam search (``mode == "beam"``): the prompt is prefilled once per sequence and its cache rows, the
+        ``PreparedVision`` values, key mask, position ids and last cross-attention row are replicated to the beams;
+        then one replay per step.  At most two replays are in flight: before enqueuing replay t the host waits for
+        replay t - 2 and reads the "all sequences done" flag it copied to pinned memory, so decoding stops at most two
+        steps after the eager loop would (done sequences are inert).  Returns the host copies of the final state."""
+        from . import ops
+        o = self.owner
+        B, L, _ = mm_embeds.shape
+        if L + self.max_new > self.t_max:
+            raise RuntimeError("prompt + new tokens exceed the captured cache length")
+        self.params[0].fill_(float(repetition_penalty))
+        self.params[1].fill_(float(length_penalty))
+        rep = torch.arange(B, device=mm_embeds.device).repeat_interleave(self.nb)   # beam row -> sequence
+        pv = o.mm_decoder.prepare_vision(feats)                             # the prefill's B rows, then one per beam
+        for idx, val in pv.values.items():
+            torch.index_select(val, 0, rep, out=self.pv.values[idx])
+        pre = o.mm_decoder.static_cache(B, L, dtype=mm_embeds.dtype, device=mm_embeds.device)
+        out = o.mm_decoder(inputs_embeds=mm_embeds, attention_mask=attention_mask, position_ids=position_ids,
+                           past_key_values=pre, vision_hidden_states=pv, cross_attention_mask=cross, use_cache=True,
+                           return_dict=True)
+        logits0 = o.text_decoder.logits(out.last_hidden_state[:, -1:])[:, -1].float().index_select(0, rep)
+        for dst, src in zip(self.past, pre):                                # a copy of the prompt rows, no recompute
+            dst.k[:, :L].copy_(src.k.index_select(0, rep))
+            dst.v[:, :L].copy_(src.v.index_select(0, rep))
+        del pre, pv
+        mask_r, pos_r, cross_r = (t.index_select(0, rep) for t in (attention_mask, position_ids, cross[:, -1:, :]))
+        self._prefill_done(L, lambda: self._reset(L, mask_r, pos_r, cross_r, logits0))
+        torch.cuda.current_stream().synchronize()                           # no copy into all_done is pending
+        self.all_done.zero_()
+        events = (torch.cuda.Event(), torch.cuda.Event())
+        n = 0
+        for t in range(self.max_new):
+            if t >= 2:
+                events[t % 2].synchronize()                                 # replay t - 2 has finished
+                if bool(self.all_done[0]):
+                    break
+            self.graph.replay()
+            events[t % 2].record()
+            n += 1
+        self.replays = n
+        ops.launch_counter[0] += self.launches * n
+        self._set_graph_mode(False, L)
+        return dict(history=self.history[:, :n].cpu(), beam_scores=self.beam_scores.cpu(), done=self.finished.cpu(),
+                    hyp_scores=self.hyp_scores.cpu(), hyp_ids=self.hyp_ids.cpu(), hyp_meta=self.hyp_meta.cpu())
 
 
 class InterleavedForward(nn.Module):
@@ -556,24 +649,34 @@ class InterleavedForward(nn.Module):
         ``sampling=True`` also graphs ``use_nucleus_sampling`` (temperature + top-p).  Its draws come from the kernel's
         counter-based generator (Philox4x32-10 keyed by a per-call seed taken from the caller's ``generator``, by
         row and by step): a seeded call reproduces itself, but the tokens are NOT those of the eager loop, whose
-        ``torch.multinomial`` consumes the generator differently.  Without it, sampled decoding runs eagerly."""
+        ``torch.multinomial`` consumes the generator differently.  Without it, sampled decoding runs eagerly.
+
+        Beam search (``num_beams > 1``, within ``ops.beam_select_supported``: at most 8 beams and 4 eos ids) is graphed
+        too: one replay per step of ``ops.beam_select`` + ``ops.kv_beam_reorder`` + the decoder, with the eager loop's
+        tokens.  One caveat: the kernel's log-softmax sums in a different order from ``torch.log_softmax``, so graphed
+        and eager tokens can differ where two candidates' scores are within a few fp32 ulps of each other."""
         self._decode_graphs = {} if enabled else None
         self._decode_graph_sampling = bool(enabled and sampling)
         return self
 
-    @torch.no_grad()
-    def _graphed_decode(self, mm_embeds, cross, feats, attention_mask, position_ids, max_new_tokens, eos_ids, pad_id,
-                        min_length, mode, repetition_penalty, temperature, top_p, generator):
+    def _decode_graph(self, mm_embeds, feats, max_new_tokens, eos_ids, pad_id, min_length, mode, num_beams=1):
+        """The ``_GraphedDecoder`` for this shape and these settings, built on first use (at most four are kept)."""
         B, L, _ = mm_embeds.shape
         t_max = ((L + max_new_tokens + 255) // 256) * 256                  # cache-length bucket: one graph serves nearby prompts
         key = (B, t_max, tuple(feats.shape), mm_embeds.dtype, mm_embeds.device, tuple(eos_ids), int(pad_id), int(min_length),
-               int(max_new_tokens), mode)
+               int(max_new_tokens), int(num_beams), mode)
         dec = self._decode_graphs.get(key)
         if dec is None:
             if len(self._decode_graphs) >= 4:
                 self._decode_graphs.pop(next(iter(self._decode_graphs)))
             dec = self._decode_graphs[key] = _GraphedDecoder(self, B, t_max, feats.shape, mm_embeds.dtype, mm_embeds.device,
-                                                             eos_ids, pad_id, min_length, max_new_tokens, mode)
+                                                             eos_ids, pad_id, min_length, max_new_tokens, mode, num_beams)
+        return dec
+
+    @torch.no_grad()
+    def _graphed_decode(self, mm_embeds, cross, feats, attention_mask, position_ids, max_new_tokens, eos_ids, pad_id,
+                        min_length, mode, repetition_penalty, temperature, top_p, generator):
+        dec = self._decode_graph(mm_embeds, feats, max_new_tokens, eos_ids, pad_id, min_length, mode)
         return dec.generate(mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty, temperature, top_p,
                             generator)
 
@@ -641,17 +744,26 @@ class InterleavedForward(nn.Module):
         Under ``enable_decode_graphs()`` greedy decoding (with or without the penalty) replays one CUDA graph per token
         with the eager loop's tokens; nucleus sampling is graphed only after ``enable_decode_graphs(True,
         sampling=True)``, and then draws from the kernel's Philox stream instead of ``torch.multinomial`` (same
-        distribution, different tokens for a given ``generator`` seed).  Beam search always runs eagerly."""
+        distribution, different tokens for a given ``generator`` seed).  Beam search replays one graph per step when
+        its sizes are within ``ops.beam_select_supported`` (else it runs the eager loop), with the eager loop's tokens
+        except where two candidates' scores lie within a few fp32 ulps (the kernel's log-softmax sums in another
+        order than ``torch.log_softmax``)."""
+        from . import ops
+        eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
         if num_beams > 1:
             if use_nucleus_sampling:
                 raise NotImplementedError("beam-sample (num_beams > 1 with sampling) is not implemented")
-            return self._beam_search(text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, max_new_tokens,
-                                     eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams, length_penalty,
-                                     num_return_sequences)
+            beam_args = (text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, max_new_tokens,
+                         eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams, length_penalty,
+                         num_return_sequences)
+            V = self.text_decoder.head.weight.shape[0]
+            if (self._decode_graphs is not None and text_ids.is_cuda and max_new_tokens > 0
+                    and ops.beam_select_supported(num_beams, len(eos_ids), V)):
+                return self._graphed_beam_search(*beam_args)
+            return self._beam_search(*beam_args)
         B, L = text_ids.shape
         if attention_mask is None:
             attention_mask = torch.ones((B, L), dtype=torch.long, device=text_ids.device)
-        eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
         mm_embeds, cross, feats = self.prepare(text_ids, visual_output, num_image_per_seq, max_num_image)
         position_ids = (attention_mask.long().cumsum(-1) - 1).masked_fill(attention_mask == 0, 1)   # causal_lm_cascade.py:181-183
         graphed = (self._decode_graphs is not None and static_cache and text_ids.is_cuda and max_new_tokens > 0 and
@@ -710,11 +822,12 @@ class InterleavedForward(nn.Module):
                      eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams, length_penalty, num_return):
         """Beam search with the bookkeeping of HF ``GenerationMixin.beam_search`` + ``BeamSearchScorer`` (transformers
         4.31, the version the reference pins; ``early_stopping=False``, one beam group): log-softmax scores, logits
-        processors on the log-probabilities, top 2*num_beams candidates per sequence, finished hypotheses ranked by
-        ``sum_logprobs / len(generated) ** length_penalty``, a sequence is done once ``num_beams`` hypotheses are all
-        at least as good as the best running beam could become.  The prompt is prefilled ONCE per sequence and its
-        cache rows are replicated per beam; every step re-gathers the cache rows by beam index (``_reorder_cache``)."""
-        from .llama_mmfs import StaticKV
+        processors on the log-probabilities, top ``max(2, 1 + n_eos) * num_beams`` candidates per sequence (the
+        reference's own beam search, beam_search_monkey_patch.py:265-269: enough that ``num_beams`` of them are never
+        eos), finished hypotheses ranked by ``sum_logprobs / len(generated) ** length_penalty``, a sequence is done once
+        ``num_beams`` hypotheses are all at least as good as the best running beam could become.  The prompt is
+        prefilled ONCE per sequence and its cache rows are replicated per beam; every step re-gathers the cache rows by
+        beam index (``_reorder_cache``)."""
         B, L = text_ids.shape
         nb, dev = num_beams, text_ids.device
         if attention_mask is None:
@@ -739,17 +852,9 @@ class InterleavedForward(nn.Module):
         beam_scores[:, 1:] = -1e9
         beam_scores = beam_scores.view(-1)
         seqs = torch.zeros((B * nb, 0), dtype=torch.long, device=dev)              # generated ids per beam row
-        hyps = [[] for _ in range(B)]                                              # per sequence: (score, ids list)
-        worst = [1e9] * B
+        hyps = [_BeamHypotheses(nb, length_penalty) for _ in range(B)]
         done = [False] * B
-
-        def add_hyp(b, ids, sum_logprobs):
-            score = sum_logprobs / (max(len(ids), 1) ** length_penalty)
-            if len(hyps[b]) < nb or score > worst[b]:
-                hyps[b].append((score, ids))
-                if len(hyps[b]) > nb:
-                    hyps[b].remove(min(hyps[b], key=lambda h: h[0]))
-                worst[b] = min(h[0] for h in hyps[b])
+        n_cand = max(2, 1 + len(eos_ids)) * nb
 
         for step_idx in range(max_new_tokens):
             scores = torch.log_softmax(logits[:, -1].float(), dim=-1)
@@ -760,7 +865,7 @@ class InterleavedForward(nn.Module):
                 scores[:, eos_ids] = float("-inf")
             V = scores.shape[-1]
             cand = (scores + beam_scores[:, None]).view(B, nb * V)
-            top_s, top_i = cand.topk(2 * nb, dim=1, largest=True, sorted=True)
+            top_s, top_i = cand.topk(n_cand, dim=1, largest=True, sorted=True)
             top_s_h, top_i_h, seqs_h = top_s.tolist(), top_i.tolist(), seqs.tolist()   # one host round trip per step
             cur_len = seqs.shape[1] + 1
             nxt_scores = [[0.0] * nb for _ in range(B)]
@@ -775,13 +880,13 @@ class InterleavedForward(nn.Module):
                     if tok in eos_ids:
                         if rank >= nb:
                             continue
-                        add_hyp(b, seqs_h[row], sc)
+                        hyps[b].add(seqs_h[row], sc)
                     else:
                         nxt_scores[b][k], nxt_tokens[b][k], nxt_rows[b][k] = sc, tok, row
                         k += 1
                     if k == nb:
                         break
-                if len(hyps[b]) >= nb and worst[b] >= top_s_h[b][0] / (cur_len ** length_penalty):
+                if len(hyps[b].beams) >= nb and hyps[b].worst >= top_s_h[b][0] / (cur_len ** length_penalty):
                     done[b] = True
             beam_scores = torch.tensor(nxt_scores, dtype=torch.float32, device=dev).view(-1)
             tok_t = torch.tensor(nxt_tokens, dtype=torch.long, device=dev).view(-1)
@@ -798,25 +903,73 @@ class InterleavedForward(nn.Module):
                                    past_key_values=past, vision_hidden_states=feats_b, cross_attention_mask=last_cross,
                                    use_cache=True, return_dict=True)
             logits = self.text_decoder.logits(step.last_hidden_state)
+        return _beam_finalize(hyps, done, seqs.tolist(), beam_scores.tolist(), num_return, max_new_tokens, pad_token_id,
+                              eos_ids).to(dev)
 
-        # finalize: running beams of unfinished sequences become hypotheses; best `num_return` per sequence
-        seqs_h, bs_h = seqs.tolist(), beam_scores.tolist()
-        for b in range(B):
-            if not done[b]:
-                for j in range(nb):
-                    add_hyp(b, seqs_h[b * nb + j], bs_h[b * nb + j])
-        best = []
-        for b in range(B):
-            ranked = sorted(hyps[b], key=lambda h: h[0])
-            for _ in range(num_return):
-                best.append(ranked.pop()[1])
-        width = min(max(len(x) for x in best) + 1, max_new_tokens)
-        out_ids = torch.full((len(best), width), pad_token_id, dtype=torch.long)
-        for i, x in enumerate(best):
-            out_ids[i, :len(x)] = torch.tensor(x, dtype=torch.long)
-            if len(x) < width and eos_ids:
-                out_ids[i, len(x)] = eos_ids[0]
-        return out_ids.to(dev)
+    @torch.no_grad()
+    def _graphed_beam_search(self, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask,
+                             max_new_tokens, eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams,
+                             length_penalty, num_return):
+        """``_beam_search`` on one CUDA graph replay per step (``_GraphedDecoder`` in beam mode); same arguments, same
+        finalize."""
+        B, L = text_ids.shape
+        nb = num_beams
+        if attention_mask is None:
+            attention_mask = torch.ones((B, L), dtype=torch.long, device=text_ids.device)
+        eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
+        mm_embeds, cross, feats = self.prepare(text_ids, visual_output, num_image_per_seq, max_num_image)
+        position_ids = (attention_mask.long().cumsum(-1) - 1).masked_fill(attention_mask == 0, 1)   # causal_lm_cascade.py:181-183
+        dec = self._decode_graph(mm_embeds, feats, max_new_tokens, eos_ids, pad_token_id, min_length, "beam", nb)
+        st = dec.generate_beams(mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty, length_penalty)
+        hyps = []
+        for b in range(B):                                                 # the slots in insertion order
+            meta, ids, sc = st["hyp_meta"][b].tolist(), st["hyp_ids"][b].tolist(), st["hyp_scores"][b].tolist()
+            slots = sorted((m[1], j) for j, m in enumerate(meta) if m[0] >= 0)
+            hyps.append(_BeamHypotheses(nb, length_penalty, [(sc[j], ids[j][:meta[j][0]]) for _, j in slots]))
+        done = [bool(d) for d in st["done"].tolist()]
+        return _beam_finalize(hyps, done, st["history"].tolist(), st["beam_scores"].tolist(), num_return, max_new_tokens,
+                              pad_token_id, eos_ids).to(text_ids.device)
+
+
+class _BeamHypotheses:
+    """The finished hypotheses of one sequence as HF's ``BeamHypotheses`` keeps them (``early_stopping=False``):
+    ``(score, ids)`` in insertion order, at most ``num_beams``; a full set drops its first lowest-scored entry."""
+
+    def __init__(self, num_beams, length_penalty, beams=()):
+        self.num_beams, self.length_penalty = num_beams, length_penalty
+        self.beams = list(beams)
+        self.worst = min((h[0] for h in self.beams), default=1e9)
+
+    def add(self, ids, sum_logprobs):
+        score = sum_logprobs / (max(len(ids), 1) ** self.length_penalty)
+        if len(self.beams) < self.num_beams or score > self.worst:
+            self.beams.append((score, ids))
+            if len(self.beams) > self.num_beams:
+                self.beams.remove(min(self.beams, key=lambda h: h[0]))
+            self.worst = min(h[0] for h in self.beams)
+
+
+def _beam_finalize(hyps, done, seqs, beam_scores, num_return, max_new_tokens, pad_token_id, eos_ids):
+    """End of beam search (eager and graphed): the running beams of unfinished sequences become hypotheses, the best
+    ``num_return`` per sequence are returned as (B * num_return, width) ids on the CPU, padded with ``pad_token_id``
+    after one ``eos_ids[0]``; width = min(longest + 1, max_new_tokens)."""
+    nb = len(seqs) // len(hyps)
+    for b, h in enumerate(hyps):
+        if not done[b]:
+            for j in range(nb):
+                h.add(seqs[b * nb + j], beam_scores[b * nb + j])
+    best = []
+    for h in hyps:
+        ranked = sorted(h.beams, key=lambda x: x[0])
+        for _ in range(num_return):
+            best.append(ranked.pop()[1])
+    width = min(max(len(x) for x in best) + 1, max_new_tokens)
+    out_ids = torch.full((len(best), width), pad_token_id, dtype=torch.long)
+    for i, x in enumerate(best):
+        out_ids[i, :len(x)] = torch.tensor(x, dtype=torch.long)
+        if len(x) < width and eos_ids:
+            out_ids[i, len(x)] = eos_ids[0]
+    return out_ids
 
 
 def _llm_config_from(llm_config, llm_model_path, txt_vocab_size, image_embed_dim, cross_attention_frequency, spatial_shapes):

@@ -154,6 +154,104 @@ def decode_select(logits: torch.Tensor, out_ids: torch.Tensor, step: torch.Tenso
     launch_counter[0] += 1
 
 
+def beam_candidates(num_beams: int, n_eos: int) -> int:
+    """Candidates per sequence of one beam step, the reference's ``max(2, 1 + n_eos) * num_beams``."""
+    return max(2, 1 + n_eos) * num_beams
+
+
+def beam_select_supported(num_beams: int, n_eos: int, V: int) -> bool:
+    """Whether ``beam_select`` takes this shape (its limits: num_beams <= 8, n_eos <= 4, the candidates fit in V)."""
+    return (1 <= num_beams <= _lib.BEAM_MAX_BEAMS and 0 <= n_eos <= _lib.BEAM_MAX_EOS
+            and beam_candidates(num_beams, n_eos) <= V <= 1 << 17)
+
+
+def beam_select(logits: torch.Tensor, step: torch.Tensor, params: torch.Tensor, beam_scores: torch.Tensor,
+                history: torch.Tensor, next_ids: torch.Tensor, parent: torch.Tensor, done: torch.Tensor,
+                hyp_scores: torch.Tensor, hyp_ids: torch.Tensor, hyp_meta: torch.Tensor, scratch: torch.Tensor,
+                num_beams: int, eos: Optional[torch.Tensor] = None, pad_id: int = 0, min_length: int = 0) -> None:
+    """One beam-search step in one call (csrc/beam_select_sm100.cu, two kernels): log-softmax, repetition penalty,
+    min-length ban and beam score per row, the sequence's top ``max(2, 1 + n_eos) * num_beams`` candidates, then
+    ``BeamSearchScorer.process``: new ``beam_scores``, ``next_ids`` and ``parent`` rows, the hypotheses and ``done``
+    flags updated in place and ``history`` reordered by parent with the new token appended at column ``step``.
+    ``logits`` fp32 (B * num_beams, V); ``step`` (1,) int64 and ``params`` (2,) float64 ``[repetition_penalty,
+    length_penalty]`` are read on the device; ``history`` (R, max_new) int64; ``hyp_scores`` (B, num_beams) float64;
+    ``hyp_ids`` (B, num_beams, max_new) int64; ``hyp_meta`` (B, num_beams, 2) int64 ``[length (-1 = free), serial]``;
+    ``scratch`` >= R * K int64 entries private to the call.  See include/mmfs_b200.h for the rules."""
+    inference_only("beam_select", logits)
+    _require(logits.is_cuda and logits.dim() == 2 and logits.dtype == torch.float32 and logits.stride(1) == 1,
+             "beam_select: logits must be a CUDA fp32 (R, V) tensor with unit column stride")
+    R, V = logits.shape
+    dev = logits.device
+    _require(num_beams > 0 and R % num_beams == 0, "beam_select: the rows must be whole groups of num_beams")
+    B = R // num_beams
+
+    def dense(t, name, dtype, shape):
+        _require(t.device == dev and t.dtype == dtype and tuple(t.shape) == shape and t.is_contiguous(),
+                 f"beam_select: {name} must be a contiguous {dtype} {shape} tensor on the logits' device")
+
+    _require(history.dim() == 2, "beam_select: history must be (R, max_new)")
+    max_new = history.shape[1]
+    dense(step, "step", torch.int64, (1,))
+    dense(params, "params", torch.float64, (2,))
+    dense(beam_scores, "beam_scores", torch.float32, (R,))
+    dense(history, "history", torch.int64, (R, max_new))
+    dense(next_ids, "next_ids", torch.int64, tuple(next_ids.shape))
+    _require(next_ids.numel() == R, "beam_select: next_ids must have R entries")
+    dense(parent, "parent", torch.int64, (R,))
+    _require(done.device == dev and done.dtype in (torch.bool, torch.uint8) and done.numel() == B and done.is_contiguous(),
+             "beam_select: done must be contiguous bool / uint8 with B entries")
+    dense(hyp_scores, "hyp_scores", torch.float64, (B, num_beams))
+    dense(hyp_ids, "hyp_ids", torch.int64, (B, num_beams, max_new))
+    dense(hyp_meta, "hyp_meta", torch.int64, (B, num_beams, 2))
+    n_eos = 0
+    if eos is not None:
+        _require(eos.device == dev and eos.dtype == torch.int64 and eos.dim() == 1 and eos.is_contiguous(),
+                 "beam_select: eos must be a contiguous 1-D int64 device tensor")
+        n_eos = eos.numel()
+    _require(scratch.device == dev and scratch.dtype == torch.int64 and scratch.is_contiguous()
+             and scratch.numel() >= R * beam_candidates(num_beams, n_eos),
+             "beam_select: scratch must be contiguous int64 with R * max(2, 1 + n_eos) * num_beams entries")
+    with torch.cuda.device(dev):
+        rc = _lib.lib().mmfs_beam_select(logits.data_ptr(), logits.stride(0), step.data_ptr(), params.data_ptr(),
+                                         beam_scores.data_ptr(), history.data_ptr(), next_ids.data_ptr(), parent.data_ptr(),
+                                         done.data_ptr(), hyp_scores.data_ptr(), hyp_ids.data_ptr(), hyp_meta.data_ptr(),
+                                         eos.data_ptr() if eos is not None else None, n_eos, int(pad_id), int(min_length),
+                                         scratch.data_ptr(), B, num_beams, V, max_new, _stream())
+    _lib.check(rc, "beam_select")
+    launch_counter[0] += 2
+
+
+def kv_beam_reorder(kv: torch.Tensor, parent: torch.Tensor, cur: torch.Tensor, step: torch.Tensor, num_beams: int,
+                    max_positions: int, done: Optional[torch.Tensor] = None) -> None:
+    """Beam search's KV-cache reorder in place, generated positions only, in one launch over every cache tensor:
+    ``kv`` (n, R, T_max, ...) holds n caches (every layer's K and V) with dense rows; within each group of
+    ``num_beams`` rows, row j takes the contents of row ``parent[j]`` at positions ``[cur - step, cur)``.  ``cur`` and
+    ``step`` are (1,) int64 device tensors (``step <= max_positions``); groups with ``done`` set are skipped."""
+    inference_only("kv_beam_reorder", kv)
+    _require(kv.is_cuda and kv.dim() >= 3, "kv_beam_reorder: kv must be a CUDA (n, R, T_max, ...) tensor")
+    n, R, T = kv.shape[:3]
+    dev = kv.device
+    row_bytes = kv[0, 0, 0].numel() * kv.element_size()
+    _require(kv[0, 0, 0].is_contiguous() and kv.stride(2) * kv.element_size() >= row_bytes,
+             "kv_beam_reorder: each (cache, row, position) entry must be dense")
+    _require(num_beams > 0 and R % num_beams == 0, "kv_beam_reorder: the rows must be whole groups of num_beams")
+    _require(parent.device == dev and parent.dtype == torch.int64 and parent.numel() == R and parent.is_contiguous(),
+             "kv_beam_reorder: parent must be contiguous int64 with R entries")
+    for t, name in ((cur, "cur"), (step, "step")):
+        _require(t.device == dev and t.dtype == torch.int64 and t.numel() == 1, f"kv_beam_reorder: {name} must be a (1,) int64 device tensor")
+    if done is not None:
+        _require(done.device == dev and done.dtype in (torch.bool, torch.uint8) and done.numel() == R // num_beams
+                 and done.is_contiguous(), "kv_beam_reorder: done must be contiguous bool / uint8 with one entry per group")
+    _require(0 < max_positions <= T, "kv_beam_reorder: max_positions must be in [1, T_max]")
+    es = kv.element_size()
+    with torch.cuda.device(dev):
+        rc = _lib.lib().mmfs_kv_beam_reorder(kv.data_ptr(), n, kv.stride(0) * es, R, kv.stride(1) * es, kv.stride(2) * es,
+                                             row_bytes, num_beams, parent.data_ptr(), cur.data_ptr(), step.data_ptr(),
+                                             done.data_ptr() if done is not None else None, int(max_positions), _stream())
+    _lib.check(rc, "kv_beam_reorder")
+    launch_counter[0] += 1
+
+
 def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
     """act_fn(gate) * up on a (..., 2*I) tensor holding [gate | up] (LlamaMLP, :188-189)."""
     inference_only("swiglu", gate_up)
