@@ -330,6 +330,31 @@ int mmfs_beam_select(const float *logits, long ld, const int64_t *step, const do
                      uint64_t *scratch, int B, int num_beams, int V, int max_new, void *stream);
 
 /*
+ * One step of beam-sample decoding (HF GenerationMixin.beam_sample, transformers 4.31), two launches like
+ * mmfs_beam_select, with the same buffers and the same scorer; only the candidates differ.  Per row r the score s of
+ * token i is mmfs_beam_select's (log_softmax, repetition penalty, min-length ban, + beam_scores[r]), then the warpers:
+ * s / temperature (times the fp32 reciprocal), top-k with k = min(max(top_k, 2), V) (top_k == 0: none; every s below
+ * the k-th largest removed, ties at it kept), and top-p over the remaining tokens with mmfs_decode_select's rule (2^-40
+ * fixed-point masses, ties at the threshold kept), never removing the two largest (min_tokens_to_keep = 2; skipped when
+ * top_p >= 1).  The draw: per sequence, the 2 * num_beams largest keys s - log(-log u) over its kept tokens, an exact
+ * draw without replacement proportional to softmax(s) (torch.multinomial's law), u from Philox4x32-10 keyed by
+ * (*seed, step, r, i) or u = uniforms[r * V + i] when uniforms != NULL (values in (0, 1)).  The drawn candidates are
+ * ordered by s, higher first, then by the lower flat index row_in_group * V + token, and BeamSearchScorer.process runs
+ * on them as in mmfs_beam_select; the new beam scores are their (warped) s.  A sequence left with fewer than num_beams
+ * non-eos candidates sets *error = 1 (sticky; 4.31 raises ValueError) and fills the missing beams with pad_id.
+ *   params: DEVICE double {repetition_penalty, length_penalty, temperature, top_p}; seed: DEVICE int64, may be NULL
+ *   with uniforms; uniforms (R, V) fp32 or NULL; error: DEVICE int32; scratch: R * 4 * num_beams uint64 of device
+ *   memory private to the call; every other argument as mmfs_beam_select.
+ * Limits: num_beams <= 8, n_eos <= 4, 2 * num_beams <= V <= 131072, top_k >= 0; outside them MMFS_EINVAL.  The
+ * per-call values (step, params, seed) are read on the device, so one captured CUDA graph serves any of them.
+ */
+int mmfs_beam_sample(const float *logits, long ld, const int64_t *step, const double *params, const int64_t *seed,
+                     const float *uniforms, float *beam_scores, int64_t *history, int64_t *next_ids, int64_t *parent,
+                     uint8_t *done, double *hyp_scores, int64_t *hyp_ids, int64_t *hyp_meta, int32_t *error,
+                     const int64_t *eos_ids, int n_eos, long pad_id, int min_length, int top_k, uint64_t *scratch, int B,
+                     int num_beams, int V, int max_new, void *stream);
+
+/*
  * The KV-cache reorder of beam search, in place and over the generated positions only: for each of n_caches cache
  * tensors (base pointer cache + i * cache_stride bytes) and each group of num_beams rows, row j gets the contents of
  * row parent[j] (an absolute row index in the same group) at positions [*cur - *step, *cur); the prompt positions are

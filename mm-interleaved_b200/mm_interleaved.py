@@ -401,7 +401,9 @@ class _GraphedDecoder:
     ``"beam"``: beam search over B * num_beams rows (``generate_beams``); the step is ``ops.beam_select`` (scores,
     hypotheses, done flags, history) -> ``ops.kv_beam_reorder`` (the generated positions of every layer's K and V, held
     in one tensor ``kv``) -> the decoder on the next tokens, with the repetition and length penalties in a device
-    buffer.  ``finished`` then holds the per-sequence done flags."""
+    buffer.  ``finished`` then holds the per-sequence done flags.  ``"beam_sample"``: the same with ``ops.beam_sample``
+    (temperature and top_p in the device buffer too, one seed per call as ``"sample"``, a sticky error flag) and every
+    beam starting at score 0."""
 
     def __init__(self, owner, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, mode=None,
                  num_beams=1):
@@ -412,7 +414,7 @@ class _GraphedDecoder:
         R = B * self.nb                                                     # decoder rows: one per beam
         model = owner.mm_decoder
         n_img = feats_shape[1]
-        if mode == "beam":
+        if mode in ("beam", "beam_sample"):
             H = model.config.num_attention_heads
             self.kv = torch.zeros((2 * len(model.layers), R, t_max, H, model.config.hidden_size // H), dtype=dtype,
                                   device=device)
@@ -441,17 +443,22 @@ class _GraphedDecoder:
         if mode in ("greedy", "sample"):
             self.params = torch.ones((3,), dtype=torch.float32, device=device)   # penalty, temperature, top_p
             self.seed = torch.zeros((1,), dtype=torch.long, device=device)
-        if mode == "beam":
+        if mode in ("beam", "beam_sample"):
             nb = self.nb
-            self.params = torch.ones((2,), dtype=torch.float64, device=device)   # repetition_penalty, length_penalty
+            # repetition_penalty, length_penalty (+ temperature, top_p when sampling)
+            self.params = torch.ones((2 if mode == "beam" else 4,), dtype=torch.float64, device=device)
             self.beam_scores = torch.zeros((R,), dtype=torch.float32, device=device)
             self.history = torch.zeros((R, max_new), dtype=torch.long, device=device)
             self.parent = torch.zeros((R,), dtype=torch.long, device=device)
             self.hyp_scores = torch.zeros((B, nb), dtype=torch.float64, device=device)
             self.hyp_ids = torch.zeros((B, nb, max_new), dtype=torch.long, device=device)
             self.hyp_meta = torch.zeros((B, nb, 2), dtype=torch.long, device=device)          # length (-1: free), serial
-            self.scratch = torch.zeros((R * ops.beam_candidates(nb, len(eos_ids)),), dtype=torch.long, device=device)
+            n_scratch = R * ops.beam_candidates(nb, len(eos_ids)) if mode == "beam" else ops.beam_sample_scratch(nb, R)
+            self.scratch = torch.zeros((n_scratch,), dtype=torch.long, device=device)
             self.all_done = torch.zeros((1,), dtype=torch.bool).pin_memory()                 # written by every replay
+        if mode == "beam_sample":
+            self.seed = torch.zeros((1,), dtype=torch.long, device=device)
+            self.error = torch.zeros((1,), dtype=torch.int32, device=device)
         self.graph = None
         self.launches = 0
         self.replays = 0
@@ -476,10 +483,16 @@ class _GraphedDecoder:
                 self.finished.logical_or_((nxt[:, None] == self.eos[None, :]).any(dim=1))
             self.out_ids.index_copy_(1, self.step, nxt[:, None])
             fed = nxt[:, None]
-        elif self.mode == "beam":                                          # scorer, then the cache follows the parents
-            ops.beam_select(self.logits, self.step, self.params, self.beam_scores, self.history, self.next_ids,
-                            self.parent, self.finished, self.hyp_scores, self.hyp_ids, self.hyp_meta, self.scratch,
-                            self.nb, eos=self.eos, pad_id=self.pad_id, min_length=self.min_length)
+        elif self.mode in ("beam", "beam_sample"):                         # scorer, then the cache follows the parents
+            if self.mode == "beam":
+                ops.beam_select(self.logits, self.step, self.params, self.beam_scores, self.history, self.next_ids,
+                                self.parent, self.finished, self.hyp_scores, self.hyp_ids, self.hyp_meta, self.scratch,
+                                self.nb, eos=self.eos, pad_id=self.pad_id, min_length=self.min_length)
+            else:
+                ops.beam_sample(self.logits, self.step, self.params, self.beam_scores, self.history, self.next_ids,
+                                self.parent, self.finished, self.hyp_scores, self.hyp_ids, self.hyp_meta, self.error,
+                                self.scratch, self.nb, eos=self.eos, pad_id=self.pad_id, min_length=self.min_length,
+                                top_k=_BEAM_SAMPLE_TOP_K, seed=self.seed)
             ops.kv_beam_reorder(self.kv, self.parent, self.cur, self.step, self.nb, self.max_new, done=self.finished)
             fed = self.next_ids
         else:                                                              # processors, choice and bookkeeping: one kernel
@@ -494,7 +507,7 @@ class _GraphedDecoder:
         self.logits.copy_(o.text_decoder.logits(hid)[:, -1].float())
         self.step.add_(1)
         self.cur.add_(1)
-        if self.mode == "beam":                                            # read by the host two replays later
+        if self.mode in ("beam", "beam_sample"):                           # read by the host two replays later
             self.all_done.copy_(self.finished.all().view(1), non_blocking=True)
 
     def _reset(self, L, attention_mask, position_ids, cross, logits0):
@@ -510,6 +523,10 @@ class _GraphedDecoder:
         if self.mode == "beam":
             self.beam_scores.fill_(-1e9)
             self.beam_scores[::self.nb] = 0.0                              # only the first beam of a sequence is live
+        if self.mode == "beam_sample":
+            self.beam_scores.zero_()                                       # beam_sample starts every beam at 0
+            self.error.zero_()
+        if self.mode in ("beam", "beam_sample"):
             self.history.fill_(self.pad_id)
             self.hyp_scores.zero_()
             self.hyp_meta.fill_(-1)
@@ -572,9 +589,10 @@ class _GraphedDecoder:
         return self.out_ids.clone()
 
     def generate_beams(self, mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty=1.0,
-                       length_penalty=1.0):
-        """Beam search (``mode == "beam"``): the prompt is prefilled once per sequence and its cache rows, the
-        ``PreparedVision`` values, key mask, position ids and last cross-attention row are replicated to the beams;
+                       length_penalty=1.0, temperature=1.0, top_p=1.0, generator=None):
+        """Beam search (``mode == "beam"`` or ``"beam_sample"``): the prompt is prefilled once per sequence and its
+        cache rows, the ``PreparedVision`` values, key mask, position ids and last cross-attention row are replicated
+        to the beams (beam sample: to the ``self.B // B`` independent searches of each prompt, then to their beams);
         then one replay per step.  At most two replays are in flight: before enqueuing replay t the host waits for
         replay t - 2 and reads the "all sequences done" flag it copied to pinned memory, so decoding stops at most two
         steps after the eager loop would (done sequences are inert).  Returns the host copies of the final state."""
@@ -585,7 +603,11 @@ class _GraphedDecoder:
             raise RuntimeError("prompt + new tokens exceed the captured cache length")
         self.params[0].fill_(float(repetition_penalty))
         self.params[1].fill_(float(length_penalty))
-        rep = torch.arange(B, device=mm_embeds.device).repeat_interleave(self.nb)   # beam row -> sequence
+        if self.mode == "beam_sample":
+            self.params[2].fill_(float(temperature))
+            self.params[3].fill_(float(top_p))
+            self.seed.random_(generator=generator)                          # one seed per call, drawn on the device
+        rep = torch.arange(B, device=mm_embeds.device).repeat_interleave(self.B // B * self.nb)   # beam row -> prompt
         pv = o.mm_decoder.prepare_vision(feats)                             # the prefill's B rows, then one per beam
         for idx, val in pv.values.items():
             torch.index_select(val, 0, rep, out=self.pv.values[idx])
@@ -615,8 +637,11 @@ class _GraphedDecoder:
         self.replays = n
         ops.launch_counter[0] += self.launches * n
         self._set_graph_mode(False, L)
-        return dict(history=self.history[:, :n].cpu(), beam_scores=self.beam_scores.cpu(), done=self.finished.cpu(),
-                    hyp_scores=self.hyp_scores.cpu(), hyp_ids=self.hyp_ids.cpu(), hyp_meta=self.hyp_meta.cpu())
+        out = dict(history=self.history[:, :n].cpu(), beam_scores=self.beam_scores.cpu(), done=self.finished.cpu(),
+                   hyp_scores=self.hyp_scores.cpu(), hyp_ids=self.hyp_ids.cpu(), hyp_meta=self.hyp_meta.cpu())
+        if self.mode == "beam_sample":
+            out["error"] = bool(self.error.item())
+        return out
 
 
 class InterleavedForward(nn.Module):
@@ -654,14 +679,20 @@ class InterleavedForward(nn.Module):
         Beam search (``num_beams > 1``, within ``ops.beam_select_supported``: at most 8 beams and 4 eos ids) is graphed
         too: one replay per step of ``ops.beam_select`` + ``ops.kv_beam_reorder`` + the decoder, with the eager loop's
         tokens.  One caveat: the kernel's log-softmax sums in a different order from ``torch.log_softmax``, so graphed
-        and eager tokens can differ where two candidates' scores are within a few fp32 ulps of each other."""
+        and eager tokens can differ where two candidates' scores are within a few fp32 ulps of each other.
+
+        With ``sampling=True`` beam sample (``num_beams > 1`` with ``use_nucleus_sampling``, within
+        ``ops.beam_sample_supported``) is graphed as well: ``ops.beam_sample`` + ``ops.kv_beam_reorder`` + the decoder,
+        its draws from the kernel's Philox stream keyed by a per-call seed, so again not the eager loop's tokens."""
         self._decode_graphs = {} if enabled else None
         self._decode_graph_sampling = bool(enabled and sampling)
         return self
 
-    def _decode_graph(self, mm_embeds, feats, max_new_tokens, eos_ids, pad_id, min_length, mode, num_beams=1):
-        """The ``_GraphedDecoder`` for this shape and these settings, built on first use (at most four are kept)."""
+    def _decode_graph(self, mm_embeds, feats, max_new_tokens, eos_ids, pad_id, min_length, mode, num_beams=1, expand=1):
+        """The ``_GraphedDecoder`` for this shape and these settings, built on first use (at most four are kept);
+        ``expand`` independent beam searches per prompt (beam sample's ``num_return_sequences``)."""
         B, L, _ = mm_embeds.shape
+        B *= expand
         t_max = ((L + max_new_tokens + 255) // 256) * 256                  # cache-length bucket: one graph serves nearby prompts
         key = (B, t_max, tuple(feats.shape), mm_embeds.dtype, mm_embeds.device, tuple(eos_ids), int(pad_id), int(min_length),
                int(max_new_tokens), int(num_beams), mode)
@@ -739,7 +770,11 @@ class InterleavedForward(nn.Module):
         is suppressed while fewer than ``min_length`` tokens were generated), several ``eos_token_id`` values (the
         reference passes [eos, soi]), and ``use_nucleus_sampling`` = temperature + top-p sampling.  ``num_beams > 1``
         runs HF-style beam search (``_beam_search`` below; the reference's captioning default is 5 beams) and returns
-        (B * num_return_sequences, <= max_new_tokens) padded ids; otherwise (B, max_new_tokens) ids.
+        (B * num_return_sequences, <= max_new_tokens) padded ids; otherwise (B, max_new_tokens) ids.  ``num_beams > 1``
+        with ``use_nucleus_sampling`` is HF 4.31's beam sample (``_beam_sample``: temperature, top-k 50 and top-p on
+        the beam scores, 2 * num_beams candidates drawn per sequence, ``num_return_sequences`` independent searches
+        per prompt); it raises ``ValueError`` where 4.31 does, when a step leaves fewer than num_beams non-eos
+        candidates.
 
         Under ``enable_decode_graphs()`` greedy decoding (with or without the penalty) replays one CUDA graph per token
         with the eager loop's tokens; nucleus sampling is graphed only after ``enable_decode_graphs(True,
@@ -747,18 +782,21 @@ class InterleavedForward(nn.Module):
         distribution, different tokens for a given ``generator`` seed).  Beam search replays one graph per step when
         its sizes are within ``ops.beam_select_supported`` (else it runs the eager loop), with the eager loop's tokens
         except where two candidates' scores lie within a few fp32 ulps (the kernel's log-softmax sums in another
-        order than ``torch.log_softmax``)."""
+        order than ``torch.log_softmax``).  Beam sample is graphed under ``enable_decode_graphs(True, sampling=True)``
+        within ``ops.beam_sample_supported``, with Philox draws like graphed nucleus sampling."""
         from . import ops
         eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
         if num_beams > 1:
-            if use_nucleus_sampling:
-                raise NotImplementedError("beam-sample (num_beams > 1 with sampling) is not implemented")
             beam_args = (text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, max_new_tokens,
                          eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams, length_penalty,
                          num_return_sequences)
             V = self.text_decoder.head.weight.shape[0]
-            if (self._decode_graphs is not None and text_ids.is_cuda and max_new_tokens > 0
-                    and ops.beam_select_supported(num_beams, len(eos_ids), V)):
+            graphs = self._decode_graphs is not None and text_ids.is_cuda and max_new_tokens > 0
+            if use_nucleus_sampling:                                     # HF beam_sample
+                if graphs and self._decode_graph_sampling and ops.beam_sample_supported(num_beams, len(eos_ids), V):
+                    return self._graphed_beam_search(*beam_args, sampling=(temperature, top_p, generator))
+                return self._beam_sample(*beam_args, temperature=temperature, top_p=top_p, generator=generator)
+            if graphs and ops.beam_select_supported(num_beams, len(eos_ids), V):
                 return self._graphed_beam_search(*beam_args)
             return self._beam_search(*beam_args)
         B, L = text_ids.shape
@@ -819,7 +857,8 @@ class InterleavedForward(nn.Module):
 
     @torch.no_grad()
     def _beam_search(self, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, max_new_tokens,
-                     eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams, length_penalty, num_return):
+                     eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams, length_penalty, num_return,
+                     sampling=None):
         """Beam search with the bookkeeping of HF ``GenerationMixin.beam_search`` + ``BeamSearchScorer`` (transformers
         4.31, the version the reference pins; ``early_stopping=False``, one beam group): log-softmax scores, logits
         processors on the log-probabilities, top ``max(2, 1 + n_eos) * num_beams`` candidates per sequence (the
@@ -827,19 +866,26 @@ class InterleavedForward(nn.Module):
         eos), finished hypotheses ranked by ``sum_logprobs / len(generated) ** length_penalty``, a sequence is done once
         ``num_beams`` hypotheses are all at least as good as the best running beam could become.  The prompt is
         prefilled ONCE per sequence and its cache rows are replicated per beam; every step re-gathers the cache rows by
-        beam index (``_reorder_cache``)."""
-        B, L = text_ids.shape
+        beam index (``_reorder_cache``).
+
+        ``sampling = (temperature, top_p, generator)`` runs 4.31's ``beam_sample`` instead (``_beam_sample_candidates``
+        chooses the candidates): every beam starts at score 0, each sequence is expanded to ``num_return`` independent
+        beam searches that return their best hypothesis, and a step with fewer than ``num_beams`` non-eos candidates
+        raises ``ValueError`` as 4.31 does."""
+        B0, L = text_ids.shape
         nb, dev = num_beams, text_ids.device
+        expand = num_return if sampling is not None else 1
+        B = B0 * expand                                                            # independent beam searches
         if attention_mask is None:
-            attention_mask = torch.ones((B, L), dtype=torch.long, device=dev)
+            attention_mask = torch.ones((B0, L), dtype=torch.long, device=dev)
         eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
         mm_embeds, cross, feats = self.prepare(text_ids, visual_output, num_image_per_seq, max_num_image)
         position_ids = (attention_mask.long().cumsum(-1) - 1).masked_fill(attention_mask == 0, 1)   # causal_lm_cascade.py:181-183
-        pre = self.mm_decoder.static_cache(B, L, dtype=mm_embeds.dtype, device=dev)
+        pre = self.mm_decoder.static_cache(B0, L, dtype=mm_embeds.dtype, device=dev)
         out = self.mm_decoder(inputs_embeds=mm_embeds, attention_mask=attention_mask, position_ids=position_ids,
                               past_key_values=pre, vision_hidden_states=feats, cross_attention_mask=cross, use_cache=True,
                               return_dict=True)
-        rep = torch.arange(B, device=dev).repeat_interleave(nb)                    # beam row -> sequence
+        rep = torch.arange(B0, device=dev).repeat_interleave(expand * nb)         # beam row -> prompt
         past = self.mm_decoder.static_cache(B * nb, L + max_new_tokens, dtype=mm_embeds.dtype, device=dev)
         for dst, src in zip(past, pre):
             dst.k[:, :L].copy_(src.k.index_select(0, rep)); dst.v[:, :L].copy_(src.v.index_select(0, rep)); dst.length = L
@@ -849,7 +895,8 @@ class InterleavedForward(nn.Module):
         mask, pos = attention_mask.index_select(0, rep), position_ids[:, -1:].index_select(0, rep)
 
         beam_scores = torch.zeros((B, nb), dtype=torch.float32, device=dev)
-        beam_scores[:, 1:] = -1e9
+        if sampling is None:
+            beam_scores[:, 1:] = -1e9                                              # beam_sample starts every beam at 0
         beam_scores = beam_scores.view(-1)
         seqs = torch.zeros((B * nb, 0), dtype=torch.long, device=dev)              # generated ids per beam row
         hyps = [_BeamHypotheses(nb, length_penalty) for _ in range(B)]
@@ -864,8 +911,10 @@ class InterleavedForward(nn.Module):
             if step_idx < min_length and eos_ids:
                 scores[:, eos_ids] = float("-inf")
             V = scores.shape[-1]
-            cand = (scores + beam_scores[:, None]).view(B, nb * V)
-            top_s, top_i = cand.topk(n_cand, dim=1, largest=True, sorted=True)
+            if sampling is None:
+                top_s, top_i = (scores + beam_scores[:, None]).view(B, nb * V).topk(n_cand, dim=1, largest=True, sorted=True)
+            else:
+                top_s, top_i = _beam_sample_candidates(scores, beam_scores, B, nb, *sampling)
             top_s_h, top_i_h, seqs_h = top_s.tolist(), top_i.tolist(), seqs.tolist()   # one host round trip per step
             cur_len = seqs.shape[1] + 1
             nxt_scores = [[0.0] * nb for _ in range(B)]
@@ -886,6 +935,9 @@ class InterleavedForward(nn.Module):
                         k += 1
                     if k == nb:
                         break
+                if k < nb and sampling is not None:
+                    raise ValueError(f"At most {nb} tokens in {[i % V for i in top_i_h[b]]} can be equal to "
+                                     f"`eos_token_id: {eos_ids}`. Make sure {[i % V for i in top_i_h[b]]} are corrected.")
                 if len(hyps[b].beams) >= nb and hyps[b].worst >= top_s_h[b][0] / (cur_len ** length_penalty):
                     done[b] = True
             beam_scores = torch.tensor(nxt_scores, dtype=torch.float32, device=dev).view(-1)
@@ -903,32 +955,67 @@ class InterleavedForward(nn.Module):
                                    past_key_values=past, vision_hidden_states=feats_b, cross_attention_mask=last_cross,
                                    use_cache=True, return_dict=True)
             logits = self.text_decoder.logits(step.last_hidden_state)
-        return _beam_finalize(hyps, done, seqs.tolist(), beam_scores.tolist(), num_return, max_new_tokens, pad_token_id,
-                              eos_ids).to(dev)
+        return _beam_finalize(hyps, done, seqs.tolist(), beam_scores.tolist(), num_return // expand, max_new_tokens,
+                              pad_token_id, eos_ids).to(dev)
+
+    def _beam_sample(self, *beam_args, temperature=1.0, top_p=1.0, generator=None):
+        """HF 4.31 ``beam_sample`` in torch ops: ``_beam_search``'s loop with ``_beam_sample_candidates``."""
+        return self._beam_search(*beam_args, sampling=(temperature, top_p, generator))
 
     @torch.no_grad()
     def _graphed_beam_search(self, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask,
                              max_new_tokens, eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams,
-                             length_penalty, num_return):
-        """``_beam_search`` on one CUDA graph replay per step (``_GraphedDecoder`` in beam mode); same arguments, same
-        finalize."""
+                             length_penalty, num_return, sampling=None):
+        """``_beam_search`` on one CUDA graph replay per step (``_GraphedDecoder`` in ``"beam"`` mode, or in
+        ``"beam_sample"`` mode with ``sampling = (temperature, top_p, generator)``); same arguments, same finalize."""
         B, L = text_ids.shape
         nb = num_beams
+        expand = num_return if sampling is not None else 1
         if attention_mask is None:
             attention_mask = torch.ones((B, L), dtype=torch.long, device=text_ids.device)
         eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
         mm_embeds, cross, feats = self.prepare(text_ids, visual_output, num_image_per_seq, max_num_image)
         position_ids = (attention_mask.long().cumsum(-1) - 1).masked_fill(attention_mask == 0, 1)   # causal_lm_cascade.py:181-183
-        dec = self._decode_graph(mm_embeds, feats, max_new_tokens, eos_ids, pad_token_id, min_length, "beam", nb)
-        st = dec.generate_beams(mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty, length_penalty)
+        mode = "beam" if sampling is None else "beam_sample"
+        dec = self._decode_graph(mm_embeds, feats, max_new_tokens, eos_ids, pad_token_id, min_length, mode, nb, expand)
+        st = dec.generate_beams(mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty, length_penalty,
+                                *(sampling or ()))
+        if st.get("error"):
+            raise ValueError(f"At most {nb} tokens in the {2 * nb} sampled candidates of a sequence can be equal to "
+                             f"`eos_token_id: {eos_ids}`: a step drew more than {nb} eos candidates")
         hyps = []
-        for b in range(B):                                                 # the slots in insertion order
+        for b in range(B * expand):                                        # the slots in insertion order
             meta, ids, sc = st["hyp_meta"][b].tolist(), st["hyp_ids"][b].tolist(), st["hyp_scores"][b].tolist()
             slots = sorted((m[1], j) for j, m in enumerate(meta) if m[0] >= 0)
             hyps.append(_BeamHypotheses(nb, length_penalty, [(sc[j], ids[j][:meta[j][0]]) for _, j in slots]))
         done = [bool(d) for d in st["done"].tolist()]
-        return _beam_finalize(hyps, done, st["history"].tolist(), st["beam_scores"].tolist(), num_return, max_new_tokens,
-                              pad_token_id, eos_ids).to(text_ids.device)
+        return _beam_finalize(hyps, done, st["history"].tolist(), st["beam_scores"].tolist(), num_return // expand,
+                              max_new_tokens, pad_token_id, eos_ids).to(text_ids.device)
+
+
+_BEAM_SAMPLE_TOP_K = 50              # transformers 4.31 GenerationConfig.top_k, which the reference never overrides
+
+
+def _beam_sample_candidates(scores, beam_scores, B, nb, temperature, top_p, generator):
+    """Steps 3-5 of one 4.31 ``beam_sample`` step on the processed log-probabilities ``scores`` (B * nb, V): add the
+    beam scores, warp (temperature, top-k 50, top-p; ``min_tokens_to_keep = 2``), draw ``2 * nb`` candidates per
+    sequence with ``torch.multinomial`` (without replacement) and sort them by warped score.  Returns (scores, flat
+    indices), each (B, 2 * nb)."""
+    s = scores + beam_scores[:, None]
+    if temperature != 1.0:                                                  # TemperatureLogitsWarper
+        s = s / temperature
+    V = s.shape[-1]
+    k = min(max(_BEAM_SAMPLE_TOP_K, 2), V)                                  # TopKLogitsWarper
+    s = s.masked_fill(s < s.topk(k, dim=-1).values[:, -1:], float("-inf"))
+    if top_p < 1.0:                                                         # TopPLogitsWarper
+        srt, idx = s.sort(dim=-1, descending=False)
+        drop = srt.softmax(-1).cumsum(-1) <= (1.0 - top_p)
+        drop[:, -2:] = False
+        s = s.masked_fill(drop.scatter(1, idx, drop), float("-inf"))
+    s = s.view(B, nb * V)
+    pick = torch.multinomial(s.softmax(-1), 2 * nb, generator=generator)
+    picked, order = s.gather(1, pick).sort(dim=1, descending=True, stable=True)   # ties: in draw order
+    return picked, pick.gather(1, order)
 
 
 class _BeamHypotheses:

@@ -165,6 +165,43 @@ def beam_select_supported(num_beams: int, n_eos: int, V: int) -> bool:
             and beam_candidates(num_beams, n_eos) <= V <= 1 << 17)
 
 
+def _check_beam_step(what, logits, step, params, n_params, beam_scores, history, next_ids, parent, done, hyp_scores,
+                     hyp_ids, hyp_meta, num_beams, eos):
+    """The buffer checks ``beam_select`` and ``beam_sample`` share; returns (B, V, max_new, n_eos)."""
+    inference_only(what, logits)
+    _require(logits.is_cuda and logits.dim() == 2 and logits.dtype == torch.float32 and logits.stride(1) == 1,
+             f"{what}: logits must be a CUDA fp32 (R, V) tensor with unit column stride")
+    R, V = logits.shape
+    dev = logits.device
+    _require(num_beams > 0 and R % num_beams == 0, f"{what}: the rows must be whole groups of num_beams")
+    B = R // num_beams
+
+    def dense(t, name, dtype, shape):
+        _require(t.device == dev and t.dtype == dtype and tuple(t.shape) == shape and t.is_contiguous(),
+                 f"{what}: {name} must be a contiguous {dtype} {shape} tensor on the logits' device")
+
+    _require(history.dim() == 2, f"{what}: history must be (R, max_new)")
+    max_new = history.shape[1]
+    dense(step, "step", torch.int64, (1,))
+    dense(params, "params", torch.float64, (n_params,))
+    dense(beam_scores, "beam_scores", torch.float32, (R,))
+    dense(history, "history", torch.int64, (R, max_new))
+    dense(next_ids, "next_ids", torch.int64, tuple(next_ids.shape))
+    _require(next_ids.numel() == R, f"{what}: next_ids must have R entries")
+    dense(parent, "parent", torch.int64, (R,))
+    _require(done.device == dev and done.dtype in (torch.bool, torch.uint8) and done.numel() == B and done.is_contiguous(),
+             f"{what}: done must be contiguous bool / uint8 with B entries")
+    dense(hyp_scores, "hyp_scores", torch.float64, (B, num_beams))
+    dense(hyp_ids, "hyp_ids", torch.int64, (B, num_beams, max_new))
+    dense(hyp_meta, "hyp_meta", torch.int64, (B, num_beams, 2))
+    n_eos = 0
+    if eos is not None:
+        _require(eos.device == dev and eos.dtype == torch.int64 and eos.dim() == 1 and eos.is_contiguous(),
+                 f"{what}: eos must be a contiguous 1-D int64 device tensor")
+        n_eos = eos.numel()
+    return B, V, max_new, n_eos
+
+
 def beam_select(logits: torch.Tensor, step: torch.Tensor, params: torch.Tensor, beam_scores: torch.Tensor,
                 history: torch.Tensor, next_ids: torch.Tensor, parent: torch.Tensor, done: torch.Tensor,
                 hyp_scores: torch.Tensor, hyp_ids: torch.Tensor, hyp_meta: torch.Tensor, scratch: torch.Tensor,
@@ -177,47 +214,71 @@ def beam_select(logits: torch.Tensor, step: torch.Tensor, params: torch.Tensor, 
     length_penalty]`` are read on the device; ``history`` (R, max_new) int64; ``hyp_scores`` (B, num_beams) float64;
     ``hyp_ids`` (B, num_beams, max_new) int64; ``hyp_meta`` (B, num_beams, 2) int64 ``[length (-1 = free), serial]``;
     ``scratch`` >= R * K int64 entries private to the call.  See include/mmfs_b200.h for the rules."""
-    inference_only("beam_select", logits)
-    _require(logits.is_cuda and logits.dim() == 2 and logits.dtype == torch.float32 and logits.stride(1) == 1,
-             "beam_select: logits must be a CUDA fp32 (R, V) tensor with unit column stride")
-    R, V = logits.shape
-    dev = logits.device
-    _require(num_beams > 0 and R % num_beams == 0, "beam_select: the rows must be whole groups of num_beams")
-    B = R // num_beams
-
-    def dense(t, name, dtype, shape):
-        _require(t.device == dev and t.dtype == dtype and tuple(t.shape) == shape and t.is_contiguous(),
-                 f"beam_select: {name} must be a contiguous {dtype} {shape} tensor on the logits' device")
-
-    _require(history.dim() == 2, "beam_select: history must be (R, max_new)")
-    max_new = history.shape[1]
-    dense(step, "step", torch.int64, (1,))
-    dense(params, "params", torch.float64, (2,))
-    dense(beam_scores, "beam_scores", torch.float32, (R,))
-    dense(history, "history", torch.int64, (R, max_new))
-    dense(next_ids, "next_ids", torch.int64, tuple(next_ids.shape))
-    _require(next_ids.numel() == R, "beam_select: next_ids must have R entries")
-    dense(parent, "parent", torch.int64, (R,))
-    _require(done.device == dev and done.dtype in (torch.bool, torch.uint8) and done.numel() == B and done.is_contiguous(),
-             "beam_select: done must be contiguous bool / uint8 with B entries")
-    dense(hyp_scores, "hyp_scores", torch.float64, (B, num_beams))
-    dense(hyp_ids, "hyp_ids", torch.int64, (B, num_beams, max_new))
-    dense(hyp_meta, "hyp_meta", torch.int64, (B, num_beams, 2))
-    n_eos = 0
-    if eos is not None:
-        _require(eos.device == dev and eos.dtype == torch.int64 and eos.dim() == 1 and eos.is_contiguous(),
-                 "beam_select: eos must be a contiguous 1-D int64 device tensor")
-        n_eos = eos.numel()
-    _require(scratch.device == dev and scratch.dtype == torch.int64 and scratch.is_contiguous()
+    B, V, max_new, n_eos = _check_beam_step("beam_select", logits, step, params, 2, beam_scores, history, next_ids,
+                                            parent, done, hyp_scores, hyp_ids, hyp_meta, num_beams, eos)
+    R = B * num_beams
+    _require(scratch.device == logits.device and scratch.dtype == torch.int64 and scratch.is_contiguous()
              and scratch.numel() >= R * beam_candidates(num_beams, n_eos),
              "beam_select: scratch must be contiguous int64 with R * max(2, 1 + n_eos) * num_beams entries")
-    with torch.cuda.device(dev):
+    with torch.cuda.device(logits.device):
         rc = _lib.lib().mmfs_beam_select(logits.data_ptr(), logits.stride(0), step.data_ptr(), params.data_ptr(),
                                          beam_scores.data_ptr(), history.data_ptr(), next_ids.data_ptr(), parent.data_ptr(),
                                          done.data_ptr(), hyp_scores.data_ptr(), hyp_ids.data_ptr(), hyp_meta.data_ptr(),
                                          eos.data_ptr() if eos is not None else None, n_eos, int(pad_id), int(min_length),
                                          scratch.data_ptr(), B, num_beams, V, max_new, _stream())
     _lib.check(rc, "beam_select")
+    launch_counter[0] += 2
+
+
+def beam_sample_supported(num_beams: int, n_eos: int, V: int) -> bool:
+    """Whether ``beam_sample`` takes this shape (its limits: num_beams <= 8, n_eos <= 4, 2 * num_beams <= V <= 2^17)."""
+    return (1 <= num_beams <= _lib.BEAM_MAX_BEAMS and 0 <= n_eos <= _lib.BEAM_MAX_EOS
+            and 2 * num_beams <= V <= 1 << 17)
+
+
+def beam_sample_scratch(num_beams: int, rows: int) -> int:
+    """int64 entries of the ``scratch`` of ``beam_sample`` over ``rows`` beam rows: two words per drawn candidate."""
+    return rows * 4 * num_beams
+
+
+def beam_sample(logits: torch.Tensor, step: torch.Tensor, params: torch.Tensor, beam_scores: torch.Tensor,
+                history: torch.Tensor, next_ids: torch.Tensor, parent: torch.Tensor, done: torch.Tensor,
+                hyp_scores: torch.Tensor, hyp_ids: torch.Tensor, hyp_meta: torch.Tensor, error: torch.Tensor,
+                scratch: torch.Tensor, num_beams: int, eos: Optional[torch.Tensor] = None, pad_id: int = 0,
+                min_length: int = 0, top_k: int = 50, seed: Optional[torch.Tensor] = None,
+                uniforms: Optional[torch.Tensor] = None) -> None:
+    """One beam-sample step in one call (csrc/beam_select_sm100.cu, two kernels): ``beam_select``'s row scores, then
+    temperature, top-k (``min(max(top_k, 2), V)``; 0 = none) and top-p with two tokens always kept, then 2 * num_beams
+    candidates per sequence drawn without replacement from the softmax of the warped scores, ordered by warped score,
+    and ``BeamSearchScorer.process`` as in ``beam_select``.  ``params`` (4,) float64 ``[repetition_penalty,
+    length_penalty, temperature, top_p]`` and ``seed`` (1,) int64 are read on the device; ``uniforms`` (R, V) fp32 in
+    (0, 1) replaces the Philox draw when given; ``error`` (1,) int32 is set to 1 (and stays set) when a sequence gets
+    fewer than num_beams non-eos candidates; ``scratch`` >= ``beam_sample_scratch(num_beams, R)`` int64 entries private
+    to the call; the other buffers as ``beam_select``.  See include/mmfs_b200.h for the rules."""
+    B, V, max_new, n_eos = _check_beam_step("beam_sample", logits, step, params, 4, beam_scores, history, next_ids,
+                                            parent, done, hyp_scores, hyp_ids, hyp_meta, num_beams, eos)
+    R, dev = B * num_beams, logits.device
+    _require(error.device == dev and error.dtype == torch.int32 and error.numel() == 1,
+             "beam_sample: error must be a (1,) int32 device tensor")
+    _require(scratch.device == dev and scratch.dtype == torch.int64 and scratch.is_contiguous()
+             and scratch.numel() >= beam_sample_scratch(num_beams, R),
+             "beam_sample: scratch must be contiguous int64 with R * 4 * num_beams entries")
+    _require(seed is not None or uniforms is not None, "beam_sample: needs a seed or uniforms")
+    if seed is not None:
+        _require(seed.device == dev and seed.dtype == torch.int64 and seed.numel() == 1, "beam_sample: seed must be a (1,) int64 device tensor")
+    if uniforms is not None:
+        _require(uniforms.device == dev and uniforms.dtype == torch.float32 and tuple(uniforms.shape) == (R, V)
+                 and uniforms.is_contiguous(), "beam_sample: uniforms must be a contiguous fp32 (R, V) tensor")
+    _require(top_k >= 0, "beam_sample: top_k must be >= 0")
+    with torch.cuda.device(dev):
+        rc = _lib.lib().mmfs_beam_sample(logits.data_ptr(), logits.stride(0), step.data_ptr(), params.data_ptr(),
+                                         seed.data_ptr() if seed is not None else None,
+                                         uniforms.data_ptr() if uniforms is not None else None, beam_scores.data_ptr(),
+                                         history.data_ptr(), next_ids.data_ptr(), parent.data_ptr(), done.data_ptr(),
+                                         hyp_scores.data_ptr(), hyp_ids.data_ptr(), hyp_meta.data_ptr(), error.data_ptr(),
+                                         eos.data_ptr() if eos is not None else None, n_eos, int(pad_id), int(min_length),
+                                         int(top_k), scratch.data_ptr(), B, num_beams, V, max_new, _stream())
+    _lib.check(rc, "beam_sample")
     launch_counter[0] += 2
 
 

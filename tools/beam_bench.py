@@ -5,10 +5,13 @@
   long:    the 2048-token 4-image prompt of tools/decode_bench.py, B in {1, 2}.  At B = 4 its 20 beam rows need a
            34 GB cache (38 GB graphed) next to the 26 GB of weights, their ~18 GB of fused copies and the prefill
            cache: more than an 80 GB card holds, in either loop.
-With random weights eos is practically never chosen, so every step decodes.  ms per token = (time of a 20-token call -
-time of a 1-token call) / 19, each the best of 2 runs; the ids of the eager and graphed runs are compared.  Then the
-two kernels alone at the step in the middle of a run (step 10), CUDA events over many launches.  Prints one JSON
-object with the card name, its power limit and SM clock read in the same run.
+The same for beam sample (``use_nucleus_sampling=True``, top_p 0.9, temperature 1: eager ``_beam_sample`` against
+the graphed ``ops.beam_sample`` step under ``enable_decode_graphs(True, sampling=True)``; their draws differ by design,
+so those ids are not compared).  With random weights eos is practically never chosen, so every step decodes.  ms per
+token = (time of a 20-token call - time of a 1-token call) / 19, each the best of 2 runs; the ids of the eager and
+graphed beam searches are compared.  Then the kernels alone (beam_select, beam_sample, the cache reorder) at the step
+in the middle of a run (step 10), CUDA events over many launches.  Prints one JSON object with the card name, its
+power limit and SM clock read in the same run.
 
     python tools/beam_bench.py
 """
@@ -73,6 +76,11 @@ def kernel_rows(rows, step=MAX_NEW // 2):
                     scratch=torch.zeros(R * ops.beam_candidates(NB, 2), dtype=torch.long, device="cuda"))
         rows[f"beam_select_B{B}_us"] = timed(lambda: ops.beam_select(logits, st, num_beams=NB, eos=eos, min_length=MIN_LEN,
                                                                       **bufs), 200)
+        sbufs = dict(bufs, params=torch.tensor([1.0, 1.0, 1.0, 0.9], dtype=torch.float64, device="cuda"),
+                     scratch=torch.zeros(ops.beam_sample_scratch(NB, R), dtype=torch.long, device="cuda"),
+                     error=torch.zeros(1, dtype=torch.int32, device="cuda"), seed=torch.tensor([5], device="cuda"))
+        rows[f"beam_sample_B{B}_us"] = timed(lambda: ops.beam_sample(logits, st, num_beams=NB, eos=eos, min_length=MIN_LEN,
+                                                                      **sbufs), 200)
         # the cache reorder at 13B widths, every row moved (cyclic parents), prompt of 2048 tokens
         T = 2048 + MAX_NEW
         kv = torch.zeros((2 * LAYERS, R, T, HEADS, HIDDEN // HEADS), dtype=torch.bfloat16, device="cuda")
@@ -114,14 +122,15 @@ with torch.no_grad():
             ids, img, nimg = ids.cuda(), img.cuda(), nimg.cuda()
             vis = model._tokenize(img)
 
-            def per_token(graphed):
+            def per_token(graphed, sample=False):
                 """Best of 2 calls at MAX_NEW and at 1 new token (the first graphed call of a length captures its
                 graph); one beam graph is alive at a time, since one cache at the long shape takes up to 19 GB."""
-                gen = lambda n: InterleavedForward.generate_texts(model, ids, vis, nimg, n_img, max_new_tokens=n,
-                                                                  eos_token_id=eos, min_length=MIN_LEN, num_beams=NB)
+                gen = lambda n: InterleavedForward.generate_texts(
+                    model, ids, vis, nimg, n_img, max_new_tokens=n, eos_token_id=eos, min_length=MIN_LEN, num_beams=NB,
+                    use_nucleus_sampling=sample, top_p=0.9, generator=torch.Generator(device="cuda").manual_seed(0))
                 best, out = {}, None
                 for n in (MAX_NEW, 1):
-                    model.enable_decode_graphs(graphed)
+                    model.enable_decode_graphs(graphed, sampling=sample)
                     for _ in range(2):
                         torch.cuda.synchronize(); t0 = time.time()
                         o = gen(n)
@@ -137,6 +146,8 @@ with torch.no_grad():
             rows[f"{key}_eager_ms_per_token"], out_e = per_token(False)
             rows[f"{key}_graphed_ms_per_token"], out_g = per_token(True)
             rows[f"{key}_ids_equal"] = bool(torch.equal(out_e, out_g))
+            rows[f"{key}_sample_eager_ms_per_token"], _ = per_token(False, sample=True)
+            rows[f"{key}_sample_graphed_ms_per_token"], _ = per_token(True, sample=True)
             del vis
             torch.cuda.empty_cache()
 rows.update(beams=NB, new_tokens=MAX_NEW, min_length=MIN_LEN)
