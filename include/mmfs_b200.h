@@ -235,6 +235,57 @@ int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, co
                       float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream);
 
 /*
+ * mmfs_attn_forward that also writes the row log-sum-exp the backward pass needs (training path).  Same arguments,
+ * requirements and output (O is bit-identical to mmfs_attn_forward's), plus
+ *   lse  (B, H, Tq) fp32, contiguous: lse[b,h,i] = ln sum_j exp(scale * q_i . k_j) over the keys row i sees, in
+ *        NATURAL-log units; +INFINITY for a row that sees no key (its output row is 0, and +inf makes every
+ *        recomputed probability of that row exp(s - inf) = 0, so it gets zero gradient).
+ */
+int mmfs_attn_forward_lse(const void *q, const void *k, const void *v, void *out, float *lse, const uint8_t *key_mask,
+                          int B, int H, int Tq, int Tkv, int hd,
+                          long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
+                          float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream);
+
+/*
+ * Gradient of out = softmax(q k^T * scale + mask) v for the causal prefill of LlamaAttention under autograd
+ * (decoders/modeling_llama_mmfs.py:246-264): query i sees keys j <= i with key_mask[b, j] != 0 (key_mask (B, T) uint8
+ * or NULL); Tq = Tkv = T, no KV cache.  q, k, v, out, d_out, dq, dk, dv are (B, T, H, 128) views with batch / token
+ * strides in elements and dense heads (e.g. q / k / v and dq / dk / dv as slices of (B, T, 3, H, 128) buffers); lse
+ * (B, H, T) fp32 from mmfs_attn_forward_lse on the same q, k, v, mask and scale; delta: B*H*T floats of device scratch
+ * private to the call (it receives rowsum(d_out * out) in fp32).  dq, dk, dv are fully overwritten.
+ * Three launches (delta; dK and dV per key tile; dQ per query tile) on mma.sync tensor-core MMAs, each output element
+ * accumulated by one thread in a fixed order: no atomics, two runs give bit-identical gradients.
+ * Requires hd = 128, bf16 / f16, 16-byte aligned pointers and strides of q, k, v, d_out, dq, dk, dv, B, H <= 65535:
+ * MMFS_EUNSUPPORTED otherwise.
+ */
+int mmfs_attn_backward(const void *q, const void *k, const void *v, const void *out, const void *d_out, const float *lse,
+                       void *dq, void *dk, void *dv, float *delta, const uint8_t *key_mask, int B, int H, int T, int hd,
+                       long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
+                       long do_bs, long do_ts, long dq_bs, long dq_ts, long dk_bs, long dk_ts, long dv_bs, long dv_ts,
+                       float scale, int dtype, void *stream);
+
+/*
+ * Gradient of mmfs_rmsnorm (training path): dx (rows, cols) from x, weight and dy, fp32 math; the forward's rounding
+ * of x * rsqrt(mean(x^2) + eps) to the element type is treated as the identity.  With dweight != NULL also
+ * dweight (cols) = sum over rows of dy * cast(x * rsqrt(.)), from per-CTA fp32 partials in `partials`
+ * (min(rows, MMFS_RMSNORM_BWD_PARTS) * cols floats of device scratch private to the call) summed in a fixed order:
+ * run-to-run reproducible.  partials may be NULL when dweight is.  bf16 / f16, cols % 8 == 0, cols <= 8192, 16-byte
+ * aligned rows: MMFS_EUNSUPPORTED otherwise.
+ */
+#define MMFS_RMSNORM_BWD_PARTS 256
+int mmfs_rmsnorm_backward(const void *x, const void *weight, const void *dy, void *dx, void *dweight, float *partials,
+                          long rows, int cols, float eps, int dtype, void *stream);
+
+/*
+ * Gradient of mmfs_swiglu (training path): d_gate_up (rows, 2*inter) = [d gate | d up] of out = silu(gate) * up from
+ * gate_up (rows, 2*inter) and d_out (rows, inter), in fp32.  bf16 / f16, inter % 8 == 0, 16-byte aligned rows:
+ * MMFS_EUNSUPPORTED otherwise.  (The backward of mmfs_rope_qk is mmfs_rope_qk itself with the sin table negated: the
+ * transpose of a rotation by theta is the rotation by -theta.)
+ */
+int mmfs_swiglu_backward(const void *gate_up, const void *d_out, void *d_gate_up, long rows, int inter, int dtype,
+                         void *stream);
+
+/*
  * 2-D convolution as an implicit GEMM on the tensor cores (wgmma, TMA-shifted input boxes, no im2col buffer).
  * Replaces the cuDNN convolutions diffusers' UNet issues in the denoise step (called from
  * utils/monkey_patch/sd_unet_forward_monkey_patch.py:235-366; 3x3 stride 1/2 and 1x1, NHWC).

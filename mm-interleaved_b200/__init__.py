@@ -15,6 +15,7 @@ from .functions import MSDeformAttnFunction  # noqa: F401
 from .sampler import mmfs_sampler_forward, mmfs_sampler_locw  # noqa: F401
 from .mmfs import MMFS  # noqa: F401
 from . import ops  # noqa: F401
+from . import autograd_ops  # noqa: F401
 from .sd_mmfs import MMFSBlock, MMFSNet, PreparedSDFeatures  # noqa: F401
 from . import unet_sd, visual_tokenizer  # noqa: F401
 from .llama_mmfs import (LlamaAttention, LlamaDecoderLayer, LlamaMLP, LlamaMMFSAttention, LlamaMMFSConfig,  # noqa: F401

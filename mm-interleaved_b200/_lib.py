@@ -49,12 +49,17 @@ SIGNATURES = {
     "mmfs_attn_decode_scratch_floats": (_L, [_I] * 4),
     "mmfs_attn_decode": (_I, [_P] * 6 + [_I] * 4 + [_L] * 6 + [_F, _I, _I, _I, _P]),
     "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
+    "mmfs_attn_forward_lse": (_I, [_P] * 6 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
+    "mmfs_attn_backward": (_I, [_P] * 11 + [_I] * 4 + [_L] * 16 + [_F, _I, _P]),
+    "mmfs_rmsnorm_backward": (_I, [_P] * 6 + [_L, _I, _F, _I, _P]),
+    "mmfs_swiglu_backward": (_I, [_P] * 3 + [_L, _I, _I, _P]),
     "mmfs_decode_select": (_I, [_P, _L] + [_P] * 5 + [_I, _L, _I] + [_P] * 3 + [_I] * 4 + [_P]),
     "mmfs_beam_select": (_I, [_P, _L] + [_P] * 11 + [_I, _L, _I, _P] + [_I] * 4 + [_P]),
     "mmfs_beam_sample": (_I, [_P, _L] + [_P] * 14 + [_I, _L, _I, _I, _P] + [_I] * 4 + [_P]),
     "mmfs_kv_beam_reorder": (_I, [_P, _I, _L, _I, _L, _L, _L, _I] + [_P] * 4 + [_I, _P]),
 }
 BEAM_MAX_BEAMS, BEAM_MAX_EOS = 8, 4                  # limits of mmfs_beam_select / mmfs_beam_sample / mmfs_kv_beam_reorder
+RMSNORM_BWD_PARTS = 256                              # MMFS_RMSNORM_BWD_PARTS: dweight partial rows of mmfs_rmsnorm_backward
 
 
 def lib() -> ctypes.CDLL:

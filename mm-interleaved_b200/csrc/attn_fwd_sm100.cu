@@ -33,10 +33,13 @@ constexpr int kConsumers = 256;
 //   Q [HD/64 boxes][128 rows][128 B] | K [2 stages][HD/64][64][128 B] | V [2][HD/64][64][128 B] | barriers | items [2]
 template <int HD> constexpr int attn_ctas_per_sm() { return HD == 64 ? 2 : 1; }
 
-template <typename T, int HD>
+// LSE: also write the row log-sum-exp for the backward pass to `lse` (B, H, Tq), natural log (mmfs_attn_forward_lse).
+// The argument comes last so that the inference instantiation (LSE = false) compiles to the same code as before it.
+template <typename T, int HD, bool LSE>
 __global__ void __launch_bounds__(kAttnThreads, attn_ctas_per_sm<HD>())
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                const __grid_constant__ CUtensorMap map_v, const AttnParams p, unsigned *__restrict__ sched, int n_work) {
+                const __grid_constant__ CUtensorMap map_v, const AttnParams p, unsigned *__restrict__ sched, int n_work,
+                float *__restrict__ lse) {
     constexpr int NBOX = HD / 64;
     constexpr uint32_t QBOX_BYTES = kBM * 128, KBOX_BYTES = kBN * 128;
     constexpr uint32_t Q_BYTES = NBOX * QBOX_BYTES, KV_BYTES = NBOX * KBOX_BYTES;
@@ -229,6 +232,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
             l += __shfl_xor_sync(0xffffffffu, l, 2);
             const float inv = (l > 0.f) ? 1.f / l : 0.f;     // fully masked row -> zeros
             const int q = r0 + 8 * i;
+            if constexpr (LSE) {   // ln sum_j exp(s_j * scale) = (m * scale * log2(e) + log2(l)) * ln(2); +inf when fully masked
+                if (tq == 0 && q < p.Tq)
+                    lse[((long)b * p.H + h) * p.Tq + q] =
+                        (l > 0.f) ? fmaf(m_run[i], p.scale_log2e, __log2f(l)) * 0.6931471805599453f : INFINITY;
+            }
             if (q < p.Tq) {
                 T *op = out + (long)q * p.o_ts + 2 * tq;
 #pragma unroll
@@ -285,14 +293,14 @@ static int make_map_uncached(CUtensorMap *map, const void *ptr, int dtype, int B
     return MMFS_OK;
 }
 
-template <typename T, int HD>
+template <typename T, int HD, bool LSE>
 static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const AttnParams &p,
-                       unsigned *work_counter, cudaStream_t st) {
+                       unsigned *work_counter, float *lse, cudaStream_t st) {
     const int n_q = (p.Tq + kBM - 1) / kBM;
     const long n_work = (long)n_q * p.H * p.B;
     if (n_work >= (1L << 30)) { set_error("attn_forward: %ld work items", n_work); return MMFS_EUNSUPPORTED; }
     constexpr size_t smem = (size_t)(HD / 64) * (kBM * 128 + 4 * kBN * 128) + 14 * 8 + 2 * sizeof(int);
-    constexpr auto kern = attn_fwd_kernel<T, HD>;
+    constexpr auto kern = attn_fwd_kernel<T, HD, LSE>;
     const int rc = ensure_dynamic_smem<kern>(smem);
     if (rc != MMFS_OK) return rc;
     // more items than resident CTAs: persistent over the items the zeroed counter hands out, otherwise one item per CTA
@@ -300,7 +308,7 @@ static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUten
     const bool persistent = n_work > resident;
     if (persistent) MMFS_CUDA(cudaMemsetAsync(work_counter, 0, sizeof(unsigned), st));
     const int grid = persistent ? resident : (int)n_work;
-    kern<<<grid, kAttnThreads, smem, st>>>(mq, mk, mv, p, persistent ? work_counter : nullptr, (int)n_work);
+    kern<<<grid, kAttnThreads, smem, st>>>(mq, mk, mv, p, persistent ? work_counter : nullptr, (int)n_work, lse);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -309,10 +317,10 @@ static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUten
 
 using namespace mmfs;
 
-extern "C" int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
-                                 int B, int H, int Tq, int Tkv, int hd,
-                                 long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
-                                 float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream) {
+static int attn_forward(const void *q, const void *k, const void *v, void *out, float *lse, const uint8_t *key_mask,
+                        int B, int H, int Tq, int Tkv, int hd, long q_bs, long q_ts, long k_bs, long k_ts, long v_bs,
+                        long v_ts, long o_bs, long o_ts, float scale, int causal, int past, int dtype, unsigned *work_counter,
+                        void *stream) {
     MMFS_CHECK_ARG(B >= 0 && H > 0 && Tq >= 0 && Tkv > 0, "attn_forward: bad shape");
     if (B == 0 || Tq == 0) return MMFS_OK;
     MMFS_CHECK_ARG(q && k && v && out && work_counter, "attn_forward: null pointer argument");
@@ -337,6 +345,27 @@ extern "C" int mmfs_attn_forward(const void *q, const void *k, const void *v, vo
     cudaStream_t st = (cudaStream_t)stream;
     return dispatch_dtype<kF16Types>(dtype, "attn_forward", [&](auto tag) {
         using T = typename decltype(tag)::type;
-        return hd == 64 ? launch_attn<T, 64>(mq, mk, mv, p, work_counter, st) : launch_attn<T, 128>(mq, mk, mv, p, work_counter, st);
+        if (lse != nullptr)
+            return hd == 64 ? launch_attn<T, 64, true>(mq, mk, mv, p, work_counter, lse, st)
+                            : launch_attn<T, 128, true>(mq, mk, mv, p, work_counter, lse, st);
+        return hd == 64 ? launch_attn<T, 64, false>(mq, mk, mv, p, work_counter, lse, st)
+                        : launch_attn<T, 128, false>(mq, mk, mv, p, work_counter, lse, st);
     });
+}
+
+extern "C" int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask,
+                                 int B, int H, int Tq, int Tkv, int hd,
+                                 long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
+                                 float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream) {
+    return attn_forward(q, k, v, out, nullptr, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts,
+                        scale, causal, past, dtype, work_counter, stream);
+}
+
+extern "C" int mmfs_attn_forward_lse(const void *q, const void *k, const void *v, void *out, float *lse,
+                                     const uint8_t *key_mask, int B, int H, int Tq, int Tkv, int hd,
+                                     long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
+                                     float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream) {
+    MMFS_CHECK_ARG(lse != nullptr, "attn_forward_lse: null pointer argument (lse)");
+    return attn_forward(q, k, v, out, lse, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts,
+                        scale, causal, past, dtype, work_counter, stream);
 }

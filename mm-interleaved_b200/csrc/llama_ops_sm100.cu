@@ -4,6 +4,7 @@
 //   mmfs_rope_qk      apply_rotary_pos_emb / rotate_half decoders/modeling_llama_mmfs.py:158-172
 //   mmfs_swiglu       LlamaMLP: act_fn(gate) * up        decoders/modeling_llama_mmfs.py:188-189
 //   mmfs_layernorm    nn.LayerNorm (CLIP / Q-Former / MMFSBlock norms)
+//   mmfs_rmsnorm_backward, mmfs_swiglu_backward   their gradients (training path, 16-bit tensors, fp32 math)
 //
 // Each mimics the rounding points of the reference's tensor pipeline in the storage type T (a
 // tensor op in bf16 rounds its result to bf16), so a bf16 run tracks the reference's bf16 run and
@@ -421,6 +422,114 @@ static int launch_rope_append(void *q, const void *k, const void *v, const float
     return MMFS_OK;
 }
 
+
+// ---- RMSNorm backward: dx = r * (g - x * r^2 * mean(g * x)), g = dy * w; dweight = sum over rows of dy * cast_T(x * r) --
+// CTA p of kRmsBwdParts takes rows p, p + parts, ... in that order and keeps its dweight partial in shared memory
+// (every thread owns the same columns for every row, so no synchronisation); the partials are summed per column in
+// part order by rmsnorm_dw_reduce_kernel.  The part count depends only on `rows`, so the sum is run-to-run reproducible.
+constexpr int kRmsBwdParts = MMFS_RMSNORM_BWD_PARTS;
+constexpr int kRmsBwdMaxCols = 8192;
+
+template <typename T>
+__global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const T *__restrict__ x, const T *__restrict__ w,
+                                                          const T *__restrict__ dy, T *__restrict__ dx,
+                                                          float *__restrict__ partials, long rows, int cols, float eps) {
+    constexpr int VEC = 16 / (int)sizeof(T);
+    extern __shared__ float s_dw[];                           // cols floats, only with partials
+    __shared__ float s_red[32];
+    const int nvec = cols / VEC;
+    if (partials)
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x)
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) s_dw[i * VEC + k] = 0.f;
+    for (long row = blockIdx.x; row < rows; row += gridDim.x) {
+        const T *xr = x + row * cols, *dyr = dy + row * cols;
+        float ss = 0.f, sg = 0.f;
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+            float f[VEC], g[VEC], d[VEC];
+            Vec16<T>::unpack(ldg_nc_v4(xr + i * VEC), f);
+            Vec16<T>::unpack(ldg_nc_v4(w + i * VEC), g);
+            Vec16<T>::unpack(ldg_nc_v4(dyr + i * VEC), d);
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) { ss = fmaf(f[k], f[k], ss); sg = fmaf(d[k] * g[k], f[k], sg); }
+        }
+        ss = block_sum(ss, s_red);
+        sg = block_sum(sg, s_red);
+        const float r = rsqrtf(ss / (float)cols + eps);         // the forward's statistic
+        const float coef = r * r * r * sg / (float)cols;
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+            float f[VEC], g[VEC], d[VEC], o[VEC];
+            Vec16<T>::unpack(ldg_nc_v4(xr + i * VEC), f);
+            Vec16<T>::unpack(ldg_nc_v4(w + i * VEC), g);
+            Vec16<T>::unpack(ldg_nc_v4(dyr + i * VEC), d);
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) o[k] = fmaf(r * d[k], g[k], -f[k] * coef);
+            stg_v4(dx + row * cols + i * VEC, Vec16<T>::pack(o));
+            if (partials)
+#pragma unroll
+                for (int k = 0; k < VEC; ++k) s_dw[i * VEC + k] = fmaf(d[k], rnd<T>(f[k] * r), s_dw[i * VEC + k]);
+        }
+    }
+    if (partials)
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x)
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) partials[(long)blockIdx.x * cols + i * VEC + k] = s_dw[i * VEC + k];
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) rmsnorm_dw_reduce_kernel(const float *__restrict__ partials, T *__restrict__ dw,
+                                                                int parts, int cols) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= cols) return;
+    float s = 0.f;
+    for (int p = 0; p < parts; ++p) s += partials[(long)p * cols + c];
+    dw[c] = from_op<T>(s);
+}
+
+// ---- SwiGLU backward: out = silu(g) * u  ->  dg = d * u * s * (1 + g * (1 - s)), du = d * silu(g), s = sigmoid(g) ----
+template <typename T>
+__global__ void __launch_bounds__(256) swiglu_bwd_kernel(const T *__restrict__ gu, const T *__restrict__ d_out,
+                                                         T *__restrict__ d_gu, long rows, int I) {
+    constexpr int VEC = 16 / (int)sizeof(T);
+    const int nvec = I / VEC;
+    for (long r = blockIdx.x; r < rows; r += gridDim.x)
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+            float g[VEC], u[VEC], d[VEC], dg[VEC], du[VEC];
+            Vec16<T>::unpack(ldg_nc_v4(gu + r * 2 * I + i * VEC), g);
+            Vec16<T>::unpack(ldg_nc_v4(gu + r * 2 * I + I + i * VEC), u);
+            Vec16<T>::unpack(ldg_nc_v4(d_out + r * I + i * VEC), d);
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) {
+                const float s = 1.f / (1.f + expf(-g[k]));
+                dg[k] = d[k] * u[k] * s * fmaf(g[k], 1.f - s, 1.f);
+                du[k] = d[k] * g[k] * s;
+            }
+            stg_v4(d_gu + r * 2 * I + i * VEC, Vec16<T>::pack(dg));
+            stg_v4(d_gu + r * 2 * I + I + i * VEC, Vec16<T>::pack(du));
+        }
+}
+
+template <typename T>
+static int launch_rmsnorm_bwd(const void *x, const void *w, const void *dy, void *dx, void *dw, float *partials, long rows,
+                              int cols, float eps, cudaStream_t st) {
+    const int parts = (int)(rows < kRmsBwdParts ? rows : kRmsBwdParts);
+    rmsnorm_bwd_kernel<T><<<parts, 256, dw ? cols * sizeof(float) : 0, st>>>(
+        (const T *)x, (const T *)w, (const T *)dy, (T *)dx, dw ? partials : nullptr, rows, cols, eps);
+    MMFS_CUDA(cudaGetLastError());
+    if (dw) {
+        rmsnorm_dw_reduce_kernel<T><<<(cols + 255) / 256, 256, 0, st>>>(partials, (T *)dw, parts, cols);
+        MMFS_CUDA(cudaGetLastError());
+    }
+    return MMFS_OK;
+}
+
+template <typename T>
+static int launch_swiglu_bwd(const void *gu, const void *d_out, void *d_gu, long rows, int inter, cudaStream_t st) {
+    swiglu_bwd_kernel<T><<<capped_grid(rows, 8), 256, 0, st>>>((const T *)gu, (const T *)d_out, (T *)d_gu, rows, inter);
+    MMFS_CUDA(cudaGetLastError());
+    return MMFS_OK;
+}
+
 }  // namespace mmfs
 
 using namespace mmfs;
@@ -501,5 +610,37 @@ extern "C" int mmfs_geglu(const void *value_gate, void *out, long rows, int inte
                    "geglu: rows must be 16-byte aligned");
     return dispatch_dtype<kF32Types>(dtype, "geglu", [&](auto tag) {
         return launch_glu<typename decltype(tag)::type>(value_gate, out, rows, inter, true, (cudaStream_t)stream);
+    });
+}
+
+extern "C" int mmfs_rmsnorm_backward(const void *x, const void *weight, const void *dy, void *dx, void *dweight,
+                                     float *partials, long rows, int cols, float eps, int dtype, void *stream) {
+    MMFS_CHECK_ARG(rows >= 0 && cols > 0, "rmsnorm_backward: bad shape");
+    if (rows == 0) return MMFS_OK;
+    MMFS_CHECK_ARG(x && weight && dy && dx && (!dweight || partials), "rmsnorm_backward: null pointer argument");
+    if (!(dtype == MMFS_BF16 || dtype == MMFS_F16) || cols % 8 != 0 || cols > kRmsBwdMaxCols ||
+        ((uintptr_t)x | (uintptr_t)weight | (uintptr_t)dy | (uintptr_t)dx) % 16 != 0) {
+        set_error("rmsnorm_backward: needs bf16 / f16, cols %% 8 == 0, cols <= %d, 16-byte aligned rows (got cols=%d dtype=%d)",
+                  kRmsBwdMaxCols, cols, dtype);
+        return MMFS_EUNSUPPORTED;
+    }
+    return dispatch_dtype<kF16Types, MMFS_EUNSUPPORTED>(dtype, "rmsnorm_backward", [&](auto tag) {
+        return launch_rmsnorm_bwd<typename decltype(tag)::type>(x, weight, dy, dx, dweight, partials, rows, cols, eps,
+                                                                (cudaStream_t)stream);
+    });
+}
+
+extern "C" int mmfs_swiglu_backward(const void *gate_up, const void *d_out, void *d_gate_up, long rows, int inter, int dtype,
+                                    void *stream) {
+    MMFS_CHECK_ARG(rows >= 0 && inter > 0, "swiglu_backward: bad shape");
+    if (rows == 0) return MMFS_OK;
+    MMFS_CHECK_ARG(gate_up && d_out && d_gate_up, "swiglu_backward: null pointer argument");
+    if (!(dtype == MMFS_BF16 || dtype == MMFS_F16) || inter % 8 != 0 ||
+        ((uintptr_t)gate_up | (uintptr_t)d_out | (uintptr_t)d_gate_up) % 16 != 0) {
+        set_error("swiglu_backward: needs bf16 / f16, inter %% 8 == 0 and 16-byte aligned rows (got inter=%d dtype=%d)", inter, dtype);
+        return MMFS_EUNSUPPORTED;
+    }
+    return dispatch_dtype<kF16Types, MMFS_EUNSUPPORTED>(dtype, "swiglu_backward", [&](auto tag) {
+        return launch_swiglu_bwd<typename decltype(tag)::type>(gate_up, d_out, d_gate_up, rows, inter, (cudaStream_t)stream);
     });
 }

@@ -29,7 +29,9 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from . import ops
+import torch.utils.checkpoint
+
+from . import autograd_ops, ops
 from ._cache import SourceCache, WeightCache
 from .mmfs import MMFS
 
@@ -53,6 +55,28 @@ class LlamaMMFSConfig:
     use_cache: bool = True
 
 
+def records_grad(module, *tensors) -> bool:
+    """Whether autograd records this call: grad mode is on and an input or a parameter of ``module`` requires grad.
+    Only then do the modules below take their training path (autograd_ops); otherwise they run the inference kernels."""
+    if not torch.is_grad_enabled():
+        return False
+    return (any(t is not None and torch.is_tensor(t) and t.requires_grad for t in tensors)
+            or any(p.requires_grad for p in module.parameters()))
+
+
+def check_training_dtype(what, t):
+    if t.dtype not in (torch.bfloat16, torch.float16):
+        raise RuntimeError(f"{what}: the backward kernels take bf16 / fp16 only (got {t.dtype}); cast the model, or run "
+                           "under torch.no_grad()")
+
+
+def _cat_weight(cat, linears):
+    """The concatenated weight, differentiable when a source weight is trainable (the cached copy is built without grad)."""
+    if any(l.weight.requires_grad for l in linears):
+        return torch.cat([l.weight for l in linears], 0)
+    return cat.get()
+
+
 class LlamaRMSNorm(nn.Module):
     def __init__(self, hidden_size, eps=1e-6):
         super().__init__()
@@ -60,6 +84,9 @@ class LlamaRMSNorm(nn.Module):
         self.variance_epsilon = eps
 
     def forward(self, hidden_states):
+        if records_grad(self, hidden_states):
+            check_training_dtype("LlamaRMSNorm", hidden_states)
+            return autograd_ops.rmsnorm(hidden_states, self.weight.to(hidden_states.dtype), self.variance_epsilon)
         return ops.rmsnorm(hidden_states.contiguous(), self.weight, self.variance_epsilon)
 
 
@@ -126,6 +153,12 @@ class LlamaMLP(nn.Module):
 
     def forward(self, x, residual=None, inplace=False):
         """``inplace``: accumulate into ``residual``'s storage (beta = 1 GEMM epilogue, no copy of the stream)."""
+        if records_grad(self, x, residual):
+            check_training_dtype("LlamaMLP", x)
+            act = autograd_ops.swiglu(F.linear(x, _cat_weight(self._gate_up, (self.gate_proj, self.up_proj))))
+            if residual is None:
+                return self.down_proj(act)
+            return _addmm_residual(residual, act, self.down_proj.weight, False)
         gu = F.linear(x, self._gate_up.get())                 # [gate | up] in one GEMM
         act = ops.swiglu(gu)
         if residual is None:
@@ -206,6 +239,8 @@ class LlamaAttention(nn.Module):
             raise NotImplementedError("attention probabilities are never materialised by the fused kernel")
         B, T, _ = hidden_states.shape
         H, hd = self.num_heads, self.head_dim
+        if records_grad(self, hidden_states, residual):
+            return self._forward_training(hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual)
         qkv = F.linear(hidden_states, self._qkv.get()).view(B, T, 3, H, hd)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
         static = isinstance(past_key_value, StaticKV)
@@ -242,6 +277,30 @@ class LlamaAttention(nn.Module):
         ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)       # (B, T, H*hd)
         out = self.o_proj(ctx) if residual is None else _addmm_residual(residual, ctx, self.o_proj.weight, inplace)
         return out, None, present
+
+    def _forward_training(self, hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual):
+        """The prefill under autograd: QKV GEMM -> RoPE -> causal attention (saving O and the row log-sum-exp) -> o_proj,
+        each step with its backward (autograd_ops)."""
+        if past_key_value is not None or use_cache:
+            raise RuntimeError("LlamaAttention under autograd runs the prefill without a KV cache: pass use_cache=False "
+                               "and no past_key_values, or run under torch.no_grad()")
+        check_training_dtype("LlamaAttention", hidden_states)
+        if self.head_dim != 128:
+            raise RuntimeError(f"LlamaAttention under autograd needs head dim 128 (the attention backward kernel's), "
+                               f"got {self.head_dim}")
+        B, T, _ = hidden_states.shape
+        w = _cat_weight(self._qkv, (self.q_proj, self.k_proj, self.v_proj))
+        qkv = F.linear(hidden_states, w).view(B, T, 3, self.num_heads, self.head_dim)
+        if position_ids is None:
+            position_ids = torch.arange(T, device=hidden_states.device)
+        cos, sin = self.rope_tables(hidden_states.device, T)
+        qkv = autograd_ops.rope_qkv(qkv, cos, sin, position_ids)
+        key_mask = attention_mask
+        if attention_mask is not None and attention_mask.dim() == 4:
+            key_mask = attention_mask[:, 0, -1, :] > (torch.finfo(attention_mask.dtype).min / 2)
+        ctx = autograd_ops.attention(qkv, key_mask)
+        out = self.o_proj(ctx) if residual is None else _addmm_residual(residual, ctx, self.o_proj.weight, False)
+        return out, None, None
 
 
 class LlamaMMFSAttention(nn.Module):
@@ -293,6 +352,8 @@ class LlamaMMFSAttention(nn.Module):
         return self.attn.project_value(self.norm2(vision_hidden_states))
 
     def forward(self, hidden_states, vision_hidden_states=None, cross_attention_mask=None, residual=None, inplace=False):
+        if records_grad(self, hidden_states, residual, vision_hidden_states if torch.is_tensor(vision_hidden_states) else None):
+            return self._forward_training(hidden_states, vision_hidden_states, cross_attention_mask, residual)
         h = self.norm1(hidden_states)
         value = None
         if isinstance(vision_hidden_states, PreparedVision):
@@ -321,6 +382,20 @@ class LlamaMMFSAttention(nn.Module):
         if residual is None:
             return out * gate
         return torch.addcmul(residual, out, gate)
+
+    def _forward_training(self, hidden_states, vision_hidden_states, cross_attention_mask, residual):
+        """Under autograd: RMSNorms with their backward, then MMFS's differentiable path (front end in PyTorch, the
+        gather through MSDeformAttnFunction) and the tanh gate."""
+        if isinstance(vision_hidden_states, PreparedVision):
+            raise RuntimeError("LlamaMMFSAttention under autograd takes the vision feature tensor, not PreparedVision "
+                               "(an inference-only cache)")
+        h = self.norm1(hidden_states)
+        v = self.norm2(vision_hidden_states)
+        _, n_img, hw, _ = v.shape
+        shapes, starts, ref = self._geometry(h.device, n_img, hw, h.shape[1])
+        out = self.attn.forward_differentiable(h, ref, v, shapes, starts, cross_attention_mask)
+        out = out * self.gate.tanh().to(out.dtype)
+        return out if residual is None else residual + out
 
 
 class LlamaDecoderLayer(nn.Module):
@@ -402,7 +477,9 @@ class LlamaModel(nn.Module):
     def forward(self, input_ids=None, attention_mask=None, position_ids=None, past_key_values=None,
                 inputs_embeds=None, vision_hidden_states=None, cross_attention_mask=None, use_cache=None,
                 output_attentions=None, output_hidden_states=None, return_dict=None):
-        use_cache = self.config.use_cache if use_cache is None else use_cache
+        if use_cache is None:   # under autograd the default is no cache, as HF's training path forces it
+            grad = records_grad(self, inputs_embeds, vision_hidden_states if torch.is_tensor(vision_hidden_states) else None)
+            use_cache = False if grad else self.config.use_cache
         return_dict = True if return_dict is None else return_dict
         if output_attentions:
             raise NotImplementedError("attention probabilities are never materialised")
@@ -427,6 +504,12 @@ class LlamaModel(nn.Module):
                 raise ValueError(f"attention_mask should be of size {(B, past + T)}, but is {tuple(attention_mask.shape)}")
             key_mask = attention_mask.to(torch.uint8)
 
+        training = records_grad(self, inputs_embeds, vision_hidden_states if torch.is_tensor(vision_hidden_states) else None)
+        if training:
+            if use_cache or past_key_values is not None:
+                raise RuntimeError("LlamaModel under autograd runs the prefill without a KV cache: pass use_cache=False "
+                                   "and no past_key_values, or run under torch.no_grad()")
+            check_training_dtype("LlamaModel", inputs_embeds)
         hidden_states = inputs_embeds
         inplace = not torch.is_grad_enabled() and not output_hidden_states
         if inplace:                      # one private copy of the stream; every layer then accumulates into it
@@ -436,10 +519,15 @@ class LlamaModel(nn.Module):
         for idx, layer in enumerate(self.layers):
             if output_hidden_states:
                 all_hidden += (hidden_states,)
-            outs = layer(hidden_states, vision_hidden_states, cross_attention_mask, attention_mask=key_mask,
-                         position_ids=position_ids,
-                         past_key_value=past_key_values[idx] if past_key_values is not None else None,
-                         use_cache=use_cache, inplace=inplace)
+            if training and self.gradient_checkpointing:   # activations recomputed in the backward, per layer (as HF)
+                outs = torch.utils.checkpoint.checkpoint(layer, hidden_states, vision_hidden_states, cross_attention_mask,
+                                                         attention_mask=key_mask, position_ids=position_ids,
+                                                         use_reentrant=False)
+            else:
+                outs = layer(hidden_states, vision_hidden_states, cross_attention_mask, attention_mask=key_mask,
+                             position_ids=position_ids,
+                             past_key_value=past_key_values[idx] if past_key_values is not None else None,
+                             use_cache=use_cache, inplace=inplace)
             hidden_states = outs[0]
             if use_cache:
                 next_cache += (outs[1],)

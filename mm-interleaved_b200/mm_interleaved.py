@@ -1121,7 +1121,7 @@ class MMInterleaved(InterleavedForward):
         self.loss_img_weight, self.loss_txt_weight = loss_img_weight, loss_txt_weight
         self.num_img_token = num_img_token
         self.dataset_to_ignore_noimage_cond_loss = list(dataset_to_ignore_noimage_cond_loss)
-        self.mm_decoder.gradient_checkpointing = use_llama_gradient_checkpointing      # inference: unused
+        self.mm_decoder.gradient_checkpointing = use_llama_gradient_checkpointing      # used under autograd only
         self._tok_graph = None
 
     # ---------------------------------------------------------------------------------------------------------
@@ -1197,7 +1197,16 @@ class MMInterleaved(InterleavedForward):
         ``image_tensors``) with the per-image contexts and previous-image MMFS features (from ``nearest_bos_idxs``),
         ``loss_img`` = its detached mean and ``loss = loss_txt * w_txt + loss_img * w_img``; ``multiscale_features``
         then leaves the output, as there.  ``generator`` (keyword) seeds the image loss's random draws.
-        Inference-only kernels: call under ``torch.no_grad()``."""
+        Under autograd the text loss is differentiable (``freeze_like_reference``); a trainable visual tokenizer or an
+        image loss raises up front, as neither has a backward here."""
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            if any(p.requires_grad for p in self.visual_tokenizer.parameters()):
+                raise RuntimeError("MMInterleaved.forward under autograd: the visual tokenizer has no backward here; "
+                                   "freeze it (model.visual_tokenizer.requires_grad_(False)) or run under torch.no_grad()")
+            if self._has_image_loss():
+                raise RuntimeError("MMInterleaved.forward under autograd: the image-decoder loss has no backward here; "
+                                   "build the image decoder's VAE without an encoder (no image loss) or run under "
+                                   "torch.no_grad()")
         return_loss = kwargs.pop("return_loss", True)
         generator = kwargs.pop("generator", None)
         out = self._prepare_mm_embeds(text_ids, image_tensors, num_image_per_seq, meta, kwargs.pop("max_num_image", None))
@@ -1227,6 +1236,22 @@ class MMInterleaved(InterleavedForward):
             wi = self.loss_img_weight if loss_img_weight is None else loss_img_weight
             out.update(loss_img=loss_img.detach(), loss=out["loss"] + loss_img * wi)
         return out
+
+    def freeze_like_reference(self):
+        """The trainable set of the reference's constructor that this repository can differentiate (mm_interleaved.py:74-78,
+        decoder_text.py:50-51): the LLM frozen except its ``llama_cross_attn`` blocks, the text head frozen except
+        ``head_new``, ``soi_token`` trainable.  Returns ``self``.
+
+        The reference also trains the visual tokenizer's adapter and Q-Former and the image decoder; those have no
+        backward here, so this leaves them as they are, and ``forward`` under autograd raises while any visual-tokenizer
+        parameter requires grad or the image loss is on: freeze them (``model.visual_tokenizer.requires_grad_(False)``)
+        to train the text loss."""
+        for name, p in self.mm_decoder.named_parameters():
+            p.requires_grad_("llama_cross_attn" in name)
+        self.text_decoder.requires_grad_(False)
+        self.text_decoder.head_new.requires_grad_(True)
+        self.soi_token.requires_grad_(True)
+        return self
 
     def _has_image_loss(self) -> bool:
         sd = getattr(self.image_decoder, "decoder", None)

@@ -185,3 +185,44 @@ class MMFS(nn.Module):
         if output_weight is not None:
             return F.linear(sampled, output_weight, output_bias)
         return self.output_proj(sampled)
+
+    def forward_differentiable(self, query, reference_points, input_flatten, input_spatial_shapes, input_level_start_index,
+                               attention_mask):
+        """``forward`` under autograd (prefill; 2-D reference points; no padding mask): the sampler's front end restated
+        in PyTorch -- per-image offsets and logits from ``dynamic_offset_mask(query)`` plus the ``query_relpos`` row of
+        the image's relative index, ``scale_ratios``, the -1e4 image mask, the null slot -log L, the softmax over
+        L * (P + 1) and the locations ``ref + off / (W, H)`` (mmfs.py:174-250) -- then the gather through
+        ``MSDeformAttnFunction`` (deterministic backward kernel), the ignore-token term and ``output_proj``.  The
+        (N, Lq, M, L, P, 2) locations and (N, Lq, M, L, P) weights are materialised on this path only."""
+        from .functions import MSDeformAttnFunction
+        N, Lq, _ = query.shape
+        n_img = attention_mask.shape[-1]
+        M, P, NL = self.n_heads, self.n_points, self.n_levels
+        L = n_img * NL
+        if input_spatial_shapes.shape[0] != L or input_flatten.shape[1] != n_img:
+            raise RuntimeError("MMFS: input_spatial_shapes / input_flatten must cover n_images * n_levels levels")
+        if n_img >= self.max_num_image_per_seq:
+            raise RuntimeError(f"MMFS: {n_img} images per sequence need max_num_image_per_seq > {n_img}")
+        if attention_mask.ndim == 3 and attention_mask.shape[1] != Lq:
+            raise RuntimeError("MMFS under autograd takes the prefill's (N, Lq, n_images) or (N, n_images) mask")
+        value = self.project_value(input_flatten, cache=False)                     # (N, n_img*hw, M, D)
+        rel = relative_image_index(attention_mask, Lq).long()                     # (N, n_img, 1 | Lq)
+        q = self.dynamic_offset_mask(query)[:, None] + self.query_relpos(rel)      # (N, n_img, Lq, C)
+        off = self.sampling_offsets(q).view(N, n_img, Lq, M, 1, P, 2).permute(0, 2, 3, 1, 4, 5, 6)
+        off = (off * self.scale_ratios.to(off.dtype).view(1, 1, 1, 1, NL, 1, 1)).reshape(N, Lq, M, L, P, 2)
+        aw = self.attention_weights(q).view(N, n_img, Lq, M, NL, P + 1).permute(0, 2, 3, 1, 4, 5).reshape(N, Lq, M, L, P + 1)
+        am = (1.0 - attention_mask.to(aw.dtype)) * -10000.0
+        am = am.view(N, 1 if am.ndim == 2 else Lq, 1, n_img, 1).repeat_interleave(NL, dim=3)
+        aw = aw + am
+        aw = torch.cat([aw[..., :-1], torch.full_like(aw[..., -1:], -math.log(L))], -1)
+        aw = F.softmax(aw.reshape(N, Lq, M, L * (P + 1)), -1).view(N, Lq, M, L, P + 1)
+        null_mass = aw[..., -1].sum(3)                                              # (N, Lq, M)
+        shapes = input_spatial_shapes
+        normalizer = torch.stack([shapes[..., 1], shapes[..., 0]], -1).to(off.dtype)
+        loc = reference_points[:, :, None, :, None, :] + off / normalizer[None, None, None, :, None, :]
+        sampled = MSDeformAttnFunction.apply(value, shapes.contiguous(), input_level_start_index.contiguous(),
+                                             loc.to(value.dtype).contiguous(), aw[..., :-1].to(value.dtype).contiguous(),
+                                             self.im2col_step)
+        ign = self.ignore_token.view(1, 1, M, -1).to(sampled.dtype)                 # mmfs.py:236-241
+        sampled = sampled + (ign * null_mass.unsqueeze(-1).to(sampled.dtype)).reshape(N, Lq, -1)
+        return self.output_proj(sampled)

@@ -386,6 +386,106 @@ def attention(q, k, v, key_mask=None, causal=True, past=0, scale=None, force_gen
     return out.view(B, Tq, H * hd)
 
 
+# ---- training path: backward kernels (csrc/attn_bwd_sm100.cu, csrc/llama_ops_sm100.cu).  autograd_ops.py wraps them in
+# autograd Functions; like the forward wrappers they refuse to run where autograd would record them.
+
+def _check_qkv_view(t, B, T, H, hd, what):
+    _require(t.is_cuda and tuple(t.shape) == (B, T, H, hd) and t.stride(3) == 1 and t.stride(2) == hd,
+             f"{what}: tensors must be (B, T, H, hd) CUDA views with dense heads")
+
+
+def attention_forward_lse(q, k, v, key_mask=None, scale=None):
+    """Causal ``attention`` on the wgmma kernel that also returns the row log-sum-exp: ``(out (B,T,H,hd), lse (B,H,T)
+    fp32)``, natural log, +inf for a row that sees no key.  ``out`` is bit-identical to ``attention``'s (same kernel)."""
+    B, T, H, hd = q.shape
+    inference_only("attention_forward_lse", q, k, v)
+    for t in (q, k, v):
+        _check_qkv_view(t, B, T, H, hd, "attention_forward_lse")
+    scale = float(scale if scale is not None else hd ** -0.5)
+    out = torch.empty((B, T, H, hd), dtype=q.dtype, device=q.device)
+    lse = torch.empty((B, H, T), dtype=torch.float32, device=q.device)
+    km = None
+    if key_mask is not None:
+        km = key_mask.to(torch.uint8).contiguous()
+        _require(tuple(km.shape) == (B, T), "attention_forward_lse: key_mask must be (B, T)")
+    counter = torch.empty((1,), dtype=torch.int32, device=q.device)
+    with torch.cuda.device(q.device):
+        rc = _lib.lib().mmfs_attn_forward_lse(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), km.data_ptr() if km is not None else None,
+            B, H, T, T, hd, q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1),
+            out.stride(0), out.stride(1), scale, 1, 0, _DTYPE_CODE[q.dtype], counter.data_ptr(), _stream())
+    _lib.check(rc, "attention_forward_lse")
+    launch_counter[0] += 1
+    return out, lse
+
+
+def attention_backward(q, k, v, out, d_out, lse, dq, dk, dv, key_mask=None, scale=None) -> None:
+    """dQ, dK, dV of causal ``attention_forward_lse`` (hd 128, bf16 / fp16), written into the (B, T, H, hd) views
+    ``dq`` / ``dk`` / ``dv`` -- e.g. slices of one (B, T, 3, H, hd) buffer, so that the QKV projection's backward is
+    one GEMM.  Deterministic: no atomics, two calls give bit-identical results."""
+    B, T, H, hd = q.shape
+    inference_only("attention_backward", q, k, v, out, d_out)
+    for t in (q, k, v, out, d_out, dq, dk, dv):
+        _check_qkv_view(t, B, T, H, hd, "attention_backward")
+    _require(all(t.dtype == q.dtype for t in (k, v, out, d_out, dq, dk, dv)), "attention_backward: dtype mismatch")
+    _require(lse.dtype == torch.float32 and tuple(lse.shape) == (B, H, T) and lse.is_contiguous(),
+             "attention_backward: lse must be contiguous fp32 (B, H, T)")
+    scale = float(scale if scale is not None else hd ** -0.5)
+    km = None
+    if key_mask is not None:
+        km = key_mask.to(torch.uint8).contiguous()
+        _require(tuple(km.shape) == (B, T), "attention_backward: key_mask must be (B, T)")
+    delta = torch.empty((B, H, T), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        rc = _lib.lib().mmfs_attn_backward(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), d_out.data_ptr(), lse.data_ptr(), dq.data_ptr(),
+            dk.data_ptr(), dv.data_ptr(), delta.data_ptr(), km.data_ptr() if km is not None else None, B, H, T, hd,
+            q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1), out.stride(0), out.stride(1),
+            d_out.stride(0), d_out.stride(1), dq.stride(0), dq.stride(1), dk.stride(0), dk.stride(1), dv.stride(0),
+            dv.stride(1), scale, _DTYPE_CODE[q.dtype], _stream())
+    _lib.check(rc, "attention_backward")
+    launch_counter[0] += 3
+
+
+def rmsnorm_backward(x: torch.Tensor, weight: torch.Tensor, dy: torch.Tensor, eps: float, weight_grad: bool = True):
+    """(dx, dweight) of ``rmsnorm`` over the last dim; dweight is None unless ``weight_grad``.  dweight is reduced from
+    fixed per-CTA partials in a fixed order (run-to-run reproducible)."""
+    inference_only("rmsnorm_backward", x, weight, dy)
+    _require(x.is_cuda and x.is_contiguous() and dy.is_contiguous() and weight.is_contiguous() and dy.shape == x.shape,
+             "rmsnorm_backward: contiguous CUDA tensors of one shape required")
+    _require(weight.dtype == x.dtype == dy.dtype and weight.numel() == x.shape[-1], "rmsnorm_backward: weight dtype / size mismatch")
+    cols = x.shape[-1]
+    rows = x.numel() // cols
+    dx = torch.empty_like(x)
+    dw = torch.empty_like(weight) if weight_grad else None
+    partials = (torch.empty((min(rows, _lib.RMSNORM_BWD_PARTS), cols), dtype=torch.float32, device=x.device)
+                if weight_grad else None)
+    with torch.cuda.device(x.device):
+        rc = _lib.lib().mmfs_rmsnorm_backward(x.data_ptr(), weight.data_ptr(), dy.data_ptr(), dx.data_ptr(),
+                                              dw.data_ptr() if dw is not None else None,
+                                              partials.data_ptr() if partials is not None else None, rows, cols, float(eps),
+                                              _DTYPE_CODE[x.dtype], _stream())
+    _lib.check(rc, "rmsnorm_backward")
+    launch_counter[0] += 2 if weight_grad else 1
+    return dx, dw
+
+
+def swiglu_backward(gate_up: torch.Tensor, d_out: torch.Tensor) -> torch.Tensor:
+    """d(gate_up) of ``swiglu``: [d gate | d up], computed in fp32."""
+    inference_only("swiglu_backward", gate_up, d_out)
+    _require(gate_up.is_cuda and gate_up.is_contiguous() and d_out.is_contiguous() and gate_up.shape[-1] % 2 == 0
+             and d_out.shape == gate_up.shape[:-1] + (gate_up.shape[-1] // 2,) and d_out.dtype == gate_up.dtype,
+             "swiglu_backward: bad input")
+    inter = gate_up.shape[-1] // 2
+    d_gu = torch.empty_like(gate_up)
+    with torch.cuda.device(gate_up.device):
+        rc = _lib.lib().mmfs_swiglu_backward(gate_up.data_ptr(), d_out.data_ptr(), d_gu.data_ptr(),
+                                             gate_up.numel() // (2 * inter), inter, _DTYPE_CODE[gate_up.dtype], _stream())
+    _lib.check(rc, "swiglu_backward")
+    launch_counter[0] += 1
+    return d_gu
+
+
 def conv2d_supported(x: torch.Tensor, weight: torch.Tensor, stride: int, padding: int) -> bool:
     """Whether ``conv2d`` can take this layer (else the caller keeps it on cuDNN: conv_in / conv_out of the UNet)."""
     if x.dtype not in (torch.bfloat16, torch.float16) or not x.is_cuda or x.dim() != 4:
