@@ -265,6 +265,36 @@ int mmfs_attn_backward(const void *q, const void *k, const void *v, const void *
                        float scale, int dtype, void *stream);
 
 /*
+ * mmfs_attn_backward for any head dim the forward takes, with or without causality, and with queries and keys of
+ * different lengths (the Q-Former's self-attention over its queries and cross-attention to the image tokens): query i
+ * sees keys j < Tkv with key_mask[b, j] != 0 (key_mask (B, Tkv) uint8 or NULL) and, when `causal`, j <= i.  q, out,
+ * d_out, dq are (B, Tq, H, hd) views and k, v, dk, dv (B, Tkv, H, hd) views, each with its own batch / token strides in
+ * elements and dense heads; lse (B, H, Tq) fp32 from mmfs_attn_forward_lse on the same q, k, v, mask, scale and
+ * causality; delta: B*H*Tq floats of device scratch private to the call.  dq, dk, dv are fully overwritten (a key no
+ * query sees gets zero dk / dv).  Same kernels, launches and determinism as mmfs_attn_backward, which is this call with
+ * hd = 128, causal = 1 and Tq = Tkv.
+ * Negative B, H <= 0, Tq <= 0, Tkv <= 0, hd <= 0, causal with Tq != Tkv, null pointers: MMFS_EINVAL.  hd not in
+ * {64, 128}, a dtype other than bf16 / f16, pointers or strides of q, k, v, d_out, dq, dk, dv not 16-byte aligned,
+ * B or H > 65535: MMFS_EUNSUPPORTED.
+ */
+int mmfs_attn_backward_general(const void *q, const void *k, const void *v, const void *out, const void *d_out,
+                               const float *lse, void *dq, void *dk, void *dv, float *delta, const uint8_t *key_mask,
+                               int B, int H, int Tq, int Tkv, int hd, long q_bs, long q_ts, long k_bs, long k_ts, long v_bs,
+                               long v_ts, long o_bs, long o_ts, long do_bs, long do_ts, long dq_bs, long dq_ts, long dk_bs,
+                               long dk_ts, long dv_bs, long dv_ts, float scale, int causal, int dtype, void *stream);
+
+/*
+ * Gradient of mmfs_layernorm (training path): dx (rows, cols) from x, weight and dy, with the row mean and biased
+ * variance recomputed from x in fp32 (the forward rounds only its output).  With dweight and / or dbias != NULL also
+ * dweight (cols) = sum over rows of dy * (x - mean) * rsqrt(var + eps) and dbias (cols) = sum over rows of dy, from
+ * per-CTA fp32 partials in `partials` (2 * min(rows, MMFS_RMSNORM_BWD_PARTS) * cols floats of device scratch private to
+ * the call) summed in a fixed order: run-to-run reproducible.  partials may be NULL when dweight and dbias are.  bf16 /
+ * f16, cols % 8 == 0, cols <= 8192, 16-byte aligned rows: MMFS_EUNSUPPORTED otherwise.
+ */
+int mmfs_layernorm_backward(const void *x, const void *weight, const void *dy, void *dx, void *dweight, void *dbias,
+                            float *partials, long rows, int cols, float eps, int dtype, void *stream);
+
+/*
  * Gradient of mmfs_rmsnorm (training path): dx (rows, cols) from x, weight and dy, fp32 math; the forward's rounding
  * of x * rsqrt(mean(x^2) + eps) to the element type is treated as the identity.  With dweight != NULL also
  * dweight (cols) = sum over rows of dy * cast(x * rsqrt(.)), from per-CTA fp32 partials in `partials`

@@ -51,7 +51,9 @@ SIGNATURES = {
     "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
     "mmfs_attn_forward_lse": (_I, [_P] * 6 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
     "mmfs_attn_backward": (_I, [_P] * 11 + [_I] * 4 + [_L] * 16 + [_F, _I, _P]),
+    "mmfs_attn_backward_general": (_I, [_P] * 11 + [_I] * 5 + [_L] * 16 + [_F, _I, _I, _P]),
     "mmfs_rmsnorm_backward": (_I, [_P] * 6 + [_L, _I, _F, _I, _P]),
+    "mmfs_layernorm_backward": (_I, [_P] * 7 + [_L, _I, _F, _I, _P]),
     "mmfs_swiglu_backward": (_I, [_P] * 3 + [_L, _I, _I, _P]),
     "mmfs_decode_select": (_I, [_P, _L] + [_P] * 5 + [_I, _L, _I] + [_P] * 3 + [_I] * 4 + [_P]),
     "mmfs_beam_select": (_I, [_P, _L] + [_P] * 11 + [_I, _L, _I, _P] + [_I] * 4 + [_P]),

@@ -1,4 +1,5 @@
-"""Autograd Functions over the decoder-layer kernels: the training path of the Llama decoder's self-attention layer.
+"""Autograd Functions over the decoder-layer kernels: the training path of the Llama decoder's self-attention layer
+and of the visual tokenizer's Q-Former head.
 
 Each forward runs the same sm_90a kernel as the inference wrapper in ops.py (a Function's forward runs with grad
 disabled, so the wrappers' ``inference_only`` guard does not fire there) and saves what its backward kernel reads:
@@ -9,10 +10,15 @@ disabled, so the wrappers' ``inference_only`` guard does not fire there) and sav
 * ``AttentionFunction`` -- causal ``mmfs_attn_forward_lse`` on that QKV buffer, saving O and the row log-sum-exp;
   ``mmfs_attn_backward`` writes dQ / dK / dV into one (B, T, 3, H, hd) gradient, so the QKV projection's backward
   stays one GEMM;
-* ``SwiGLUFunction``    -- ``mmfs_swiglu`` / ``mmfs_swiglu_backward`` on the [gate | up] buffer.
+* ``SwiGLUFunction``    -- ``mmfs_swiglu`` / ``mmfs_swiglu_backward`` on the [gate | up] buffer;
+* ``LayerNormFunction`` -- ``mmfs_layernorm`` / ``mmfs_layernorm_backward`` (dweight / dbias only when asked for);
+* ``GeneralAttentionFunction`` -- non-causal ``mmfs_attn_forward_lse`` on separate q (B, Tq, H, hd) and k / v
+  (B, Tkv, H, hd) with an optional (B, Tkv) key mask (the Q-Former's self- and cross-attention);
+  ``mmfs_attn_backward_general`` returns dq, dk, dv.
 
-The backward kernels take bf16 / fp16 only, and the attention backward head dim 128 without a KV cache; other inputs
-are refused with the library's message.  Double backward is not supported.
+The backward kernels take bf16 / fp16 only, the causal attention backward head dim 128 without a KV cache and the
+general one head dim 64 or 128; other inputs are refused with the library's message.  Double backward is not
+supported.
 """
 from __future__ import annotations
 
@@ -93,6 +99,46 @@ class SwiGLUFunction(Function):
         return ops.swiglu_backward(gate_up, d_out.contiguous())
 
 
+class LayerNormFunction(Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, eps):
+        x = x.contiguous()
+        ctx.eps = eps
+        ctx.save_for_backward(x, weight)
+        return ops.layernorm(x, weight, bias, eps)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, weight = ctx.saved_tensors
+        dx, dw, db = ops.layernorm_backward(x, weight, dy.contiguous(), ctx.eps, weight_grad=ctx.needs_input_grad[1],
+                                            bias_grad=ctx.needs_input_grad[2])
+        return dx, dw, db, None
+
+
+class GeneralAttentionFunction(Function):
+    @staticmethod
+    def forward(ctx, q, k, v, key_mask, scale):
+        """Non-causal attention of q (B, Tq, H, hd) over k / v (B, Tkv, H, hd) (dense heads, any batch / token strides);
+        ``key_mask`` (B, Tkv) (1 = attend) or None.  Returns (B, Tq, H * hd)."""
+        B, Tq, H, hd = q.shape
+        out, lse = ops.attention_forward_lse(q, k, v, key_mask=key_mask, scale=scale, causal=False)
+        ctx.scale = scale
+        ctx.save_for_backward(q, k, v, out, lse, key_mask)
+        return out.view(B, Tq, H * hd)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_out):
+        q, k, v, out, lse, key_mask = ctx.saved_tensors
+        d_out = d_out.contiguous().view(out.shape)
+        dq = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+        dk = torch.empty(k.shape, dtype=k.dtype, device=k.device)
+        dv = torch.empty(v.shape, dtype=v.dtype, device=v.device)
+        ops.attention_backward_general(q, k, v, out, d_out, lse, dq, dk, dv, key_mask=key_mask, scale=ctx.scale)
+        return dq, dk, dv, None, None
+
+
 def rmsnorm(x, weight, eps):
     return RMSNormFunction.apply(x, weight, eps)
 
@@ -107,3 +153,11 @@ def attention(qkv, key_mask=None, scale=None):
 
 def swiglu(gate_up):
     return SwiGLUFunction.apply(gate_up)
+
+
+def layernorm(x, weight, bias, eps):
+    return LayerNormFunction.apply(x, weight, bias, eps)
+
+
+def attention_general(q, k, v, key_mask=None, scale=None):
+    return GeneralAttentionFunction.apply(q, k, v, key_mask, float(scale if scale is not None else q.shape[-1] ** -0.5))

@@ -4,7 +4,8 @@
 //   mmfs_rope_qk      apply_rotary_pos_emb / rotate_half decoders/modeling_llama_mmfs.py:158-172
 //   mmfs_swiglu       LlamaMLP: act_fn(gate) * up        decoders/modeling_llama_mmfs.py:188-189
 //   mmfs_layernorm    nn.LayerNorm (CLIP / Q-Former / MMFSBlock norms)
-//   mmfs_rmsnorm_backward, mmfs_swiglu_backward   their gradients (training path, 16-bit tensors, fp32 math)
+//   mmfs_rmsnorm_backward, mmfs_swiglu_backward, mmfs_layernorm_backward
+//                     their gradients (training path, 16-bit tensors, fp32 math)
 //
 // Each mimics the rounding points of the reference's tensor pipeline in the storage type T (a
 // tensor op in bf16 rounds its result to bf16), so a bf16 run tracks the reference's bf16 run and
@@ -486,6 +487,94 @@ __global__ void __launch_bounds__(256) rmsnorm_dw_reduce_kernel(const float *__r
     dw[c] = from_op<T>(s);
 }
 
+// ---- LayerNorm backward: xhat = (x - mean) r, g = dy * w; dx = r * (g - mean(g) - xhat * mean(g * xhat));
+// dweight = sum over rows of dy * xhat, dbias = sum over rows of dy.  The statistics are recomputed from x in fp32 (the
+// forward rounds only its output).  Same part scheme as the RMSNorm backward: CTA p takes rows p, p + parts, ... and keeps
+// its dweight / dbias partials in shared memory; layernorm_dwdb_reduce_kernel sums them per column in part order.  The
+// CTA is as wide as a row's 16-byte vectors (32 .. 256 threads), so that the 64-wide qk-norm rows do not idle 7 warps.
+template <typename T>
+__global__ void __launch_bounds__(256) layernorm_bwd_kernel(const T *__restrict__ x, const T *__restrict__ w,
+                                                            const T *__restrict__ dy, T *__restrict__ dx,
+                                                            float *__restrict__ partials, long rows, int cols, float eps) {
+    constexpr int VEC = 16 / (int)sizeof(T);
+    extern __shared__ float s_part[];                         // [dweight | dbias] x cols floats, only with partials
+    __shared__ float s_red[32];
+    const int nvec = cols / VEC;
+    float *s_dw = s_part, *s_db = s_part + cols;
+    if (partials)                                             // every thread owns the same columns for every row
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x)
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) s_dw[i * VEC + k] = s_db[i * VEC + k] = 0.f;
+    const float inv_n = 1.f / (float)cols;
+    for (long row = blockIdx.x; row < rows; row += gridDim.x) {
+        const T *xr = x + row * cols, *dyr = dy + row * cols;
+        float s = 0.f;
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+            float f[VEC];
+            Vec16<T>::unpack(ldg_nc_v4(xr + i * VEC), f);
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) s += f[k];
+        }
+        const float mean = block_sum(s, s_red) * inv_n;
+        float ss = 0.f, sg = 0.f, sgx = 0.f;
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+            float f[VEC], g[VEC], d[VEC];
+            Vec16<T>::unpack(ldg_nc_v4(xr + i * VEC), f);
+            Vec16<T>::unpack(ldg_nc_v4(w + i * VEC), g);
+            Vec16<T>::unpack(ldg_nc_v4(dyr + i * VEC), d);
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) {
+                const float c = f[k] - mean, gk = d[k] * g[k];
+                ss = fmaf(c, c, ss);
+                sg += gk;
+                sgx = fmaf(gk, c, sgx);
+            }
+        }
+        ss = block_sum(ss, s_red);
+        sg = block_sum(sg, s_red);
+        sgx = block_sum(sgx, s_red);
+        const float r = rsqrtf(ss * inv_n + eps);               // the forward's statistic
+        const float mg = sg * inv_n, mgx = sgx * r * inv_n;     // mean(g), mean(g * xhat)
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+            float f[VEC], g[VEC], d[VEC], o[VEC];
+            Vec16<T>::unpack(ldg_nc_v4(xr + i * VEC), f);
+            Vec16<T>::unpack(ldg_nc_v4(w + i * VEC), g);
+            Vec16<T>::unpack(ldg_nc_v4(dyr + i * VEC), d);
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) {
+                const float xh = (f[k] - mean) * r;
+                o[k] = r * (fmaf(d[k], g[k], -mg) - xh * mgx);
+                if (partials) {
+                    s_dw[i * VEC + k] = fmaf(d[k], xh, s_dw[i * VEC + k]);
+                    s_db[i * VEC + k] += d[k];
+                }
+            }
+            stg_v4(dx + row * cols + i * VEC, Vec16<T>::pack(o));
+        }
+    }
+    if (partials)
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x)
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) {
+                partials[(long)blockIdx.x * cols + i * VEC + k] = s_dw[i * VEC + k];
+                partials[((long)gridDim.x + blockIdx.x) * cols + i * VEC + k] = s_db[i * VEC + k];
+            }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) layernorm_dwdb_reduce_kernel(const float *__restrict__ partials, T *__restrict__ dw,
+                                                                    T *__restrict__ db, int parts, int cols) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= cols) return;
+    float sw = 0.f, sb = 0.f;
+    for (int p = 0; p < parts; ++p) {
+        sw += partials[(long)p * cols + c];
+        sb += partials[((long)parts + p) * cols + c];
+    }
+    if (dw) dw[c] = from_op<T>(sw);
+    if (db) db[c] = from_op<T>(sb);
+}
+
 // ---- SwiGLU backward: out = silu(g) * u  ->  dg = d * u * s * (1 + g * (1 - s)), du = d * silu(g), s = sigmoid(g) ----
 template <typename T>
 __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const T *__restrict__ gu, const T *__restrict__ d_out,
@@ -518,6 +607,26 @@ static int launch_rmsnorm_bwd(const void *x, const void *w, const void *dy, void
     MMFS_CUDA(cudaGetLastError());
     if (dw) {
         rmsnorm_dw_reduce_kernel<T><<<(cols + 255) / 256, 256, 0, st>>>(partials, (T *)dw, parts, cols);
+        MMFS_CUDA(cudaGetLastError());
+    }
+    return MMFS_OK;
+}
+
+template <typename T>
+static int launch_layernorm_bwd(const void *x, const void *w, const void *dy, void *dx, void *dw, void *db, float *partials,
+                                long rows, int cols, float eps, cudaStream_t st) {
+    const int parts = (int)(rows < kRmsBwdParts ? rows : kRmsBwdParts);
+    const int nvec = cols / (16 / (int)sizeof(T));
+    const int threads = nvec >= 256 ? 256 : (nvec + 31) / 32 * 32;
+    const bool red = dw != nullptr || db != nullptr;
+    const size_t smem = red ? 2 * (size_t)cols * sizeof(float) : 0;
+    const int rc = ensure_dynamic_smem<layernorm_bwd_kernel<T>>(smem);
+    if (rc != MMFS_OK) return rc;
+    layernorm_bwd_kernel<T><<<parts, threads, smem, st>>>((const T *)x, (const T *)w, (const T *)dy, (T *)dx,
+                                                           red ? partials : nullptr, rows, cols, eps);
+    MMFS_CUDA(cudaGetLastError());
+    if (red) {
+        layernorm_dwdb_reduce_kernel<T><<<(cols + 255) / 256, 256, 0, st>>>(partials, (T *)dw, (T *)db, parts, cols);
         MMFS_CUDA(cudaGetLastError());
     }
     return MMFS_OK;
@@ -642,5 +751,22 @@ extern "C" int mmfs_swiglu_backward(const void *gate_up, const void *d_out, void
     }
     return dispatch_dtype<kF16Types, MMFS_EUNSUPPORTED>(dtype, "swiglu_backward", [&](auto tag) {
         return launch_swiglu_bwd<typename decltype(tag)::type>(gate_up, d_out, d_gate_up, rows, inter, (cudaStream_t)stream);
+    });
+}
+
+extern "C" int mmfs_layernorm_backward(const void *x, const void *weight, const void *dy, void *dx, void *dweight, void *dbias,
+                                       float *partials, long rows, int cols, float eps, int dtype, void *stream) {
+    MMFS_CHECK_ARG(rows >= 0 && cols > 0, "layernorm_backward: bad shape");
+    if (rows == 0) return MMFS_OK;
+    MMFS_CHECK_ARG(x && weight && dy && dx && (!(dweight || dbias) || partials), "layernorm_backward: null pointer argument");
+    if (!(dtype == MMFS_BF16 || dtype == MMFS_F16) || cols % 8 != 0 || cols > kRmsBwdMaxCols ||
+        ((uintptr_t)x | (uintptr_t)weight | (uintptr_t)dy | (uintptr_t)dx) % 16 != 0) {
+        set_error("layernorm_backward: needs bf16 / f16, cols %% 8 == 0, cols <= %d, 16-byte aligned rows (got cols=%d dtype=%d)",
+                  kRmsBwdMaxCols, cols, dtype);
+        return MMFS_EUNSUPPORTED;
+    }
+    return dispatch_dtype<kF16Types, MMFS_EUNSUPPORTED>(dtype, "layernorm_backward", [&](auto tag) {
+        return launch_layernorm_bwd<typename decltype(tag)::type>(x, weight, dy, dx, dweight, dbias, partials, rows, cols, eps,
+                                                                  (cudaStream_t)stream);
     });
 }

@@ -394,26 +394,30 @@ def _check_qkv_view(t, B, T, H, hd, what):
              f"{what}: tensors must be (B, T, H, hd) CUDA views with dense heads")
 
 
-def attention_forward_lse(q, k, v, key_mask=None, scale=None):
-    """Causal ``attention`` on the wgmma kernel that also returns the row log-sum-exp: ``(out (B,T,H,hd), lse (B,H,T)
-    fp32)``, natural log, +inf for a row that sees no key.  ``out`` is bit-identical to ``attention``'s (same kernel)."""
-    B, T, H, hd = q.shape
+def attention_forward_lse(q, k, v, key_mask=None, scale=None, causal=True):
+    """``attention`` on the wgmma kernel that also returns the row log-sum-exp: ``(out (B,Tq,H,hd), lse (B,H,Tq)
+    fp32)``, natural log, +inf for a row that sees no key.  ``out`` is bit-identical to ``attention``'s on the same
+    kernel.  q (B,Tq,H,hd), k / v (B,Tkv,H,hd); causal needs Tq = Tkv (query i sees keys j <= i)."""
+    B, Tq, H, hd = q.shape
+    Tkv = k.shape[1]
     inference_only("attention_forward_lse", q, k, v)
-    for t in (q, k, v):
-        _check_qkv_view(t, B, T, H, hd, "attention_forward_lse")
+    _check_qkv_view(q, B, Tq, H, hd, "attention_forward_lse")
+    for t in (k, v):
+        _check_qkv_view(t, B, Tkv, H, hd, "attention_forward_lse")
+    _require(not causal or Tq == Tkv, "attention_forward_lse: causal attention needs Tq == Tkv")
     scale = float(scale if scale is not None else hd ** -0.5)
-    out = torch.empty((B, T, H, hd), dtype=q.dtype, device=q.device)
-    lse = torch.empty((B, H, T), dtype=torch.float32, device=q.device)
+    out = torch.empty((B, Tq, H, hd), dtype=q.dtype, device=q.device)
+    lse = torch.empty((B, H, Tq), dtype=torch.float32, device=q.device)
     km = None
     if key_mask is not None:
         km = key_mask.to(torch.uint8).contiguous()
-        _require(tuple(km.shape) == (B, T), "attention_forward_lse: key_mask must be (B, T)")
+        _require(tuple(km.shape) == (B, Tkv), "attention_forward_lse: key_mask must be (B, Tkv)")
     counter = torch.empty((1,), dtype=torch.int32, device=q.device)
     with torch.cuda.device(q.device):
         rc = _lib.lib().mmfs_attn_forward_lse(
             q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), km.data_ptr() if km is not None else None,
-            B, H, T, T, hd, q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1),
-            out.stride(0), out.stride(1), scale, 1, 0, _DTYPE_CODE[q.dtype], counter.data_ptr(), _stream())
+            B, H, Tq, Tkv, hd, q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1),
+            out.stride(0), out.stride(1), scale, 1 if causal else 0, 0, _DTYPE_CODE[q.dtype], counter.data_ptr(), _stream())
     _lib.check(rc, "attention_forward_lse")
     launch_counter[0] += 1
     return out, lse
@@ -447,6 +451,37 @@ def attention_backward(q, k, v, out, d_out, lse, dq, dk, dv, key_mask=None, scal
     launch_counter[0] += 3
 
 
+def attention_backward_general(q, k, v, out, d_out, lse, dq, dk, dv, key_mask=None, scale=None, causal=False) -> None:
+    """dQ, dK, dV of ``attention_forward_lse`` for q / out / d_out / dq (B, Tq, H, hd) and k / v / dk / dv (B, Tkv, H, hd)
+    views, hd 64 or 128, bf16 / fp16, causal (Tq = Tkv) or not, ``key_mask`` (B, Tkv) or None.  Same kernels and
+    determinism as ``attention_backward``."""
+    B, Tq, H, hd = q.shape
+    Tkv = k.shape[1]
+    inference_only("attention_backward_general", q, k, v, out, d_out)
+    for t in (q, out, d_out, dq):
+        _check_qkv_view(t, B, Tq, H, hd, "attention_backward_general")
+    for t in (k, v, dk, dv):
+        _check_qkv_view(t, B, Tkv, H, hd, "attention_backward_general")
+    _require(all(t.dtype == q.dtype for t in (k, v, out, d_out, dq, dk, dv)), "attention_backward_general: dtype mismatch")
+    _require(lse.dtype == torch.float32 and tuple(lse.shape) == (B, H, Tq) and lse.is_contiguous(),
+             "attention_backward_general: lse must be contiguous fp32 (B, H, Tq)")
+    scale = float(scale if scale is not None else hd ** -0.5)
+    km = None
+    if key_mask is not None:
+        km = key_mask.to(torch.uint8).contiguous()
+        _require(tuple(km.shape) == (B, Tkv), "attention_backward_general: key_mask must be (B, Tkv)")
+    delta = torch.empty((B, H, Tq), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        rc = _lib.lib().mmfs_attn_backward_general(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), d_out.data_ptr(), lse.data_ptr(), dq.data_ptr(),
+            dk.data_ptr(), dv.data_ptr(), delta.data_ptr(), km.data_ptr() if km is not None else None, B, H, Tq, Tkv, hd,
+            q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1), out.stride(0), out.stride(1),
+            d_out.stride(0), d_out.stride(1), dq.stride(0), dq.stride(1), dk.stride(0), dk.stride(1), dv.stride(0),
+            dv.stride(1), scale, 1 if causal else 0, _DTYPE_CODE[q.dtype], _stream())
+    _lib.check(rc, "attention_backward_general")
+    launch_counter[0] += 3
+
+
 def rmsnorm_backward(x: torch.Tensor, weight: torch.Tensor, dy: torch.Tensor, eps: float, weight_grad: bool = True):
     """(dx, dweight) of ``rmsnorm`` over the last dim; dweight is None unless ``weight_grad``.  dweight is reduced from
     fixed per-CTA partials in a fixed order (run-to-run reproducible)."""
@@ -468,6 +503,34 @@ def rmsnorm_backward(x: torch.Tensor, weight: torch.Tensor, dy: torch.Tensor, ep
     _lib.check(rc, "rmsnorm_backward")
     launch_counter[0] += 2 if weight_grad else 1
     return dx, dw
+
+
+def layernorm_backward(x: torch.Tensor, weight: torch.Tensor, dy: torch.Tensor, eps: float, weight_grad: bool = True,
+                       bias_grad: bool = True):
+    """(dx, dweight, dbias) of ``layernorm`` over the last dim, statistics recomputed from x in fp32; dweight / dbias
+    are None unless asked for.  They are reduced from fixed per-CTA partials in a fixed order (run-to-run
+    reproducible)."""
+    inference_only("layernorm_backward", x, weight, dy)
+    _require(x.is_cuda and x.is_contiguous() and dy.is_contiguous() and weight.is_contiguous() and dy.shape == x.shape,
+             "layernorm_backward: contiguous CUDA tensors of one shape required")
+    _require(weight.dtype == x.dtype == dy.dtype and weight.numel() == x.shape[-1],
+             "layernorm_backward: weight dtype / size mismatch")
+    cols = x.shape[-1]
+    rows = x.numel() // cols
+    dx = torch.empty_like(x)
+    dw = torch.empty_like(weight) if weight_grad else None
+    db = torch.empty_like(weight) if bias_grad else None
+    partials = (torch.empty((2, min(rows, _lib.RMSNORM_BWD_PARTS), cols), dtype=torch.float32, device=x.device)
+                if weight_grad or bias_grad else None)
+    with torch.cuda.device(x.device):
+        rc = _lib.lib().mmfs_layernorm_backward(x.data_ptr(), weight.data_ptr(), dy.data_ptr(), dx.data_ptr(),
+                                                dw.data_ptr() if dw is not None else None,
+                                                db.data_ptr() if db is not None else None,
+                                                partials.data_ptr() if partials is not None else None, rows, cols,
+                                                float(eps), _DTYPE_CODE[x.dtype], _stream())
+    _lib.check(rc, "layernorm_backward")
+    launch_counter[0] += 2 if partials is not None else 1
+    return dx, dw, db
 
 
 def swiglu_backward(gate_up: torch.Tensor, d_out: torch.Tensor) -> torch.Tensor:

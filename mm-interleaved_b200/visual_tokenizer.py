@@ -26,13 +26,20 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from . import autograd_ops
 from . import msda as _msda
 from . import ops
 from ._cache import WeightCache
+from .llama_mmfs import check_training_dtype, records_grad
 from .sd_mmfs import resize_abs_pos, sincos_pos_embed_2d
 
 
 def _ln(mod: nn.LayerNorm, x):
+    """``mod(x)`` on the LayerNorm kernel; through its autograd Function when autograd records the call (the trainable
+    Q-Former head), otherwise on the inference path."""
+    if records_grad(mod, x):
+        check_training_dtype("LayerNorm", x)
+        return autograd_ops.layernorm(x, mod.weight, mod.bias, mod.eps)
     return ops.layernorm(x.contiguous(), mod.weight, mod.bias, mod.eps)
 
 
@@ -420,6 +427,9 @@ class QFormerAttention(nn.Module):
         if isinstance(self.q_norm, nn.LayerNorm):
             q, k = _ln(self.q_norm, q), _ln(self.k_norm, k)
         km = None if (encoder_attention_mask is None or encoder_hidden_states is None) else encoder_attention_mask.to(torch.uint8).contiguous()
+        if records_grad(self, hidden_states, kv):       # training: forward with LSE, general attention backward
+            check_training_dtype("QFormerAttention", hidden_states)
+            return autograd_ops.attention_general(q, k, v, key_mask=km)
         return ops.attention(q.contiguous(), k.contiguous(), v.contiguous(), key_mask=km, causal=False)   # scores / sqrt(hd), softmax, @ v
 
 
