@@ -177,7 +177,7 @@ class StaticKV:
         self.k = torch.empty((batch, max_len, heads, head_dim), dtype=dtype, device=device)
         self.v = torch.empty_like(self.k)
         self.length = 0
-        # CUDA-graph decode (mm_interleaved.py::_GraphedDecoder): a (1,) int64 DEVICE tensor holding the slot the
+        # CUDA-graph decode (the graphed decoders of generation.py): a (1,) int64 DEVICE tensor holding the slot the
         # next token is written to.  While set, a step appends at ``slot`` (index_copy_, no host integer involved),
         # attends over the WHOLE buffer under the caller's key mask, and ``length`` stays pinned at max_len - 1.
         self.slot = None

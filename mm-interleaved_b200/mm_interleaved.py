@@ -15,6 +15,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from . import generation
 from ._cache import WeightCache
 from .llama_mmfs import LlamaMMFSConfig, LlamaModel
 
@@ -386,264 +387,6 @@ class ImageDecoder(nn.Module):
         return out
 
 
-class _GraphedDecoder:
-    """Static state + one CUDA graph of a decode step for ``InterleavedForward`` (see ``enable_decode_graphs``).
-
-    Everything that changes from token to token lives in DEVICE tensors the graph updates itself -- the slot the new
-    key/value row goes to, the key mask over the whole static cache, the position ids, the step counter, the finished
-    flags, the output ids -- so generating N tokens is N ``graph.replay()`` calls with no host synchronisation.  The
-    image-side tensors of the cross-attention layers are a ``PreparedVision`` over static storage, refilled eagerly once
-    per call (a graph replay bypasses Python, so nothing inside the graph may depend on a tensor-identity cache).
-
-    ``mode``: None = plain greedy (processors + arg-max in torch ops); ``"greedy"`` (with a repetition penalty) and
-    ``"sample"`` (temperature + top-p) choose the token with ``ops.decode_select``, which reads the penalty,
-    temperature, top_p and seed from device buffers written once per call, so one graph serves any of their values.
-    ``"beam"``: beam search over B * num_beams rows (``generate_beams``); the step is ``ops.beam_select`` (scores,
-    hypotheses, done flags, history) -> ``ops.kv_beam_reorder`` (the generated positions of every layer's K and V, held
-    in one tensor ``kv``) -> the decoder on the next tokens, with the repetition and length penalties in a device
-    buffer.  ``finished`` then holds the per-sequence done flags.  ``"beam_sample"``: the same with ``ops.beam_sample``
-    (temperature and top_p in the device buffer too, one seed per call as ``"sample"``, a sticky error flag) and every
-    beam starting at score 0."""
-
-    def __init__(self, owner, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, mode=None,
-                 num_beams=1):
-        from . import ops
-        from .llama_mmfs import PreparedVision, StaticKV
-        self.owner, self.B, self.t_max, self.max_new, self.min_length = owner, B, t_max, max_new, int(min_length)
-        self.mode, self.pad_id, self.nb = mode, int(pad_id), int(num_beams)
-        R = B * self.nb                                                     # decoder rows: one per beam
-        model = owner.mm_decoder
-        n_img = feats_shape[1]
-        if mode in ("beam", "beam_sample"):
-            H = model.config.num_attention_heads
-            self.kv = torch.zeros((2 * len(model.layers), R, t_max, H, model.config.hidden_size // H), dtype=dtype,
-                                  device=device)
-            self.past = [StaticKV.over(self.kv[2 * i], self.kv[2 * i + 1]) for i in range(len(model.layers))]
-        else:
-            self.past = model.static_cache(B, t_max, dtype=dtype, device=device)
-        self.pv = PreparedVision((R,) + tuple(feats_shape[1:]))
-        probe = model.prepare_vision(torch.zeros(feats_shape, dtype=dtype, device=device))
-        for idx, val in probe.values.items():
-            self.pv.values[idx] = val.new_empty((R,) + tuple(val.shape[1:]))
-        V = owner.text_decoder.head.weight.shape[0]
-        self.logits = torch.zeros((R, V), dtype=torch.float32, device=device)
-        self.key_mask = torch.zeros((R, t_max), dtype=torch.uint8, device=device)
-        self.pos = torch.zeros((R, 1), dtype=torch.long, device=device)
-        self.cur = torch.zeros((1,), dtype=torch.long, device=device)
-        self.step = torch.zeros((1,), dtype=torch.long, device=device)
-        self.finished = torch.zeros((B,), dtype=torch.bool, device=device)
-        self.out_ids = torch.zeros((B, max_new), dtype=torch.long, device=device)
-        self.cross_last = torch.zeros((R, 1, n_img), dtype=torch.float32, device=device)
-        self.eos = torch.tensor(eos_ids, dtype=torch.long, device=device) if eos_ids else None
-        self.pad = torch.tensor(int(pad_id), dtype=torch.long, device=device)
-        self.neg_inf = torch.tensor(float("-inf"), dtype=torch.float32, device=device)
-        self.zero = torch.zeros((), dtype=torch.float32, device=device)
-        if mode is not None:
-            self.next_ids = torch.zeros((R, 1), dtype=torch.long, device=device)
-        if mode in ("greedy", "sample"):
-            self.params = torch.ones((3,), dtype=torch.float32, device=device)   # penalty, temperature, top_p
-            self.seed = torch.zeros((1,), dtype=torch.long, device=device)
-        if mode in ("beam", "beam_sample"):
-            nb = self.nb
-            # repetition_penalty, length_penalty (+ temperature, top_p when sampling)
-            self.params = torch.ones((2 if mode == "beam" else 4,), dtype=torch.float64, device=device)
-            self.beam_scores = torch.zeros((R,), dtype=torch.float32, device=device)
-            self.history = torch.zeros((R, max_new), dtype=torch.long, device=device)
-            self.parent = torch.zeros((R,), dtype=torch.long, device=device)
-            self.hyp_scores = torch.zeros((B, nb), dtype=torch.float64, device=device)
-            self.hyp_ids = torch.zeros((B, nb, max_new), dtype=torch.long, device=device)
-            self.hyp_meta = torch.zeros((B, nb, 2), dtype=torch.long, device=device)          # length (-1: free), serial
-            n_scratch = R * ops.beam_candidates(nb, len(eos_ids)) if mode == "beam" else ops.beam_sample_scratch(nb, R)
-            self.scratch = torch.zeros((n_scratch,), dtype=torch.long, device=device)
-            self.all_done = torch.zeros((1,), dtype=torch.bool).pin_memory()                 # written by every replay
-        if mode == "beam_sample":
-            self.seed = torch.zeros((1,), dtype=torch.long, device=device)
-            self.error = torch.zeros((1,), dtype=torch.int32, device=device)
-        self.graph = None
-        self.launches = 0
-        self.replays = 0
-
-    def _set_graph_mode(self, on: bool, length: int = 0):
-        for c in self.past:
-            c.slot = self.cur if on else None
-            c.length = self.t_max - 1 if on else length
-
-    def _step(self):
-        """One token: processors + arg-max / draw on the pending logits, bookkeeping, decoder forward on the chosen token."""
-        from . import ops
-        o = self.owner
-        if self.mode is None:
-            scores = self.logits
-            if self.eos is not None and self.min_length > 0:               # HF MinLengthLogitsProcessor
-                bias = torch.where(self.step < self.min_length, self.neg_inf, self.zero)
-                scores = scores.index_add(1, self.eos, bias.expand(self.B, self.eos.numel()).contiguous())
-            nxt = scores.argmax(-1)
-            if self.eos is not None:
-                nxt = torch.where(self.finished, self.pad, nxt)
-                self.finished.logical_or_((nxt[:, None] == self.eos[None, :]).any(dim=1))
-            self.out_ids.index_copy_(1, self.step, nxt[:, None])
-            fed = nxt[:, None]
-        elif self.mode in ("beam", "beam_sample"):                         # scorer, then the cache follows the parents
-            if self.mode == "beam":
-                ops.beam_select(self.logits, self.step, self.params, self.beam_scores, self.history, self.next_ids,
-                                self.parent, self.finished, self.hyp_scores, self.hyp_ids, self.hyp_meta, self.scratch,
-                                self.nb, eos=self.eos, pad_id=self.pad_id, min_length=self.min_length)
-            else:
-                ops.beam_sample(self.logits, self.step, self.params, self.beam_scores, self.history, self.next_ids,
-                                self.parent, self.finished, self.hyp_scores, self.hyp_ids, self.hyp_meta, self.error,
-                                self.scratch, self.nb, eos=self.eos, pad_id=self.pad_id, min_length=self.min_length,
-                                top_k=_BEAM_SAMPLE_TOP_K, seed=self.seed)
-            ops.kv_beam_reorder(self.kv, self.parent, self.cur, self.step, self.nb, self.max_new, done=self.finished)
-            fed = self.next_ids
-        else:                                                              # processors, choice and bookkeeping: one kernel
-            ops.decode_select(self.logits, self.out_ids, self.step, self.finished, self.next_ids, self.params, eos=self.eos,
-                              pad_id=self.pad_id, min_length=self.min_length, sample=self.mode == "sample", seed=self.seed)
-            fed = self.next_ids
-        self.key_mask.index_fill_(1, self.cur, 1)                          # the fed token's cache slot becomes visible
-        self.pos.add_(1)
-        hid = o.mm_decoder(inputs_embeds=o.mm_decoder.embed_tokens(fed), attention_mask=self.key_mask,
-                           position_ids=self.pos, past_key_values=self.past, vision_hidden_states=self.pv,
-                           cross_attention_mask=self.cross_last, use_cache=True, return_dict=True).last_hidden_state
-        self.logits.copy_(o.text_decoder.logits(hid)[:, -1].float())
-        self.step.add_(1)
-        self.cur.add_(1)
-        if self.mode in ("beam", "beam_sample"):                           # read by the host two replays later
-            self.all_done.copy_(self.finished.all().view(1), non_blocking=True)
-
-    def _reset(self, L, attention_mask, position_ids, cross, logits0):
-        self.key_mask.zero_()
-        self.key_mask[:, :L].copy_(attention_mask.to(torch.uint8))
-        self.pos.copy_(position_ids[:, -1:])
-        self.cur.fill_(L)
-        self.step.zero_()
-        self.finished.zero_()
-        self.out_ids.fill_(int(self.pad))
-        self.cross_last.copy_(cross[:, -1:, :])
-        self.logits.copy_(logits0)
-        if self.mode == "beam":
-            self.beam_scores.fill_(-1e9)
-            self.beam_scores[::self.nb] = 0.0                              # only the first beam of a sequence is live
-        if self.mode == "beam_sample":
-            self.beam_scores.zero_()                                       # beam_sample starts every beam at 0
-            self.error.zero_()
-        if self.mode in ("beam", "beam_sample"):
-            self.history.fill_(self.pad_id)
-            self.hyp_scores.zero_()
-            self.hyp_meta.fill_(-1)
-
-    def _prefill_done(self, L, reset):
-        """After the prefill: zero the unused cache slots, capture the step graph once, reset the per-call state."""
-        from . import ops
-        o = self.owner
-        for c in self.past:                                                 # masked slots must hold finite numbers
-            c.k[:, L:].zero_()
-            c.v[:, L:].zero_()
-        self._set_graph_mode(True)
-        if self.graph is None:
-            reset()
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                for _ in range(2):                                          # lazy handles, weight-derived caches, RoPE tables
-                    reset()                                                 # every warm-up step is step 0
-                    self._step()
-            torch.cuda.current_stream().wait_stream(side)
-            reset()
-            before = ops.launch_counter[0]
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self._step()
-            self.launches = ops.launch_counter[0] - before
-            # the graph reads the RoPE tables by address: keep the captured storage alive even if an eager decode grows
-            # (and so replaces) the shared tables later
-            self._captured_rope = [l.self_attn._rope for l in o.mm_decoder.layers]
-            for c in self.past:                                             # the warm-up steps wrote slots L, L+1
-                c.k[:, L:].zero_()
-                c.v[:, L:].zero_()
-        reset()
-
-    def generate(self, mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty=1.0, temperature=1.0,
-                 top_p=1.0, generator=None):
-        from . import ops
-        o = self.owner
-        B, L, _ = mm_embeds.shape
-        if L + self.max_new > self.t_max:
-            raise RuntimeError("prompt + new tokens exceed the captured cache length")
-        if self.mode is not None:                                           # per-call values the graph reads on the device
-            self.params[0].fill_(float(repetition_penalty))
-            self.params[1].fill_(float(temperature))
-            self.params[2].fill_(float(top_p))
-            if self.mode == "sample":                                       # one seed per call, drawn on the device
-                self.seed.random_(generator=generator)
-        o.mm_decoder.prepare_vision(feats, out=self.pv)                     # eager, into the static buffers the graph reads
-        self._set_graph_mode(False, 0)
-        out = o.mm_decoder(inputs_embeds=mm_embeds, attention_mask=attention_mask, position_ids=position_ids,
-                           past_key_values=self.past, vision_hidden_states=self.pv, cross_attention_mask=cross,
-                           use_cache=True, return_dict=True)               # prefill straight into the static cache
-        logits0 = o.text_decoder.logits(out.last_hidden_state[:, -1:])[:, -1].float()
-        self._prefill_done(L, lambda: self._reset(L, attention_mask, position_ids, cross, logits0))
-        for _ in range(self.max_new):
-            self.graph.replay()
-        ops.launch_counter[0] += self.launches * self.max_new
-        self._set_graph_mode(False, L)
-        return self.out_ids.clone()
-
-    def generate_beams(self, mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty=1.0,
-                       length_penalty=1.0, temperature=1.0, top_p=1.0, generator=None):
-        """Beam search (``mode == "beam"`` or ``"beam_sample"``): the prompt is prefilled once per sequence and its
-        cache rows, the ``PreparedVision`` values, key mask, position ids and last cross-attention row are replicated
-        to the beams (beam sample: to the ``self.B // B`` independent searches of each prompt, then to their beams);
-        then one replay per step.  At most two replays are in flight: before enqueuing replay t the host waits for
-        replay t - 2 and reads the "all sequences done" flag it copied to pinned memory, so decoding stops at most two
-        steps after the eager loop would (done sequences are inert).  Returns the host copies of the final state."""
-        from . import ops
-        o = self.owner
-        B, L, _ = mm_embeds.shape
-        if L + self.max_new > self.t_max:
-            raise RuntimeError("prompt + new tokens exceed the captured cache length")
-        self.params[0].fill_(float(repetition_penalty))
-        self.params[1].fill_(float(length_penalty))
-        if self.mode == "beam_sample":
-            self.params[2].fill_(float(temperature))
-            self.params[3].fill_(float(top_p))
-            self.seed.random_(generator=generator)                          # one seed per call, drawn on the device
-        rep = torch.arange(B, device=mm_embeds.device).repeat_interleave(self.B // B * self.nb)   # beam row -> prompt
-        pv = o.mm_decoder.prepare_vision(feats)                             # the prefill's B rows, then one per beam
-        for idx, val in pv.values.items():
-            torch.index_select(val, 0, rep, out=self.pv.values[idx])
-        pre = o.mm_decoder.static_cache(B, L, dtype=mm_embeds.dtype, device=mm_embeds.device)
-        out = o.mm_decoder(inputs_embeds=mm_embeds, attention_mask=attention_mask, position_ids=position_ids,
-                           past_key_values=pre, vision_hidden_states=pv, cross_attention_mask=cross, use_cache=True,
-                           return_dict=True)
-        logits0 = o.text_decoder.logits(out.last_hidden_state[:, -1:])[:, -1].float().index_select(0, rep)
-        for dst, src in zip(self.past, pre):                                # a copy of the prompt rows, no recompute
-            dst.k[:, :L].copy_(src.k.index_select(0, rep))
-            dst.v[:, :L].copy_(src.v.index_select(0, rep))
-        del pre, pv
-        mask_r, pos_r, cross_r = (t.index_select(0, rep) for t in (attention_mask, position_ids, cross[:, -1:, :]))
-        self._prefill_done(L, lambda: self._reset(L, mask_r, pos_r, cross_r, logits0))
-        torch.cuda.current_stream().synchronize()                           # no copy into all_done is pending
-        self.all_done.zero_()
-        events = (torch.cuda.Event(), torch.cuda.Event())
-        n = 0
-        for t in range(self.max_new):
-            if t >= 2:
-                events[t % 2].synchronize()                                 # replay t - 2 has finished
-                if bool(self.all_done[0]):
-                    break
-            self.graph.replay()
-            events[t % 2].record()
-            n += 1
-        self.replays = n
-        ops.launch_counter[0] += self.launches * n
-        self._set_graph_mode(False, L)
-        out = dict(history=self.history[:, :n].cpu(), beam_scores=self.beam_scores.cpu(), done=self.finished.cpu(),
-                   hyp_scores=self.hyp_scores.cpu(), hyp_ids=self.hyp_ids.cpu(), hyp_meta=self.hyp_meta.cpu())
-        if self.mode == "beam_sample":
-            out["error"] = bool(self.error.item())
-        return out
-
-
 class InterleavedForward(nn.Module):
     """``mm_decoder`` + ``text_decoder`` + ``soi_token`` of ``MMInterleaved`` with the forward path of
     ``MMInterleaved.forward`` up to the text logits.  Image embeddings / multi-scale maps come from the visual
@@ -668,8 +411,8 @@ class InterleavedForward(nn.Module):
         """Greedy ``generate_texts`` then replays ONE captured CUDA graph per generated token (embedding -> 40 layers ->
         head -> logits processors -> arg-max -> state update, ~1000 kernels) instead of launching them from Python; the
         graph, its static KV cache and input buffers are kept per (batch, cache length, image count) and reused by
-        later calls (SURVEY.md 8 f3; causal_lm_cascade.py:171-204 is the loop it replaces).  Greedy decoding with a
-        ``repetition_penalty`` is graphed too (``ops.decode_select``), token-identical to the eager loop.
+        later calls (SURVEY.md 8 f3; causal_lm_cascade.py:171-204 is the loop it replaces).  The token choice, with or
+        without a ``repetition_penalty``, is one ``ops.decode_select`` launch, token-identical to the eager loop.
 
         ``sampling=True`` also graphs ``use_nucleus_sampling`` (temperature + top-p).  Its draws come from the kernel's
         counter-based generator (Philox4x32-10 keyed by a per-call seed taken from the caller's ``generator``, by
@@ -687,29 +430,6 @@ class InterleavedForward(nn.Module):
         self._decode_graphs = {} if enabled else None
         self._decode_graph_sampling = bool(enabled and sampling)
         return self
-
-    def _decode_graph(self, mm_embeds, feats, max_new_tokens, eos_ids, pad_id, min_length, mode, num_beams=1, expand=1):
-        """The ``_GraphedDecoder`` for this shape and these settings, built on first use (at most four are kept);
-        ``expand`` independent beam searches per prompt (beam sample's ``num_return_sequences``)."""
-        B, L, _ = mm_embeds.shape
-        B *= expand
-        t_max = ((L + max_new_tokens + 255) // 256) * 256                  # cache-length bucket: one graph serves nearby prompts
-        key = (B, t_max, tuple(feats.shape), mm_embeds.dtype, mm_embeds.device, tuple(eos_ids), int(pad_id), int(min_length),
-               int(max_new_tokens), int(num_beams), mode)
-        dec = self._decode_graphs.get(key)
-        if dec is None:
-            if len(self._decode_graphs) >= 4:
-                self._decode_graphs.pop(next(iter(self._decode_graphs)))
-            dec = self._decode_graphs[key] = _GraphedDecoder(self, B, t_max, feats.shape, mm_embeds.dtype, mm_embeds.device,
-                                                             eos_ids, pad_id, min_length, max_new_tokens, mode, num_beams)
-        return dec
-
-    @torch.no_grad()
-    def _graphed_decode(self, mm_embeds, cross, feats, attention_mask, position_ids, max_new_tokens, eos_ids, pad_id,
-                        min_length, mode, repetition_penalty, temperature, top_p, generator):
-        dec = self._decode_graph(mm_embeds, feats, max_new_tokens, eos_ids, pad_id, min_length, mode)
-        return dec.generate(mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty, temperature, top_p,
-                            generator)
 
     def prepare(self, text_ids, visual_output, num_image_per_seq, max_num_image: int):
         st = self.special_token_dict
@@ -769,294 +489,25 @@ class InterleavedForward(nn.Module):
         ``repetition_penalty`` (scores of already generated ids divided / multiplied), ``min_length`` (every eos id
         is suppressed while fewer than ``min_length`` tokens were generated), several ``eos_token_id`` values (the
         reference passes [eos, soi]), and ``use_nucleus_sampling`` = temperature + top-p sampling.  ``num_beams > 1``
-        runs HF-style beam search (``_beam_search`` below; the reference's captioning default is 5 beams) and returns
+        runs HF-style beam search (``generation.beam_search``; the reference's captioning default is 5 beams) and returns
         (B * num_return_sequences, <= max_new_tokens) padded ids; otherwise (B, max_new_tokens) ids.  ``num_beams > 1``
-        with ``use_nucleus_sampling`` is HF 4.31's beam sample (``_beam_sample``: temperature, top-k 50 and top-p on
+        with ``use_nucleus_sampling`` is HF 4.31's beam sample (the same loop: temperature, top-k 50 and top-p on
         the beam scores, 2 * num_beams candidates drawn per sequence, ``num_return_sequences`` independent searches
         per prompt); it raises ``ValueError`` where 4.31 does, when a step leaves fewer than num_beams non-eos
         candidates.
 
-        Under ``enable_decode_graphs()`` greedy decoding (with or without the penalty) replays one CUDA graph per token
-        with the eager loop's tokens; nucleus sampling is graphed only after ``enable_decode_graphs(True,
+        Under ``enable_decode_graphs()`` greedy decoding (with or without the penalty, vocabularies up to
+        ``ops.SELECT_MAX_V``) replays one CUDA graph per token with the eager loop's tokens; nucleus sampling is graphed only after ``enable_decode_graphs(True,
         sampling=True)``, and then draws from the kernel's Philox stream instead of ``torch.multinomial`` (same
         distribution, different tokens for a given ``generator`` seed).  Beam search replays one graph per step when
         its sizes are within ``ops.beam_select_supported`` (else it runs the eager loop), with the eager loop's tokens
         except where two candidates' scores lie within a few fp32 ulps (the kernel's log-softmax sums in another
         order than ``torch.log_softmax``).  Beam sample is graphed under ``enable_decode_graphs(True, sampling=True)``
         within ``ops.beam_sample_supported``, with Philox draws like graphed nucleus sampling."""
-        from . import ops
-        eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
-        if num_beams > 1:
-            beam_args = (text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, max_new_tokens,
-                         eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams, length_penalty,
-                         num_return_sequences)
-            V = self.text_decoder.head.weight.shape[0]
-            graphs = self._decode_graphs is not None and text_ids.is_cuda and max_new_tokens > 0
-            if use_nucleus_sampling:                                     # HF beam_sample
-                if graphs and self._decode_graph_sampling and ops.beam_sample_supported(num_beams, len(eos_ids), V):
-                    return self._graphed_beam_search(*beam_args, sampling=(temperature, top_p, generator))
-                return self._beam_sample(*beam_args, temperature=temperature, top_p=top_p, generator=generator)
-            if graphs and ops.beam_select_supported(num_beams, len(eos_ids), V):
-                return self._graphed_beam_search(*beam_args)
-            return self._beam_search(*beam_args)
-        B, L = text_ids.shape
-        if attention_mask is None:
-            attention_mask = torch.ones((B, L), dtype=torch.long, device=text_ids.device)
-        mm_embeds, cross, feats = self.prepare(text_ids, visual_output, num_image_per_seq, max_num_image)
-        position_ids = (attention_mask.long().cumsum(-1) - 1).masked_fill(attention_mask == 0, 1)   # causal_lm_cascade.py:181-183
-        graphed = (self._decode_graphs is not None and static_cache and text_ids.is_cuda and max_new_tokens > 0 and
-                   (not use_nucleus_sampling or self._decode_graph_sampling))
-        if graphed:
-            mode = "sample" if use_nucleus_sampling else ("greedy" if repetition_penalty != 1.0 else None)
-            return self._graphed_decode(mm_embeds, cross, feats, attention_mask, position_ids, max_new_tokens, eos_ids,
-                                        pad_token_id, min_length, mode, repetition_penalty, temperature, top_p, generator)
-        # the image-only half of the 10 cross-attention layers, once per call (PreparedVision)
-        feats = self.mm_decoder.prepare_vision(feats)
-        # pre-allocated per-layer caches appended in place (the reference's cat-per-token re-copies every layer's cache)
-        past = self.mm_decoder.static_cache(B, L + max_new_tokens, dtype=mm_embeds.dtype, device=mm_embeds.device) if static_cache else None
-        out = self.mm_decoder(inputs_embeds=mm_embeds, attention_mask=attention_mask, position_ids=position_ids,
-                              past_key_values=past, vision_hidden_states=feats, cross_attention_mask=cross, use_cache=True,
-                              return_dict=True)
-        past = out.past_key_values
-        logits = self.text_decoder.logits(out.last_hidden_state[:, -1:])
-        new_ids = []
-        finished = torch.zeros((B,), dtype=torch.bool, device=text_ids.device)
-        mask = attention_mask
-        last_cross = cross[:, -1:, :]
-        pos = position_ids[:, -1:]
-        for step_idx in range(max_new_tokens):
-            scores = logits[:, -1].float()
-            if repetition_penalty != 1.0 and new_ids:                    # HF RepetitionPenaltyLogitsProcessor
-                prev = torch.stack(new_ids, dim=1)
-                picked = scores.gather(1, prev)
-                scores = scores.scatter(1, prev, torch.where(picked < 0, picked * repetition_penalty, picked / repetition_penalty))
-            if step_idx < min_length and eos_ids:                        # HF MinLengthLogitsProcessor
-                scores[:, eos_ids] = float("-inf")
-            if use_nucleus_sampling:                                     # temperature, then top-p (HF warper order)
-                scores = scores / temperature
-                srt, idx = scores.sort(dim=-1, descending=False)
-                drop = srt.softmax(-1).cumsum(-1) <= (1.0 - top_p)
-                drop[:, -1] = False                                      # always keep the most likely token
-                scores = scores.masked_fill(drop.scatter(1, idx, drop), float("-inf"))
-                nxt = torch.multinomial(scores.softmax(-1), 1, generator=generator).squeeze(1)
-            else:
-                nxt = scores.argmax(-1)
-            if eos_ids:
-                nxt = torch.where(finished, torch.full_like(nxt, pad_token_id), nxt)
-                for e in eos_ids:
-                    finished = finished | (nxt == e)
-            new_ids.append(nxt)
-            mask = torch.cat([mask, torch.ones((B, 1), dtype=mask.dtype, device=mask.device)], dim=1)
-            pos = pos + 1
-            step = self.mm_decoder(inputs_embeds=self.mm_decoder.embed_tokens(nxt[:, None]), attention_mask=mask,
-                                   position_ids=pos, past_key_values=past, vision_hidden_states=feats,
-                                   cross_attention_mask=last_cross, use_cache=True, return_dict=True)
-            past = step.past_key_values
-            logits = self.text_decoder.logits(step.last_hidden_state)
-        return torch.stack(new_ids, dim=1)
-
-    @torch.no_grad()
-    def _beam_search(self, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, max_new_tokens,
-                     eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams, length_penalty, num_return,
-                     sampling=None):
-        """Beam search with the bookkeeping of HF ``GenerationMixin.beam_search`` + ``BeamSearchScorer`` (transformers
-        4.31, the version the reference pins; ``early_stopping=False``, one beam group): log-softmax scores, logits
-        processors on the log-probabilities, top ``max(2, 1 + n_eos) * num_beams`` candidates per sequence (the
-        reference's own beam search, beam_search_monkey_patch.py:265-269: enough that ``num_beams`` of them are never
-        eos), finished hypotheses ranked by ``sum_logprobs / len(generated) ** length_penalty``, a sequence is done once
-        ``num_beams`` hypotheses are all at least as good as the best running beam could become.  The prompt is
-        prefilled ONCE per sequence and its cache rows are replicated per beam; every step re-gathers the cache rows by
-        beam index (``_reorder_cache``).
-
-        ``sampling = (temperature, top_p, generator)`` runs 4.31's ``beam_sample`` instead (``_beam_sample_candidates``
-        chooses the candidates): every beam starts at score 0, each sequence is expanded to ``num_return`` independent
-        beam searches that return their best hypothesis, and a step with fewer than ``num_beams`` non-eos candidates
-        raises ``ValueError`` as 4.31 does."""
-        B0, L = text_ids.shape
-        nb, dev = num_beams, text_ids.device
-        expand = num_return if sampling is not None else 1
-        B = B0 * expand                                                            # independent beam searches
-        if attention_mask is None:
-            attention_mask = torch.ones((B0, L), dtype=torch.long, device=dev)
-        eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
-        mm_embeds, cross, feats = self.prepare(text_ids, visual_output, num_image_per_seq, max_num_image)
-        position_ids = (attention_mask.long().cumsum(-1) - 1).masked_fill(attention_mask == 0, 1)   # causal_lm_cascade.py:181-183
-        pre = self.mm_decoder.static_cache(B0, L, dtype=mm_embeds.dtype, device=dev)
-        out = self.mm_decoder(inputs_embeds=mm_embeds, attention_mask=attention_mask, position_ids=position_ids,
-                              past_key_values=pre, vision_hidden_states=feats, cross_attention_mask=cross, use_cache=True,
-                              return_dict=True)
-        rep = torch.arange(B0, device=dev).repeat_interleave(expand * nb)         # beam row -> prompt
-        past = self.mm_decoder.static_cache(B * nb, L + max_new_tokens, dtype=mm_embeds.dtype, device=dev)
-        for dst, src in zip(past, pre):
-            dst.k[:, :L].copy_(src.k.index_select(0, rep)); dst.v[:, :L].copy_(src.v.index_select(0, rep)); dst.length = L
-        del pre
-        logits = self.text_decoder.logits(out.last_hidden_state[:, -1:]).index_select(0, rep)
-        feats_b, last_cross = feats.index_select(0, rep), cross[:, -1:, :].index_select(0, rep)
-        mask, pos = attention_mask.index_select(0, rep), position_ids[:, -1:].index_select(0, rep)
-
-        beam_scores = torch.zeros((B, nb), dtype=torch.float32, device=dev)
-        if sampling is None:
-            beam_scores[:, 1:] = -1e9                                              # beam_sample starts every beam at 0
-        beam_scores = beam_scores.view(-1)
-        seqs = torch.zeros((B * nb, 0), dtype=torch.long, device=dev)              # generated ids per beam row
-        hyps = [_BeamHypotheses(nb, length_penalty) for _ in range(B)]
-        done = [False] * B
-        n_cand = max(2, 1 + len(eos_ids)) * nb
-
-        for step_idx in range(max_new_tokens):
-            scores = torch.log_softmax(logits[:, -1].float(), dim=-1)
-            if repetition_penalty != 1.0 and seqs.shape[1] > 0:
-                picked = scores.gather(1, seqs)
-                scores = scores.scatter(1, seqs, torch.where(picked < 0, picked * repetition_penalty, picked / repetition_penalty))
-            if step_idx < min_length and eos_ids:
-                scores[:, eos_ids] = float("-inf")
-            V = scores.shape[-1]
-            if sampling is None:
-                top_s, top_i = (scores + beam_scores[:, None]).view(B, nb * V).topk(n_cand, dim=1, largest=True, sorted=True)
-            else:
-                top_s, top_i = _beam_sample_candidates(scores, beam_scores, B, nb, *sampling)
-            top_s_h, top_i_h, seqs_h = top_s.tolist(), top_i.tolist(), seqs.tolist()   # one host round trip per step
-            cur_len = seqs.shape[1] + 1
-            nxt_scores = [[0.0] * nb for _ in range(B)]
-            nxt_tokens = [[pad_token_id] * nb for _ in range(B)]
-            nxt_rows = [[b * nb] * nb for b in range(B)]
-            for b in range(B):
-                if done[b]:
-                    continue
-                k = 0
-                for rank, (sc, idx) in enumerate(zip(top_s_h[b], top_i_h[b])):
-                    row, tok = b * nb + idx // V, idx % V
-                    if tok in eos_ids:
-                        if rank >= nb:
-                            continue
-                        hyps[b].add(seqs_h[row], sc)
-                    else:
-                        nxt_scores[b][k], nxt_tokens[b][k], nxt_rows[b][k] = sc, tok, row
-                        k += 1
-                    if k == nb:
-                        break
-                if k < nb and sampling is not None:
-                    raise ValueError(f"At most {nb} tokens in {[i % V for i in top_i_h[b]]} can be equal to "
-                                     f"`eos_token_id: {eos_ids}`. Make sure {[i % V for i in top_i_h[b]]} are corrected.")
-                if len(hyps[b].beams) >= nb and hyps[b].worst >= top_s_h[b][0] / (cur_len ** length_penalty):
-                    done[b] = True
-            beam_scores = torch.tensor(nxt_scores, dtype=torch.float32, device=dev).view(-1)
-            tok_t = torch.tensor(nxt_tokens, dtype=torch.long, device=dev).view(-1)
-            row_t = torch.tensor(nxt_rows, dtype=torch.long, device=dev).view(-1)
-            seqs = torch.cat([seqs.index_select(0, row_t), tok_t[:, None]], dim=1)
-            if all(done) or step_idx == max_new_tokens - 1:
-                break
-            for c in past:                                                        # _reorder_cache
-                n = c.length
-                c.k[:, :n].copy_(c.k.index_select(0, row_t)[:, :n]); c.v[:, :n].copy_(c.v.index_select(0, row_t)[:, :n])
-            mask = torch.cat([mask.index_select(0, row_t), torch.ones((B * nb, 1), dtype=mask.dtype, device=dev)], dim=1)
-            pos = pos.index_select(0, row_t) + 1
-            step = self.mm_decoder(inputs_embeds=self.mm_decoder.embed_tokens(tok_t[:, None]), attention_mask=mask, position_ids=pos,
-                                   past_key_values=past, vision_hidden_states=feats_b, cross_attention_mask=last_cross,
-                                   use_cache=True, return_dict=True)
-            logits = self.text_decoder.logits(step.last_hidden_state)
-        return _beam_finalize(hyps, done, seqs.tolist(), beam_scores.tolist(), num_return // expand, max_new_tokens,
-                              pad_token_id, eos_ids).to(dev)
-
-    def _beam_sample(self, *beam_args, temperature=1.0, top_p=1.0, generator=None):
-        """HF 4.31 ``beam_sample`` in torch ops: ``_beam_search``'s loop with ``_beam_sample_candidates``."""
-        return self._beam_search(*beam_args, sampling=(temperature, top_p, generator))
-
-    @torch.no_grad()
-    def _graphed_beam_search(self, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask,
-                             max_new_tokens, eos_token_id, pad_token_id, min_length, repetition_penalty, num_beams,
-                             length_penalty, num_return, sampling=None):
-        """``_beam_search`` on one CUDA graph replay per step (``_GraphedDecoder`` in ``"beam"`` mode, or in
-        ``"beam_sample"`` mode with ``sampling = (temperature, top_p, generator)``); same arguments, same finalize."""
-        B, L = text_ids.shape
-        nb = num_beams
-        expand = num_return if sampling is not None else 1
-        if attention_mask is None:
-            attention_mask = torch.ones((B, L), dtype=torch.long, device=text_ids.device)
-        eos_ids = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id])
-        mm_embeds, cross, feats = self.prepare(text_ids, visual_output, num_image_per_seq, max_num_image)
-        position_ids = (attention_mask.long().cumsum(-1) - 1).masked_fill(attention_mask == 0, 1)   # causal_lm_cascade.py:181-183
-        mode = "beam" if sampling is None else "beam_sample"
-        dec = self._decode_graph(mm_embeds, feats, max_new_tokens, eos_ids, pad_token_id, min_length, mode, nb, expand)
-        st = dec.generate_beams(mm_embeds, cross, feats, attention_mask, position_ids, repetition_penalty, length_penalty,
-                                *(sampling or ()))
-        if st.get("error"):
-            raise ValueError(f"At most {nb} tokens in the {2 * nb} sampled candidates of a sequence can be equal to "
-                             f"`eos_token_id: {eos_ids}`: a step drew more than {nb} eos candidates")
-        hyps = []
-        for b in range(B * expand):                                        # the slots in insertion order
-            meta, ids, sc = st["hyp_meta"][b].tolist(), st["hyp_ids"][b].tolist(), st["hyp_scores"][b].tolist()
-            slots = sorted((m[1], j) for j, m in enumerate(meta) if m[0] >= 0)
-            hyps.append(_BeamHypotheses(nb, length_penalty, [(sc[j], ids[j][:meta[j][0]]) for _, j in slots]))
-        done = [bool(d) for d in st["done"].tolist()]
-        return _beam_finalize(hyps, done, st["history"].tolist(), st["beam_scores"].tolist(), num_return // expand,
-                              max_new_tokens, pad_token_id, eos_ids).to(text_ids.device)
-
-
-_BEAM_SAMPLE_TOP_K = 50              # transformers 4.31 GenerationConfig.top_k, which the reference never overrides
-
-
-def _beam_sample_candidates(scores, beam_scores, B, nb, temperature, top_p, generator):
-    """Steps 3-5 of one 4.31 ``beam_sample`` step on the processed log-probabilities ``scores`` (B * nb, V): add the
-    beam scores, warp (temperature, top-k 50, top-p; ``min_tokens_to_keep = 2``), draw ``2 * nb`` candidates per
-    sequence with ``torch.multinomial`` (without replacement) and sort them by warped score.  Returns (scores, flat
-    indices), each (B, 2 * nb)."""
-    s = scores + beam_scores[:, None]
-    if temperature != 1.0:                                                  # TemperatureLogitsWarper
-        s = s / temperature
-    V = s.shape[-1]
-    k = min(max(_BEAM_SAMPLE_TOP_K, 2), V)                                  # TopKLogitsWarper
-    s = s.masked_fill(s < s.topk(k, dim=-1).values[:, -1:], float("-inf"))
-    if top_p < 1.0:                                                         # TopPLogitsWarper
-        srt, idx = s.sort(dim=-1, descending=False)
-        drop = srt.softmax(-1).cumsum(-1) <= (1.0 - top_p)
-        drop[:, -2:] = False
-        s = s.masked_fill(drop.scatter(1, idx, drop), float("-inf"))
-    s = s.view(B, nb * V)
-    pick = torch.multinomial(s.softmax(-1), 2 * nb, generator=generator)
-    picked, order = s.gather(1, pick).sort(dim=1, descending=True, stable=True)   # ties: in draw order
-    return picked, pick.gather(1, order)
-
-
-class _BeamHypotheses:
-    """The finished hypotheses of one sequence as HF's ``BeamHypotheses`` keeps them (``early_stopping=False``):
-    ``(score, ids)`` in insertion order, at most ``num_beams``; a full set drops its first lowest-scored entry."""
-
-    def __init__(self, num_beams, length_penalty, beams=()):
-        self.num_beams, self.length_penalty = num_beams, length_penalty
-        self.beams = list(beams)
-        self.worst = min((h[0] for h in self.beams), default=1e9)
-
-    def add(self, ids, sum_logprobs):
-        score = sum_logprobs / (max(len(ids), 1) ** self.length_penalty)
-        if len(self.beams) < self.num_beams or score > self.worst:
-            self.beams.append((score, ids))
-            if len(self.beams) > self.num_beams:
-                self.beams.remove(min(self.beams, key=lambda h: h[0]))
-            self.worst = min(h[0] for h in self.beams)
-
-
-def _beam_finalize(hyps, done, seqs, beam_scores, num_return, max_new_tokens, pad_token_id, eos_ids):
-    """End of beam search (eager and graphed): the running beams of unfinished sequences become hypotheses, the best
-    ``num_return`` per sequence are returned as (B * num_return, width) ids on the CPU, padded with ``pad_token_id``
-    after one ``eos_ids[0]``; width = min(longest + 1, max_new_tokens)."""
-    nb = len(seqs) // len(hyps)
-    for b, h in enumerate(hyps):
-        if not done[b]:
-            for j in range(nb):
-                h.add(seqs[b * nb + j], beam_scores[b * nb + j])
-    best = []
-    for h in hyps:
-        ranked = sorted(h.beams, key=lambda x: x[0])
-        for _ in range(num_return):
-            best.append(ranked.pop()[1])
-    width = min(max(len(x) for x in best) + 1, max_new_tokens)
-    out_ids = torch.full((len(best), width), pad_token_id, dtype=torch.long)
-    for i, x in enumerate(best):
-        out_ids[i, :len(x)] = torch.tensor(x, dtype=torch.long)
-        if len(x) < width and eos_ids:
-            out_ids[i, len(x)] = eos_ids[0]
-    return out_ids
+        return generation.generate_texts(self, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask,
+                                         max_new_tokens, eos_token_id, pad_token_id, static_cache, min_length,
+                                         repetition_penalty, use_nucleus_sampling, top_p, temperature, generator,
+                                         num_beams, length_penalty, num_return_sequences)
 
 
 def _llm_config_from(llm_config, llm_model_path, txt_vocab_size, image_embed_dim, cross_attention_frequency, spatial_shapes):

@@ -154,6 +154,9 @@ def decode_select(logits: torch.Tensor, out_ids: torch.Tensor, step: torch.Tenso
     launch_counter[0] += 1
 
 
+SELECT_MAX_V = 1 << 17   # the vocabulary limit of decode_select, beam_select and beam_sample (kMaxV: two V-bit maps)
+
+
 def beam_candidates(num_beams: int, n_eos: int) -> int:
     """Candidates per sequence of one beam step, the reference's ``max(2, 1 + n_eos) * num_beams``."""
     return max(2, 1 + n_eos) * num_beams
@@ -162,7 +165,7 @@ def beam_candidates(num_beams: int, n_eos: int) -> int:
 def beam_select_supported(num_beams: int, n_eos: int, V: int) -> bool:
     """Whether ``beam_select`` takes this shape (its limits: num_beams <= 8, n_eos <= 4, the candidates fit in V)."""
     return (1 <= num_beams <= _lib.BEAM_MAX_BEAMS and 0 <= n_eos <= _lib.BEAM_MAX_EOS
-            and beam_candidates(num_beams, n_eos) <= V <= 1 << 17)
+            and beam_candidates(num_beams, n_eos) <= V <= SELECT_MAX_V)
 
 
 def _check_beam_step(what, logits, step, params, n_params, beam_scores, history, next_ids, parent, done, hyp_scores,
@@ -233,7 +236,7 @@ def beam_select(logits: torch.Tensor, step: torch.Tensor, params: torch.Tensor, 
 def beam_sample_supported(num_beams: int, n_eos: int, V: int) -> bool:
     """Whether ``beam_sample`` takes this shape (its limits: num_beams <= 8, n_eos <= 4, 2 * num_beams <= V <= 2^17)."""
     return (1 <= num_beams <= _lib.BEAM_MAX_BEAMS and 0 <= n_eos <= _lib.BEAM_MAX_EOS
-            and 2 * num_beams <= V <= 1 << 17)
+            and 2 * num_beams <= V <= SELECT_MAX_V)
 
 
 def beam_sample_scratch(num_beams: int, rows: int) -> int:

@@ -1,6 +1,6 @@
 """GPU tests of beam sample (HF transformers 4.31 ``GenerationMixin.beam_sample``): ``ops.beam_sample``
 (csrc/beam_select_sm100.cu) with injected uniforms against a float64 restatement of the step that draws by the same
-Gumbel race, its tie handling and error flag, the statistics of its Philox draws, the eager ``_beam_sample`` against a
+Gumbel race, its tie handling and error flag, the statistics of its Philox draws, the eager beam-sample loop against a
 plain-Python 4.31 loop over the oracle decoder, and the graphed beam-sample decode."""
 import itertools
 
@@ -301,7 +301,7 @@ class _Race:
 
 @pytest.mark.parametrize("n_ret", [1, 2])
 def test_eager_beam_sample_matches_the_hf_algorithm_on_the_oracle_decoder(monkeypatch, n_ret):
-    """nb = 3, two eos ids, min_length, length_penalty != 1, T != 1: ``_beam_sample`` (prefill once, replicated and
+    """nb = 3, two eos ids, min_length, length_penalty != 1, T != 1: the eager beam sample (prefill once, replicated and
     re-gathered caches) against 4.31's beam_sample written out in plain Python over the oracle decoder, the draw
     replaced by the same deterministic race on both sides."""
     from tests.test_generate_gpu import _BeamHyps, _oracle_step_logits, _setup
@@ -397,13 +397,13 @@ def test_eos_dominated_model_raises_value_error_eager_and_graphed():
 
 
 class _Uncaptured:
-    """Stands in for a ``_GraphedDecoder``'s captured graph: each "replay" runs the step's kernels directly."""
+    """Stands in for a graphed decoder's captured graph: each "replay" runs the step's kernels directly."""
 
     def __init__(self, dec):
         self.replay = dec._step
 
 
-def test_graphed_beam_sample_is_seeded_reuses_one_graph_and_equals_uncaptured_steps():
+def test_graphed_beam_sample_is_seeded_reuses_one_graph_equals_uncaptured_steps_and_adds_two_launches():
     from tests.test_beam_select_gpu import _second_call
     from tests.test_generate_gpu import _setup
     cfg, dev, sd, ids, nimg, vis, vis_d = _setup()
@@ -434,7 +434,7 @@ def test_graphed_beam_sample_is_seeded_reuses_one_graph_and_equals_uncaptured_st
         dev.enable_decode_graphs(True, sampling=True)
         gen(args, 7)
         sample = next(iter(dev._decode_graphs.values()))
-        assert sample.launches == greedy.launches + 3                  # beam_sample (2 kernels) + kv_beam_reorder
+        assert sample.launches == greedy.launches + 2                  # beam_sample (2 kernels) + kv_beam_reorder - decode_select
     finally:
         dev.enable_decode_graphs(False)
 

@@ -1,5 +1,5 @@
 """GPU tests of ``ops.beam_select`` / ``ops.kv_beam_reorder`` (csrc/beam_select_sm100.cu) and of the graphed beam
-search built on them: the kernel against a restatement of one eager ``_beam_search`` step (``torch.log_softmax``,
+search built on them: the kernel against a restatement of one eager ``beam_search`` step (``torch.log_softmax``,
 ``torch.topk`` over ``max(2, 1 + n_eos) * num_beams`` candidates, ``_BeamHyps`` for the hypotheses), the in-place
 reorder against ``index_select``, and ``generate_texts(num_beams > 1)`` under ``enable_decode_graphs`` against the
 eager loop."""
@@ -26,7 +26,7 @@ class _State:
 
 
 def _restated_step(st, logits, step, eos, pad, min_length, penalty, lp):
-    """One iteration of InterleavedForward._beam_search's loop, written out again; returns (tokens, parents, margins)."""
+    """One iteration of the eager loop of generation.beam_search, written out again; returns (tokens, parents, margins)."""
     B, nb = st.B, st.nb
     scores = torch.log_softmax(logits.float(), dim=-1)
     if penalty != 1.0 and step > 0:
@@ -210,7 +210,7 @@ def test_graphed_beam_search_equals_eager_with_one_graph(nb):
         dev.enable_decode_graphs(False)
 
 
-def test_graphed_beam_search_stops_within_two_replays_and_adds_three_launches():
+def test_graphed_beam_search_stops_within_two_replays_and_adds_two_launches():
     from tests.test_generate_gpu import _setup
     cfg, dev, sd, ids, nimg, vis, vis_d = _setup()
     with torch.no_grad():
@@ -231,8 +231,8 @@ def test_graphed_beam_search_stops_within_two_replays_and_adds_three_launches():
         assert torch.equal(eager, graphed), (eager, graphed)
         assert eager_steps <= dec.replays <= eager_steps + 2, (dec.replays, eager_steps)
         dev.generate_texts(*args, max_new_tokens=n_new, eos_token_id=[5, 9])        # greedy graph of the same shape
-        greedy = [d for k, d in dev._decode_graphs.items() if k[-1] is None][0]
-        assert dec.launches == greedy.launches + 3                     # beam_select (2 kernels) + kv_beam_reorder
+        greedy = [d for k, d in dev._decode_graphs.items() if k[-1] == "greedy"][0]
+        assert dec.launches == greedy.launches + 2                     # beam_select (2 kernels) + kv_beam_reorder - decode_select
     finally:
         dev.enable_decode_graphs(False)
 

@@ -237,6 +237,37 @@ def test_graphed_sampling_is_seeded_reuses_one_graph_and_reaches_the_greedy_limi
         dev.enable_decode_graphs(False)
 
 
+def test_vocabulary_above_the_select_limit_decodes_greedily_in_the_eager_loop_under_graphs():
+    """``decode_select`` takes V <= ``ops.SELECT_MAX_V``: above it, greedy ``generate_texts`` under
+    ``enable_decode_graphs()`` keeps the eager loop (no graph is captured) instead of raising."""
+    import mm_interleaved_b200 as m
+    from mm_interleaved_b200 import ops
+    from mm_interleaved_b200.mm_interleaved import InterleavedForward
+    from tests.golden.make_golden import LLAMA_TINY, seeded_state_dict
+    V = ops.SELECT_MAX_V + 2
+    cfg = m.LlamaMMFSConfig(**dict(LLAMA_TINY, vocab_size=V))
+    model = InterleavedForward(cfg, special_tokens=dict(bos_token_id=1, image_token_id=V - 2, soi_token_id=V - 1),
+                               orig_vocab_size=V - 2)
+    model.load_state_dict(seeded_state_dict(model.state_dict(), seed=5))
+    dev = model.cuda().eval()
+    g = torch.Generator().manual_seed(3)
+    ids = torch.randint(3, 60, (2, 12), generator=g)
+    ids[:, 0] = 1
+    ids[:, 2] = V - 1                                                  # <soi> + 3 <image> tokens per sequence
+    ids[:, 3:6] = V - 2
+    vis = {"vis_embed": torch.randn((2, 3, cfg.hidden_size), generator=g).cuda(),
+           "multiscale_features": [torch.randn((2, cfg.image_embed_dim, s, s), generator=g).cuda() for s in (8, 4, 2)]}
+    args = (ids.cuda(), vis, torch.tensor([1, 1]).cuda(), 1)
+    eager = dev.generate_texts(*args, max_new_tokens=4, eos_token_id=None)
+    dev.enable_decode_graphs()
+    try:
+        graphed = dev.generate_texts(*args, max_new_tokens=4, eos_token_id=None)
+        assert len(dev._decode_graphs) == 0
+        assert torch.equal(graphed, eager)
+    finally:
+        dev.enable_decode_graphs(False)
+
+
 def test_release_inference_config_takes_the_graph_through_mm_interleaved_generate():
     from tests.test_mm_interleaved_gpu import DEV, _batch, _build
     model, _ = _build()

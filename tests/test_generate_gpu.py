@@ -255,4 +255,6 @@ def test_graphed_greedy_decode_matches_eager_across_calls_with_new_images():
     assert torch.equal(graph_a, eager_a), (graph_a, eager_a)
     assert torch.equal(graph_b, eager_b), (graph_b, eager_b)
     assert torch.equal(graph_a2, eager_a)
+    dev.generate_texts(ids.cuda(), vis_d, nimg.cuda(), 2, repetition_penalty=1.7, **kw)
+    assert len(dev._decode_graphs) == 1                                # plain and penalised greedy share one graph
     dev.enable_decode_graphs(False)

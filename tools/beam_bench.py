@@ -1,11 +1,12 @@
 """Beam-search timing of the Llama-13B MMFS decoder (random weights, bf16): 5 beams, eos [eos, soi], min_length 8,
-20 new tokens, eager ``_beam_search`` against the graphed beam step (``enable_decode_graphs``: ``ops.beam_select`` +
-``ops.kv_beam_reorder`` + the decoder in one graph replay), on two prompt shapes:
+20 new tokens, the eager beam loop (``generation.beam_search``) against the graphed beam step (``enable_decode_graphs``:
+``generation.BeamDecoder``, ``ops.beam_select`` + ``ops.kv_beam_reorder`` + the decoder in one graph replay), on two
+prompt shapes:
   caption: 1 image (64 image tokens) in an 80-token prompt, the reference's captioning setting, B in {1, 4};
   long:    the 2048-token 4-image prompt of tools/decode_bench.py, B in {1, 2}.  At B = 4 its 20 beam rows need a
            34 GB cache (38 GB graphed) next to the 26 GB of weights, their ~18 GB of fused copies and the prefill
            cache: more than an 80 GB card holds, in either loop.
-The same for beam sample (``use_nucleus_sampling=True``, top_p 0.9, temperature 1: eager ``_beam_sample`` against
+The same for beam sample (``use_nucleus_sampling=True``, top_p 0.9, temperature 1: the same eager loop with ``sample`` against
 the graphed ``ops.beam_sample`` step under ``enable_decode_graphs(True, sampling=True)``; their draws differ by design,
 so those ids are not compared).  With random weights eos is practically never chosen, so every step decodes.  ms per
 token = (time of a 20-token call - time of a 1-token call) / 19, each the best of 2 runs; the ids of the eager and

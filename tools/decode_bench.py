@@ -1,6 +1,7 @@
 """Decode timing of the Llama-13B MMFS decoder (random weights, bf16): prefill on B x 2048-token 4-image sequences,
-then N new tokens with (a) the eager loop over the pre-allocated in-place KV cache, (b) the CUDA-graphed decode step
-(InterleavedForward.enable_decode_graphs) and (c) the reference-style cat-per-token cache, greedy.
+then N new tokens with (a) the eager loop over the pre-allocated in-place KV cache (``generation.token_loop``), (b) the
+CUDA-graphed decode step (InterleavedForward.enable_decode_graphs: ``generation.TokenDecoder``, whose token choice is
+one ``ops.decode_select`` launch) and (c) the reference-style cat-per-token cache, greedy.
 Weight-read floor per token: 13.0 B parameters x 2 B / peak HBM GB/s (workloads.measured_peaks).
 
 Then the reference's release inference settings (mm_inference.yaml: top_p 0.9, temperature 1.0, repetition penalty
@@ -45,7 +46,7 @@ def card():
 
 
 def torch_chain(scores, prev, sample, gen):
-    """The eager loop's token choice (InterleavedForward.generate_texts) at the release settings."""
+    """The eager loop's token choice (generation.token_loop) at the release settings."""
     p, T, top_p = RELEASE["repetition_penalty"], RELEASE["temperature"], RELEASE["top_p"]
     picked = scores.gather(1, prev)
     scores = scores.scatter(1, prev, torch.where(picked < 0, picked * p, picked / p))
