@@ -9,9 +9,16 @@
 //
 // Thread mapping (both kernels): thread t owns the 16-byte channel vector t % (C/VEC) of every k-th pixel, so the
 // per-channel scale/shift (apply) and the partial sums (statistics) live in registers and consecutive threads
-// read consecutive 16-byte vectors of a pixel row (coalesced).  Statistics are fp32 sum / sum-of-squares, reduced
-// in a fixed order (no atomics: results are reproducible run to run); the bf16 pipeline's rounding points
-// (norm -> T, silu -> T) are kept so a bf16 run tracks diffusers' bf16 run.
+// read consecutive 16-byte vectors of a pixel row (coalesced).  Statistics are fp32 (count, mean, M2) -- M2 the sum of
+// squared deviations from the mean -- merged in a fixed order (no atomics: results are reproducible run to run); the
+// bf16 pipeline's rounding points (norm -> T, silu -> T) are kept so a bf16 run tracks diffusers' bf16 run.
+//
+// Why (count, mean, M2) and not sum / sum of squares: var = E[x^2] - mean^2 loses ~(mean/std)^2 ulps to cancellation,
+// and a group whose mean is large next to its spread (flat image regions, outlier channels) is common: with that
+// formula an fp32 group at mean/std = 16 came out 3e-4 off, at 4096 entirely wrong.  Each thread accumulates its pixels
+// shifted by its first value (a sample of the group, so the shifted sums stay small), and the partial statistics are
+// combined with Chan et al.'s pairwise update (GnMerge), whose error grows only linearly with mean/std -- the floor set
+// by rounding the mean itself to fp32.
 #include "common.cuh"
 
 namespace mmfs {
@@ -21,63 +28,111 @@ template <> __device__ __forceinline__ float gn_rnd<float>(float x) { return x; 
 
 constexpr int kGnMaxChunks = 64;     // pixel chunks per image: the partial-statistics scratch is (B, kGnMaxChunks, G, 2) floats
 
-// Pass 1: per (image, pixel chunk) partial sum / sum of squares of every group, written (not accumulated) to
-// partial[b][chunk][g][0..1].  All reductions run in a fixed order -- registers over a thread's pixels, shared memory
-// over the pixel lanes of a channel, then over the channels of a group -- so the result is bit-reproducible run to run
-// (the first version used shared + global float atomics, whose order is not).
+__device__ __forceinline__ float gn_warp_sum(float v) {   // butterfly: every lane ends with the same, fixed-order sum
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// Parts i = 0..k-1 with (n_i, mean_i, M2_i) are merged in one pass, shifted by the first part's mean m_0 (Chan, Golub
+// & LeVeque's pairwise update applied to k parts at once): with d_i = mean_i - m_0, S1 = sum n_i d_i, S2 = sum n_i d_i^2,
+// mean = m_0 + S1 / n and M2 = sum M2_i + (S2 - S1^2 / n).  The d_i are of the order of the group's spread, so nothing
+// cancels, and the loop has the shape of a plain sum: independent loads, one FMA chain per term, no division.
+struct GnMerge {
+    float m0 = 0.f, s1 = 0.f, s2 = 0.f, q = 0.f;
+    __device__ __forceinline__ void add(float n, float mean, float m2) {
+        const float d = mean - m0;
+        s1 = fmaf(n, d, s1);
+        s2 = fmaf(n * d, d, s2);
+        q += m2;
+    }
+    __device__ __forceinline__ void finish(float n, float &mean, float &m2) const {
+        const float d = s1 / n;
+        mean = m0 + d;
+        m2 = q + fmaxf(fmaf(-s1, d, s2), 0.f);
+    }
+};
+
+// Pass 1: per (image, pixel chunk) mean and M2 of every group, written (not accumulated) to partial[b][chunk][g][0..1];
+// the counts follow from (HW, ppb, C / G).  All merges run in a fixed order -- registers over a thread's pixels, shared
+// memory over the pixel lanes of a channel, then over the channels of a group -- so the result is bit-reproducible run
+// to run (the first version used shared + global float atomics, whose order is not).
 template <typename T>
 __global__ void __launch_bounds__(1024) gn_stats_kernel(const T *__restrict__ x, float *__restrict__ partial, int HW, int C,
                                                          int G, int ppb, int cvecs, int lanes) {
     constexpr int VEC = 16 / (int)sizeof(T);
-    extern __shared__ float s_dyn[];                     // [lanes][C][2] thread partials, then [C][2] channel sums in place of lane 0
+    extern __shared__ float s_dyn[];                     // [lanes][C][2] thread (mean, M2), then [C][2] channel stats in place of lane 0
     const int b = blockIdx.y, p0 = blockIdx.x * ppb, p1 = min(HW, p0 + ppb);
     const int cv = threadIdx.x % cvecs, pl = threadIdx.x / cvecs;
-    float s[VEC], ss[VEC];
+    const int np = p1 - p0;                              // pixels of this chunk; lane l takes pixels p0 + l, p0 + l + lanes, ...
+    auto lane_count = [&](int l) { return l < np ? (np - l + lanes - 1) / lanes : 0; };
+    float piv[VEC], s[VEC], ss[VEC];                     // sums of (x - piv) and (x - piv)^2, piv = the thread's first value
 #pragma unroll
-    for (int k = 0; k < VEC; ++k) s[k] = ss[k] = 0.f;
+    for (int k = 0; k < VEC; ++k) piv[k] = s[k] = ss[k] = 0.f;
     const T *base = x + ((size_t)b * HW) * C + (size_t)cv * VEC;
     if (pl < lanes) {
         int p = p0 + pl;
+        bool first = true;                               // the pivot is taken from the first batch (its own term is 0)
         for (; p + 3 * lanes < p1; p += 4 * lanes) {     // four independent 16-byte loads in flight
             uint4 v[4];
 #pragma unroll
             for (int u = 0; u < 4; ++u) v[u] = ldg_nc_v4(base + (size_t)(p + u * lanes) * C);
+            if (first) { Vec16<T>::unpack(v[0], piv); first = false; }
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
                 float f[VEC];
                 Vec16<T>::unpack(v[u], f);
 #pragma unroll
-                for (int k = 0; k < VEC; ++k) { s[k] += f[k]; ss[k] = fmaf(f[k], f[k], ss[k]); }
+                for (int k = 0; k < VEC; ++k) { const float d = f[k] - piv[k]; s[k] += d; ss[k] = fmaf(d, d, ss[k]); }
             }
         }
         for (; p < p1; p += lanes) {
             float f[VEC];
             Vec16<T>::unpack(ldg_nc_v4(base + (size_t)p * C), f);
+            if (first) {
 #pragma unroll
-            for (int k = 0; k < VEC; ++k) { s[k] += f[k]; ss[k] = fmaf(f[k], f[k], ss[k]); }
+                for (int k = 0; k < VEC; ++k) piv[k] = f[k];
+                first = false;
+            }
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) { const float d = f[k] - piv[k]; s[k] += d; ss[k] = fmaf(d, d, ss[k]); }
+        }
+        const int n = lane_count(pl);
+        const float inv = n > 0 ? 1.f / (float)n : 0.f;
+#pragma unroll
+        for (int k = 0; k < VEC; ++k) {                  // shifted sums -> (mean, M2) of the thread's pixels
+            const float ds = s[k] * inv;                 // mean - piv
+            ss[k] = fmaxf(fmaf(-s[k], ds, ss[k]), 0.f);  // sum (x - piv)^2 - n (mean - piv)^2
+            s[k] = piv[k] + ds;
         }
         float *mine = s_dyn + ((size_t)pl * C + (size_t)cv * VEC) * 2;
 #pragma unroll
         for (int k = 0; k < VEC; ++k) { mine[2 * k] = s[k]; mine[2 * k + 1] = ss[k]; }
     }
     __syncthreads();
-    if (pl == 0) {                                       // channel totals over the pixel lanes, lane order
+    if (pl == 0) {                                       // channel statistics over the pixel lanes, lane order
+        GnMerge m[VEC];
+#pragma unroll
+        for (int k = 0; k < VEC; ++k) { m[k].m0 = s[k]; m[k].q = ss[k]; }   // lane 0 = this thread: d_0 = 0
         for (int l = 1; l < lanes; ++l) {
             const float *o = s_dyn + ((size_t)l * C + (size_t)cv * VEC) * 2;
+            const float nl = (float)lane_count(l);
 #pragma unroll
-            for (int k = 0; k < VEC; ++k) { s[k] += o[2 * k]; ss[k] += o[2 * k + 1]; }
+            for (int k = 0; k < VEC; ++k) m[k].add(nl, o[2 * k], o[2 * k + 1]);
         }
-        float *mine = s_dyn + (size_t)cv * VEC * 2;
+        float *mine = s_dyn + (size_t)cv * VEC * 2;      // only this thread reads or writes these columns here
 #pragma unroll
-        for (int k = 0; k < VEC; ++k) { mine[2 * k] = s[k]; mine[2 * k + 1] = ss[k]; }
+        for (int k = 0; k < VEC; ++k) m[k].finish((float)np, mine[2 * k], mine[2 * k + 1]);
     }
     __syncthreads();
     const int cg = C / G;
-    for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) {   // group totals over the group's channels, channel order
-        const int g = i >> 1, which = i & 1;
-        float acc = 0.f;
-        for (int c = 0; c < cg; ++c) acc += s_dyn[(size_t)(g * cg + c) * 2 + which];
-        partial[(((size_t)b * kGnMaxChunks + blockIdx.x) * G + g) * 2 + which] = acc;
+    for (int g = threadIdx.x; g < G; g += blockDim.x) {  // group statistics over the group's channels (np pixels each), channel order
+        const float *cs = s_dyn + (size_t)g * cg * 2;
+        GnMerge m;
+        m.m0 = cs[0];
+        for (int c = 0; c < cg; ++c) m.add((float)np, cs[2 * c], cs[2 * c + 1]);
+        float *out = partial + (((size_t)b * kGnMaxChunks + blockIdx.x) * G + g) * 2;
+        m.finish((float)np * (float)cg, out[0], out[1]);
     }
 }
 
@@ -87,19 +142,38 @@ __global__ void __launch_bounds__(1024) gn_apply_kernel(const T *__restrict__ x,
                                                          T *__restrict__ y, int HW, int C, int G, int ppb, int cvecs, int lanes,
                                                          float eps, int silu, int chunks) {
     constexpr int VEC = 16 / (int)sizeof(T);
-    extern __shared__ float stats[];                     // [G][2] totals of this image (chunk order: reproducible)
+    extern __shared__ float stats[];                     // [G][2] mean, variance of this image (chunk order: reproducible)
     const int b = blockIdx.y, p0 = blockIdx.x * ppb, p1 = min(HW, p0 + ppb);
     const int cv = threadIdx.x % cvecs, pl = threadIdx.x / cvecs;
-    for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) {
-        float acc = 0.f;
-        for (int ch = 0; ch < chunks; ++ch) acc += partial[((size_t)b * kGnMaxChunks + ch) * 2 * G + i];
-        stats[i] = acc;
+    const int cg = C / G;
+    // a warp per group, lane l taking chunks l and l + 32 (blockDim.x is a multiple of 32): one batch of loads, then
+    // fixed-order butterfly sums, so every lane -- and every run -- gets the same result
+    static_assert(kGnMaxChunks <= 64, "two chunks per lane");
+    const int lane = threadIdx.x & 31;
+    auto count = [&](int ch) { return (float)(min(HW, (ch + 1) * ppb) - ch * ppb) * (float)cg; };
+    for (int g = threadIdx.x >> 5; g < G; g += blockDim.x >> 5) {
+        const float *pg = partial + ((size_t)b * kGnMaxChunks * G + g) * 2;   // chunk ch at pg[ch * 2G]
+        const int c0 = lane, c1 = lane + 32;
+        const float ma = c0 < chunks ? pg[(size_t)c0 * 2 * G] : 0.f, qa = c0 < chunks ? pg[(size_t)c0 * 2 * G + 1] : 0.f;
+        const float mb = c1 < chunks ? pg[(size_t)c1 * 2 * G] : 0.f, qb = c1 < chunks ? pg[(size_t)c1 * 2 * G + 1] : 0.f;
+        GnMerge m;
+        m.m0 = __shfl_sync(0xffffffffu, ma, 0);
+        if (c0 < chunks) m.add(count(c0), ma, qa);
+        if (c1 < chunks) m.add(count(c1), mb, qb);
+        m.s1 = gn_warp_sum(m.s1);
+        m.s2 = gn_warp_sum(m.s2);
+        m.q = gn_warp_sum(m.q);
+        if (lane == 0) {
+            const float n = (float)HW * (float)cg;
+            float mean, m2;
+            m.finish(n, mean, m2);
+            stats[2 * g] = mean;
+            stats[2 * g + 1] = m2 / n;
+        }
     }
     __syncthreads();
     if (pl >= lanes) return;
-    const int cg = C / G;
-    const float inv_n = 1.f / ((float)cg * (float)HW);
-    float sc[VEC], sh[VEC];
+    float sc[VEC], sh[VEC];                              // y = x * (r * gamma) + (beta - mean * r * gamma)
     {
         float gm[VEC], bt[VEC];
 #pragma unroll
@@ -109,11 +183,8 @@ __global__ void __launch_bounds__(1024) gn_apply_kernel(const T *__restrict__ x,
 #pragma unroll
         for (int k = 0; k < VEC; ++k) {
             const int g = (cv * VEC + k) / cg;
-            const float mean = stats[2 * g] * inv_n;
-            const float var = fmaxf(stats[2 * g + 1] * inv_n - mean * mean, 0.f);
-            const float r = rsqrtf(var + eps);
-            sc[k] = r * gm[k];
-            sh[k] = bt[k] - mean * sc[k];
+            sc[k] = rsqrtf(stats[2 * g + 1] + eps) * gm[k];
+            sh[k] = fmaf(-stats[2 * g], sc[k], bt[k]);
         }
     }
     const size_t off = ((size_t)b * HW) * C + (size_t)cv * VEC;
@@ -159,8 +230,9 @@ static int gn_launch(const void *x, const void *gamma, const void *beta, void *y
     if (rc != MMFS_OK) return rc;
     dim3 grid(chunks, B);
     kern<<<grid, threads, smem_stats, st>>>((const T *)x, stats, HW, C, G, ppb, cvecs, lanes);
-    gn_apply_kernel<T><<<grid, threads, 2 * G * sizeof(float), st>>>((const T *)x, (const T *)gamma, (const T *)beta, stats, (T *)y,
-                                                                    HW, C, G, ppb, cvecs, lanes, eps, silu, chunks);
+    // whole warps for the chunk merge; the padding threads (pl >= lanes) leave after it
+    gn_apply_kernel<T><<<grid, (threads + 31) / 32 * 32, 2 * G * sizeof(float), st>>>(
+        (const T *)x, (const T *)gamma, (const T *)beta, stats, (T *)y, HW, C, G, ppb, cvecs, lanes, eps, silu, chunks);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }

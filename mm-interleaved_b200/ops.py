@@ -41,9 +41,18 @@ def rmsnorm(x: torch.Tensor, weight: torch.Tensor, eps: float) -> torch.Tensor:
     return y
 
 
+def _check_affine(what: str, x: torch.Tensor, n: int, *params) -> None:
+    """Optional per-channel weight / bias: the kernels read them as n contiguous elements of x's dtype."""
+    for p in params:
+        if p is not None:
+            _require(p.dtype == x.dtype and p.numel() == n and p.is_contiguous() and p.device == x.device,
+                     f"{what}: weight / bias must be contiguous {x.dtype} tensors of {n} elements on {x.device}")
+
+
 def layernorm(x: torch.Tensor, weight, bias, eps: float) -> torch.Tensor:
     inference_only("layernorm", x, weight, bias)
     _require(x.is_cuda and x.is_contiguous(), "layernorm: contiguous CUDA tensor required")
+    _check_affine("layernorm", x, x.shape[-1], weight, bias)
     y = torch.empty_like(x)
     rows = x.numel() // x.shape[-1]
     with torch.cuda.device(x.device):
@@ -676,8 +685,10 @@ def group_norm_nhwc(x: torch.Tensor, groups: int, weight=None, bias=None, eps: f
     inference_only("group_norm_nhwc", x, weight, bias)
     _require(group_norm_supported(x), "group_norm_nhwc: need a CUDA channels_last f32/f16/bf16 tensor with C % (16/size) == 0")
     B, C, H, W = x.shape
+    _require(groups > 0 and C % groups == 0, f"group_norm_nhwc: {C} channels do not split into {groups} groups")
+    _check_affine("group_norm_nhwc", x, C, weight, bias)
     y = torch.empty_like(x, memory_format=torch.channels_last)
-    stats = torch.empty((B, 64, groups, 2), dtype=torch.float32, device=x.device)   # per-chunk partial sums
+    stats = torch.empty((B, 64, groups, 2), dtype=torch.float32, device=x.device)   # per-chunk (mean, M2) of each group
     with torch.cuda.device(x.device):
         rc = _lib.lib().mmfs_groupnorm_nhwc(x.data_ptr(), weight.data_ptr() if weight is not None else None,
                                             bias.data_ptr() if bias is not None else None, y.data_ptr(), stats.data_ptr(),
