@@ -316,6 +316,30 @@ int mmfs_swiglu_backward(const void *gate_up, const void *d_out, void *d_gate_up
                          void *stream);
 
 /*
+ * Gradient of CLIP's quick_gelu, y = h * sigmoid(1.702 h) (training path): dh = dy * (s + 1.702 h s (1 - s)) with
+ * s = sigmoid(1.702 h), over n elements of h, dy and dh, in fp32 with one rounding at the store.  16-byte vectors and a
+ * scalar tail, so any n >= 0.  n < 0, null pointers: MMFS_EINVAL.  A dtype other than bf16 / f16, pointers not 16-byte
+ * aligned: MMFS_EUNSUPPORTED.
+ */
+int mmfs_quick_gelu_backward(const void *h, const void *dy, void *dh, long n, int dtype, void *stream);
+
+/*
+ * Gradient of a bilinear resize with align_corners=False and a given scale factor (F.interpolate(x, scale_factor=f,
+ * mode="bilinear"), the ViT-Adapter's x4 / x2 / x0.5 output resizes), training path.  scale_h, scale_w = 1 / f per axis:
+ * output index o samples input r = max(scale * (o + 0.5) - 0.5, 0) along that axis, PyTorch's source-index rule with its
+ * edge clamps.  Gather form without atomics: every input pixel sums, in fp32 and in a fixed order (output rows, then
+ * columns, increasing), the weighted dy of the output pixels that sample it, and is rounded once: run-to-run
+ * reproducible.
+ *   dy (B, C, Hout, Wout): element (b, c, p), p = oy * Wout + ox, at dy[b * dy_bs + c * dy_cs + p * dy_ps] (NCHW: (C*Hout*Wout,
+ *   Hout*Wout, 1); token layout (B, Hout*Wout, C): (Hout*Wout*C, 1, C)); dx (B, Hin * Win, C) contiguous, fully overwritten
+ *   (token layout: the transpose back to (B, C, Hin, Win) is the caller's view).
+ * Negative B, non-positive C / sizes / scales, null pointers: MMFS_EINVAL.  A dtype other than bf16 / f16, C % 8 != 0, dx
+ * not 16-byte aligned: MMFS_EUNSUPPORTED.
+ */
+int mmfs_resize_bilinear_backward(const void *dy, void *dx, int B, int C, int Hin, int Win, int Hout, int Wout, long dy_bs,
+                                  long dy_cs, long dy_ps, float scale_h, float scale_w, int dtype, void *stream);
+
+/*
  * 2-D convolution as an implicit GEMM on the tensor cores (wgmma, TMA-shifted input boxes, no im2col buffer).
  * Replaces the cuDNN convolutions diffusers' UNet issues in the denoise step (called from
  * utils/monkey_patch/sd_unet_forward_monkey_patch.py:235-366; 3x3 stride 1/2 and 1x1, NHWC).

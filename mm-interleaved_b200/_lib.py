@@ -55,6 +55,8 @@ SIGNATURES = {
     "mmfs_rmsnorm_backward": (_I, [_P] * 6 + [_L, _I, _F, _I, _P]),
     "mmfs_layernorm_backward": (_I, [_P] * 7 + [_L, _I, _F, _I, _P]),
     "mmfs_swiglu_backward": (_I, [_P] * 3 + [_L, _I, _I, _P]),
+    "mmfs_quick_gelu_backward": (_I, [_P] * 3 + [_L, _I, _P]),
+    "mmfs_resize_bilinear_backward": (_I, [_P] * 2 + [_I] * 6 + [_L] * 3 + [_F, _F, _I, _P]),
     "mmfs_decode_select": (_I, [_P, _L] + [_P] * 5 + [_I, _L, _I] + [_P] * 3 + [_I] * 4 + [_P]),
     "mmfs_beam_select": (_I, [_P, _L] + [_P] * 11 + [_I, _L, _I, _P] + [_I] * 4 + [_P]),
     "mmfs_beam_sample": (_I, [_P, _L] + [_P] * 14 + [_I, _L, _I, _I, _P] + [_I] * 4 + [_P]),

@@ -649,13 +649,16 @@ class MMInterleaved(InterleavedForward):
         ``loss_img`` = its detached mean and ``loss = loss_txt * w_txt + loss_img * w_img``; ``multiscale_features``
         then leaves the output, as there.  ``generator`` (keyword) seeds the image loss's random draws.
         Under autograd the text loss is differentiable (``freeze_like_reference``), down to the visual tokenizer's head
-        (``pos_proj``, ``pos_ln``, ``post_ln``, the Q-Former, ``proj``); a trainable tokenizer encoder (CLIP ViT +
-        ViT-Adapter) or an image loss raises up front, as neither has a backward here."""
+        (``pos_proj``, ``pos_ln``, ``post_ln``, the Q-Former, ``proj``) and its ViT-Adapter, through the frozen CLIP ViT
+        (``visual_tokenizer.freeze_like_reference()``); a trainable CLIP ViT weight or an image loss raises up front, as
+        neither has a backward here."""
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            if any(p.requires_grad for p in self.visual_tokenizer.encoder.parameters()):
+            if any(p.requires_grad for n, p in self.visual_tokenizer.encoder.vision_model.named_parameters()
+                   if not n.startswith("adapter")):
                 raise RuntimeError("MMInterleaved.forward under autograd: the visual tokenizer has no backward here "
-                                   "through its CLIP ViT and ViT-Adapter; freeze them "
-                                   "(model.visual_tokenizer.encoder.requires_grad_(False)) or run under torch.no_grad()")
+                                   "for its CLIP ViT weights (the reference freezes them, and trains the ViT-Adapter); "
+                                   "call model.visual_tokenizer.freeze_like_reference(), or freeze the whole encoder "
+                                   "(model.visual_tokenizer.encoder.requires_grad_(False)), or run under torch.no_grad()")
             if self._has_image_loss():
                 raise RuntimeError("MMInterleaved.forward under autograd: the image-decoder loss has no backward here; "
                                    "build the image decoder's VAE without an encoder (no image loss) or run under "
@@ -695,12 +698,13 @@ class MMInterleaved(InterleavedForward):
         decoder_text.py:50-51): the LLM frozen except its ``llama_cross_attn`` blocks, the text head frozen except
         ``head_new``, ``soi_token`` trainable.  Returns ``self``.
 
-        The reference also trains the visual tokenizer's adapter and Q-Former head and the image decoder.  This leaves
-        the tokenizer's flags as they are.  Its head (``pos_proj``, ``pos_ln``, ``post_ln``, the Q-Former, ``proj``) has
-        a backward here, its encoder (CLIP ViT + ViT-Adapter) does not: ``forward`` under autograd raises while an
-        encoder parameter requires grad or the image loss is on.  To train the text loss with the head trainable, freeze
-        the encoder (``model.visual_tokenizer.encoder.requires_grad_(False)``); to train it without the tokenizer,
-        freeze all of it (``model.visual_tokenizer.requires_grad_(False)``)."""
+        The reference also trains the visual tokenizer's ViT-Adapter and Q-Former head and the image decoder.  This
+        leaves the tokenizer's flags as they are.  Its head (``pos_proj``, ``pos_ln``, ``post_ln``, the Q-Former,
+        ``proj``) and its ViT-Adapter have a backward here, its CLIP ViT weights do not: ``forward`` under autograd
+        raises while a CLIP ViT parameter requires grad or the image loss is on.  To train the text loss like the
+        reference, call ``model.freeze_like_reference(); model.visual_tokenizer.freeze_like_reference()``; to keep the
+        adapter frozen, freeze the encoder (``model.visual_tokenizer.encoder.requires_grad_(False)``); to train without
+        the tokenizer, freeze all of it (``model.visual_tokenizer.requires_grad_(False)``)."""
         for name, p in self.mm_decoder.named_parameters():
             p.requires_grad_("llama_cross_attn" in name)
         self.text_decoder.requires_grad_(False)

@@ -19,6 +19,13 @@ def _require(cond: bool, msg: str) -> None:
         raise RuntimeError(msg)
 
 
+def inference_only(name: str, *tensors) -> None:
+    """None of the ctypes kernels is autograd-aware: refuse to run where a gradient would be silently dropped."""
+    if torch.is_grad_enabled() and any(t is not None and torch.is_tensor(t) and t.requires_grad for t in tensors):
+        raise RuntimeError(f"{name}: this kernel is inference-only (no autograd support); call it under torch.no_grad() "
+                           "or detach its inputs / freeze its parameters")
+
+
 def _check_inputs(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step):
     # preconditions of ms_deform_attn_cuda_forward, cu:29-53, same messages
     _require(value.is_contiguous(), "value tensor has to be contiguous")
@@ -62,6 +69,7 @@ def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_lo
     through one launch on the current stream; ``im2col_step`` is validated like the
     reference does but does not change the result.  bf16 is accepted (superset).
     """
+    inference_only("ms_deform_attn_forward", value, sampling_loc, attn_weight)
     N, S, M, D, L, Lq, P = _check_inputs(value, spatial_shapes, level_start_index, sampling_loc,
                                          attn_weight, im2col_step)
     out = torch.empty((N, Lq, M * D), dtype=value.dtype, device=value.device)

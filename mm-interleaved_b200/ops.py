@@ -5,21 +5,15 @@ through the C ABI and raises if the library rejects the arguments -- there is no
 """
 from __future__ import annotations
 
+import math
 from typing import Optional
 
 import torch
 
 from . import _lib
-from .msda import _DTYPE_CODE, _require
+from .msda import _DTYPE_CODE, _require, inference_only
 
 launch_counter = [0]   # kernels of ours launched through this module (bench.py's gpu_launches)
-
-
-def inference_only(name: str, *tensors) -> None:
-    """None of the ctypes kernels is autograd-aware: refuse to run where a gradient would be silently dropped."""
-    if torch.is_grad_enabled() and any(t is not None and torch.is_tensor(t) and t.requires_grad for t in tensors):
-        raise RuntimeError(f"{name}: this kernel is inference-only (no autograd support); call it under torch.no_grad() "
-                           "or detach its inputs / freeze its parameters")
 
 
 def _stream():
@@ -559,6 +553,54 @@ def swiglu_backward(gate_up: torch.Tensor, d_out: torch.Tensor) -> torch.Tensor:
     _lib.check(rc, "swiglu_backward")
     launch_counter[0] += 1
     return d_gu
+
+
+def quick_gelu_backward(h: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
+    """dh of CLIP's quick_gelu ``h * sigmoid(1.702 h)``, computed in fp32 and rounded once (csrc/vit_bwd_sm100.cu)."""
+    inference_only("quick_gelu_backward", h, dy)
+    _require(h.is_cuda and h.is_contiguous() and dy.is_contiguous() and dy.shape == h.shape and dy.dtype == h.dtype,
+             "quick_gelu_backward: contiguous CUDA tensors of one shape and dtype required")
+    dh = torch.empty_like(h)
+    with torch.cuda.device(h.device):
+        rc = _lib.lib().mmfs_quick_gelu_backward(h.data_ptr(), dy.data_ptr(), dh.data_ptr(), h.numel(),
+                                                 _DTYPE_CODE[h.dtype], _stream())
+    _lib.check(rc, "quick_gelu_backward")
+    launch_counter[0] += 1
+    return dh
+
+
+def _pixel_stride(t: torch.Tensor):
+    """The one stride that steps pixel p = y * W + x of a (B, C, H, W) tensor, or None when H and W are not laid out
+    as one flattened pixel axis.  The stride of a size-1 dim is arbitrary in PyTorch and is not used."""
+    H, W = t.shape[2:]
+    if W > 1:
+        return t.stride(3) if H == 1 or t.stride(2) == W * t.stride(3) else None
+    return t.stride(2) if H > 1 else 1
+
+
+def resize_bilinear_backward(dy: torch.Tensor, in_hw, scale_factor: float) -> torch.Tensor:
+    """dx of ``F.interpolate(x, scale_factor=scale_factor, mode="bilinear", align_corners=False)`` for an x of spatial
+    size ``in_hw`` and the (B, C, Hout, Wout) gradient ``dy`` (read through its strides; NCHW and the token layout
+    (B, Hout*Wout, C) viewed as NCHW need no copy).  Returns dx in the token layout (B, Hin*Win, C), contiguous.
+    Gather form without atomics: bit-reproducible."""
+    inference_only("resize_bilinear_backward", dy)
+    Hin, Win = int(in_hw[0]), int(in_hw[1])
+    _require(dy.is_cuda and dy.dim() == 4, "resize_bilinear_backward: dy must be a (B, C, Hout, Wout) CUDA tensor")
+    B, C, Hout, Wout = dy.shape
+    _require((Hout, Wout) == (math.floor(Hin * scale_factor), math.floor(Win * scale_factor)),
+             "resize_bilinear_backward: dy's size is not the input size times the scale factor")
+    ps = _pixel_stride(dy)
+    if ps is None:
+        dy = dy.contiguous()
+        ps = _pixel_stride(dy)
+    dx = torch.empty((B, Hin * Win, C), dtype=dy.dtype, device=dy.device)
+    scale = float(1.0 / scale_factor)
+    with torch.cuda.device(dy.device):
+        rc = _lib.lib().mmfs_resize_bilinear_backward(dy.data_ptr(), dx.data_ptr(), B, C, Hin, Win, Hout, Wout, dy.stride(0),
+                                                      dy.stride(1), ps, scale, scale, _DTYPE_CODE[dy.dtype], _stream())
+    _lib.check(rc, "resize_bilinear_backward")
+    launch_counter[0] += 1
+    return dx
 
 
 def conv2d_supported(x: torch.Tensor, weight: torch.Tensor, stride: int, padding: int) -> bool:

@@ -31,6 +31,7 @@ from . import msda as _msda
 from . import ops
 from ._cache import WeightCache
 from .llama_mmfs import check_training_dtype, records_grad
+from .functions import MSDeformAttnFunction
 from .sd_mmfs import resize_abs_pos, sincos_pos_embed_2d
 
 
@@ -95,10 +96,20 @@ class CLIPAttention(nn.Module):
         return self._qkv.get(ps, lambda: (torch.cat(ps[:3], 0).contiguous(), torch.cat(ps[3:], 0).contiguous()))
 
     def forward(self, x):
-        """softmax(q k^T / sqrt(d)) v, no mask (CLIPXAttention.forward, xattn.py:47-141)."""
+        """softmax(q k^T / sqrt(d)) v, no mask (CLIPXAttention.forward, xattn.py:47-141).  When autograd records the call
+        (the gradient of a trainable ViT-Adapter crosses the frozen CLIP layers): forward with the row log-sum-exp and
+        the general attention backward into one (B, T, 3, H, hd) gradient, so the fused projection's backward is one
+        GEMM.  The q / k / v weights are read through a cache built without grad, so they must be frozen there."""
         B, T, _ = x.shape
         w, b = self._fused()
         qkv = F.linear(x, w, b).view(B, T, 3, self.num_heads, self.head_dim)
+        if records_grad(self, x):
+            if any(m.weight.requires_grad or m.bias.requires_grad for m in (self.q_proj, self.k_proj, self.v_proj)):
+                raise RuntimeError("CLIPAttention: the CLIP q / k / v projections have no weight gradient here (the "
+                                   "reference freezes the CLIP ViT); freeze them, e.g. with "
+                                   "VisualTokenizer.freeze_like_reference(), or run under torch.no_grad()")
+            check_training_dtype("CLIPAttention", x)
+            return self.out_proj(autograd_ops.attention(qkv, causal=False))
         ctx = ops.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], causal=False)
         return self.out_proj(ctx)
 
@@ -111,6 +122,9 @@ class CLIPMLP(nn.Module):
 
     def forward(self, x):
         h = self.fc1(x)
+        if records_grad(self, x):                                                   # same bits, backward on our kernel
+            check_training_dtype("CLIPMLP", h)
+            return self.fc2(autograd_ops.quick_gelu(h))
         return self.fc2(h * torch.sigmoid(1.702 * h))                               # quick_gelu
 
 
@@ -182,6 +196,10 @@ class MSDeformAttn(nn.Module):
             raise NotImplementedError("box reference points are not used on this path")
         normalizer = torch.stack([input_spatial_shapes[..., 1], input_spatial_shapes[..., 0]], -1)
         loc = reference_points[:, :, None, :, None, :] + off / normalizer[None, None, None, :, None, :]
+        if records_grad(self, query, input_flatten):        # deterministic backward to value, loc and attention weights
+            out = MSDeformAttnFunction.apply(value, input_spatial_shapes.contiguous(), input_level_start_index.contiguous(),
+                                             loc.to(value.dtype), aw.to(value.dtype), self.im2col_step)
+            return self.output_proj(out)
         out = _msda.ms_deform_attn_forward(value, input_spatial_shapes.contiguous(), input_level_start_index.contiguous(),
                                            loc.to(value.dtype).contiguous(), aw.to(value.dtype).contiguous(), self.im2col_step)
         return self.output_proj(out)
@@ -198,6 +216,9 @@ class ChannelsFirstLayerNorm(nn.Module):
 
     def forward(self, x):
         B, C, H, W = x.shape
+        if records_grad(self, x):
+            check_training_dtype("ChannelsFirstLayerNorm", x)
+            return autograd_ops.layernorm(x.permute(0, 2, 3, 1), self.weight, self.bias, self.eps).permute(0, 3, 1, 2)
         y = ops.layernorm(x.permute(0, 2, 3, 1).contiguous(), self.weight, self.bias, self.eps)
         return y.permute(0, 3, 1, 2)
 
@@ -336,6 +357,15 @@ def adapter_deform_inputs(h, w, device):
     return [_grid_points([(h // 16, w // 16)], device), ss1, st1], [_grid_points(s3, device), ss2, st2]
 
 
+def _resize(x, scale_factor):
+    """Bilinear resize of an adapter stage output; under autograd through the Function with the same forward bits and a
+    deterministic backward straight into the stage's token layout."""
+    if torch.is_grad_enabled() and x.requires_grad:
+        check_training_dtype("CLIPVisionTransformerAdapter", x)
+        return autograd_ops.resize_bilinear(x, scale_factor)
+    return F.interpolate(x, scale_factor=scale_factor, mode="bilinear", align_corners=False)
+
+
 class CLIPVisionTransformerAdapter(nn.Module):
     def __init__(self, config, conv_inplane=64, n_points=4):
         super().__init__()
@@ -384,9 +414,7 @@ class CLIPVisionTransformerAdapter(nn.Module):
         c1 = self.adapter_up(c2) + c1
         x1, x2, x3, x4 = outs
         last_hidden = torch.cat([cls, x4.flatten(2).transpose(1, 2)], dim=1)
-        x1 = F.interpolate(x1, scale_factor=4, mode="bilinear", align_corners=False)
-        x2 = F.interpolate(x2, scale_factor=2, mode="bilinear", align_corners=False)
-        x4 = F.interpolate(x4, scale_factor=0.5, mode="bilinear", align_corners=False)
+        x1, x2, x4 = _resize(x1, 4), _resize(x2, 2), _resize(x4, 0.5)
         return SimpleNamespace(last_hidden_state=last_hidden, pooler_output=cls,
                                hidden_states=[c1 + x1, c2 + x2, c3 + x3, c4 + x4])
 
@@ -575,6 +603,21 @@ class VisualTokenizer(nn.Module):
         if clip_normalize:
             self.register_buffer("clip_mean", torch.tensor(CLIP_MEAN).view(1, 3, 1, 1))
             self.register_buffer("clip_std", torch.tensor(CLIP_STD).view(1, 3, 1, 1))
+
+    def freeze_like_reference(self):
+        """The trainable set of the reference's tokenizer (vit_adapter_hf.py:246-252 with freeze=False, freeze_vit=True;
+        visual_tokenizer.py:27-31): in the encoder only the ViT-Adapter (parameters of ``encoder.vision_model`` whose
+        name starts with ``adapter``: the spatial prior module, injectors, extractors, ``adapter_level_embed``,
+        ``adapter_up``), the whole head (``pos_proj``, ``pos_ln``, the Q-Former, ``post_ln``, ``proj``), and not the
+        fixed ``pos_embed`` table.  The CLIP ViT stays frozen; its layers still pass the adapter's gradient on.
+        Returns ``self``.  ``MMInterleaved.freeze_like_reference()`` leaves the tokenizer alone: call both to train
+        like the reference, ``model.freeze_like_reference(); model.visual_tokenizer.freeze_like_reference()``."""
+        for name, p in self.encoder.vision_model.named_parameters():
+            p.requires_grad_(name.startswith("adapter"))
+        for name, p in self.named_parameters():
+            if not name.startswith("encoder."):
+                p.requires_grad_(name != "pos_embed")
+        return self
 
     def abs_pos(self, n):
         """``pos_embed`` without its cls row, resized to ``n`` positions.  Cached per length on the parameter itself
