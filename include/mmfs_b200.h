@@ -316,6 +316,16 @@ int mmfs_swiglu_backward(const void *gate_up, const void *d_out, void *d_gate_up
                          void *stream);
 
 /*
+ * Gradient of mmfs_geglu (training path, diffusers' GEGLU with the exact erf GELU): d_value_gate (rows, 2*inter) =
+ * [d value | d gate] of out = value * gelu(gate) from value_gate (rows, 2*inter) and d_out (rows, inter):
+ * d value = d_out * gelu(gate), d gate = d_out * value * (Phi(gate) + gate * phi(gate)), in fp32 with one rounding at the
+ * store.  16-byte vectors when inter % 8 == 0 and the pointers are 16-byte aligned, one element per step otherwise.
+ * rows < 0, inter <= 0, null pointers: MMFS_EINVAL.  A dtype other than bf16 / f16: MMFS_EUNSUPPORTED.
+ */
+int mmfs_geglu_backward(const void *value_gate, const void *d_out, void *d_value_gate, long rows, int inter, int dtype,
+                        void *stream);
+
+/*
  * Gradient of CLIP's quick_gelu, y = h * sigmoid(1.702 h) (training path): dh = dy * (s + 1.702 h s (1 - s)) with
  * s = sigmoid(1.702 h), over n elements of h, dy and dh, in fp32 with one rounding at the store.  16-byte vectors and a
  * scalar tail, so any n >= 0.  n < 0, null pointers: MMFS_EINVAL.  A dtype other than bf16 / f16, pointers not 16-byte
@@ -379,6 +389,19 @@ int mmfs_conv2d_down2x_nhwc(const void *x, const void *w, const void *bias, void
  */
 int mmfs_groupnorm_nhwc(const void *x, const void *gamma, const void *beta, void *y, float *stats, int B, int HW, int C,
                         int G, float eps, int silu, int dtype, void *stream);
+
+/*
+ * Gradient dx of mmfs_groupnorm_nhwc (training path, affine parameters frozen: no dgamma / dbeta).  With z = gamma xhat
+ * + beta: dz = dy, or with silu != 0 dz = dy s (1 + z (1 - s)), s = sigmoid(z) at z rounded to the element type as the
+ * forward rounds it; g = dz gamma; dx = r (g - mean(g) - xhat mean(g xhat)) per (image, group), r = 1 / sqrt(var + eps).
+ * The statistics are recomputed from x exactly as the forward computes them.  Three kernels; every sum is reduced in a
+ * fixed order without atomics, so dx is run-to-run reproducible.
+ *   x, dy, dx (B, HW, C) NHWC; gamma / beta (C) or NULL; scratch = 256*B*G floats of device memory private to the call.
+ * Null x / dy / dx / scratch, non-positive sizes, C % G != 0, B > 65535: MMFS_EINVAL.  f64 or an unknown dtype,
+ * C % (16/sizeof) != 0, C*sizeof > 8 KiB, tensors not 16-byte aligned: MMFS_EUNSUPPORTED.
+ */
+int mmfs_groupnorm_nhwc_backward(const void *x, const void *gamma, const void *beta, const void *dy, void *dx,
+                                 float *scratch, int B, int HW, int C, int G, float eps, int silu, int dtype, void *stream);
 
 /* modes of mmfs_decode_select */
 #define MMFS_SELECT_GREEDY 0

@@ -43,6 +43,7 @@ SIGNATURES = {
     "mmfs_geglu": (_I, [_P, _P, _L, _I, _I, _P]),
     "mmfs_attn_generic": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P]),
     "mmfs_groupnorm_nhwc": (_I, [_P] * 5 + [_I] * 4 + [_F, _I, _I, _P]),
+    "mmfs_groupnorm_nhwc_backward": (_I, [_P] * 6 + [_I] * 4 + [_F, _I, _I, _P]),
     "mmfs_conv2d_nhwc": (_I, [_P] * 6 + [_I] * 10 + [_P]),
     "mmfs_conv2d_up2x_nhwc": (_I, [_P] * 4 + [_I] * 6 + [_P]),
     "mmfs_conv2d_down2x_nhwc": (_I, [_P] * 4 + [_I] * 6 + [_P]),
@@ -55,6 +56,7 @@ SIGNATURES = {
     "mmfs_rmsnorm_backward": (_I, [_P] * 6 + [_L, _I, _F, _I, _P]),
     "mmfs_layernorm_backward": (_I, [_P] * 7 + [_L, _I, _F, _I, _P]),
     "mmfs_swiglu_backward": (_I, [_P] * 3 + [_L, _I, _I, _P]),
+    "mmfs_geglu_backward": (_I, [_P] * 3 + [_L, _I, _I, _P]),
     "mmfs_quick_gelu_backward": (_I, [_P] * 3 + [_L, _I, _P]),
     "mmfs_resize_bilinear_backward": (_I, [_P] * 2 + [_I] * 6 + [_L] * 3 + [_F, _F, _I, _P]),
     "mmfs_decode_select": (_I, [_P, _L] + [_P] * 5 + [_I, _L, _I] + [_P] * 3 + [_I] * 4 + [_P]),

@@ -1,5 +1,5 @@
-"""Autograd Functions over the decoder-layer kernels: the training path of the Llama decoder's self-attention layer
-and of the visual tokenizer's Q-Former head.
+"""Autograd Functions over the decoder-layer kernels: the training path of the Llama decoder's self-attention layer,
+of the visual tokenizer, and of the image loss through the frozen SD UNet.
 
 Each forward runs the same sm_90a kernel as the inference wrapper in ops.py (a Function's forward runs with grad
 disabled, so the wrappers' ``inference_only`` guard does not fire there) and saves what its backward kernel reads:
@@ -18,9 +18,14 @@ disabled, so the wrappers' ``inference_only`` guard does not fire there) and sav
 * ``QuickGELUFunction`` -- CLIP's ``h * sigmoid(1.702 h)`` in torch ops (the inference path's bits), backward on
   ``mmfs_quick_gelu_backward``; saves h only;
 * ``ResizeBilinearFunction`` -- ``F.interpolate(scale_factor=s, mode="bilinear")`` forward (the inference path's
-  bits), backward on ``mmfs_resize_bilinear_backward`` straight into the token layout of the input.
+  bits), backward on ``mmfs_resize_bilinear_backward`` straight into the token layout of the input;
+* ``ConvFunction`` -- the SD UNet's convolution with its fused time-embedding add and residual, forward exactly the
+  inference ``ops.conv2d`` call; the backward gives dx and d residual with the filter frozen (``conv_input_grad``);
+* ``GroupNormNHWCFunction`` -- ``mmfs_groupnorm_nhwc`` (+ SiLU) / ``mmfs_groupnorm_nhwc_backward``, saves x only;
+  frozen affine parameters;
+* ``GEGLUFunction`` -- ``mmfs_geglu`` / ``mmfs_geglu_backward`` on the [value | gate] buffer.
 
-The backward kernels take bf16 / fp16 only, the causal attention backward head dim 128 without a KV cache and the
+The backward kernels take bf16 / fp16 only (the GroupNorm backward fp32 too), the causal attention backward head dim 128 without a KV cache and the
 general one head dim 64 or 128; other inputs are refused with the library's message.  Double backward is not
 supported.
 """
@@ -175,6 +180,82 @@ class ResizeBilinearFunction(Function):
         return dx.view(B, H, W, C).permute(0, 3, 1, 2), None
 
 
+def _refuse_trainable(what, *params):
+    """The Functions below give no gradient to these tensors: refuse to drop one silently."""
+    if any(p is not None and p.requires_grad for p in params):
+        raise RuntimeError(f"{what}: the UNet's own weights have no backward here (the image loss trains what feeds the "
+                           "UNet); freeze them, e.g. unet.requires_grad_(False)")
+
+
+def conv_input_grad(conv, dy: torch.Tensor, x_shape) -> torch.Tensor:
+    """dx of ``conv`` (a ``unet_sd.Conv2d``: 3x3 / pad 1 or 1x1 / pad 0 at stride 1, or 3x3 / pad 1 at stride 2) for an
+    input of shape ``x_shape`` and output gradient ``dy``.
+
+    * stride 1: dx is the same convolution of dy with the channel-transposed, 180-degree-rotated filter
+      (``ops.dgrad_weights_khwc``) on the wgmma kernel;
+    * stride 2: dx at the 2H x 2W input is four 2x2 phase convolutions over the H x W dy, the ``conv2d_up2x`` kernel with
+      the filter folded by ``ops.fold_dgrad_down2x_weights``;
+    * where the swapped channel counts or the tile rule rule the kernels out, ``torch.nn.grad.conv2d_input`` (cuDNN)."""
+    w = conv.weight
+    stride, pad = conv.stride[0], conv.padding[0]
+    K = w.shape[-1]
+    if dy.is_cuda and not dy.is_contiguous(memory_format=torch.channels_last):
+        dy = dy.contiguous(memory_format=torch.channels_last)
+    wt = w.transpose(0, 1)                                      # (Cin, Cout, K, K): the dgrad's channel roles
+    if stride == 1 and 2 * pad == K - 1 and ops.conv2d_supported(dy, wt, 1, pad):
+        return ops.conv2d(dy, conv.weight_dgrad_khwc(), None, 1, pad)
+    if (stride == 2 and K == 3 and pad == 1 and tuple(x_shape[2:]) == (2 * dy.shape[2], 2 * dy.shape[3])
+            and ops.conv2d_up2x_supported(dy, wt)):
+        return ops.conv2d_up2x(dy, conv.weight_dgrad_down2x())
+    return torch.nn.grad.conv2d_input(tuple(x_shape), w, dy, stride=stride, padding=pad)
+
+
+class ConvFunction(Function):
+    @staticmethod
+    def forward(ctx, x, residual, conv, add_bc):
+        """``conv(x) [+ add_bc[:, :, None, None]] [+ residual]`` as the inference path computes it (``conv.fused``);
+        ``conv``'s filter, bias and ``add_bc`` (the time-embedding projection) carry no gradient."""
+        _refuse_trainable("ConvFunction", conv.weight, conv.bias, add_bc)
+        ctx.conv, ctx.x_shape = conv, tuple(x.shape)
+        return conv.fused(x, add_bc, residual)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        dx = conv_input_grad(ctx.conv, dy, ctx.x_shape) if ctx.needs_input_grad[0] else None
+        return dx, (dy if ctx.needs_input_grad[1] else None), None, None
+
+
+class GroupNormNHWCFunction(Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, groups, eps, silu):
+        _refuse_trainable("GroupNormNHWCFunction", weight, bias)
+        ctx.groups, ctx.eps, ctx.silu = groups, eps, silu
+        ctx.save_for_backward(x, weight, bias)
+        return ops.group_norm_nhwc(x, groups, weight, bias, eps, silu=silu)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, weight, bias = ctx.saved_tensors
+        dx = ops.group_norm_nhwc_backward(x, dy, ctx.groups, weight, bias, ctx.eps, silu=ctx.silu)
+        return dx, None, None, None, None, None
+
+
+class GEGLUFunction(Function):
+    @staticmethod
+    def forward(ctx, value_gate):
+        value_gate = value_gate.contiguous()
+        ctx.save_for_backward(value_gate)
+        return ops.geglu(value_gate)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_out):
+        (value_gate,) = ctx.saved_tensors
+        return ops.geglu_backward(value_gate, d_out.contiguous())
+
+
 def rmsnorm(x, weight, eps):
     return RMSNormFunction.apply(x, weight, eps)
 
@@ -205,3 +286,15 @@ def quick_gelu(h):
 
 def resize_bilinear(x, scale_factor):
     return ResizeBilinearFunction.apply(x, scale_factor)
+
+
+def conv(x, conv_module, add_bc=None, residual=None):
+    return ConvFunction.apply(x, residual, conv_module, add_bc)
+
+
+def group_norm_nhwc(x, groups, weight=None, bias=None, eps=1e-5, silu=False):
+    return GroupNormNHWCFunction.apply(x, weight, bias, groups, float(eps), bool(silu))
+
+
+def geglu(value_gate):
+    return GEGLUFunction.apply(value_gate)

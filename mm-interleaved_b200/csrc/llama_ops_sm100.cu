@@ -4,7 +4,8 @@
 //   mmfs_rope_qk      apply_rotary_pos_emb / rotate_half decoders/modeling_llama_mmfs.py:158-172
 //   mmfs_swiglu       LlamaMLP: act_fn(gate) * up        decoders/modeling_llama_mmfs.py:188-189
 //   mmfs_layernorm    nn.LayerNorm (CLIP / Q-Former / MMFSBlock norms)
-//   mmfs_rmsnorm_backward, mmfs_swiglu_backward, mmfs_layernorm_backward
+//   mmfs_geglu        diffusers GEGLU: value * gelu(gate) (the SD UNet's feed-forward)
+//   mmfs_rmsnorm_backward, mmfs_swiglu_backward, mmfs_layernorm_backward, mmfs_geglu_backward
 //                     their gradients (training path, 16-bit tensors, fp32 math)
 //
 // Each mimics the rounding points of the reference's tensor pipeline in the storage type T (a
@@ -598,6 +599,60 @@ __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const T *__restrict__ g
         }
 }
 
+// ---- GEGLU backward: out = v * gelu(g), gelu(g) = g Phi(g) (exact erf form)  ->  dv = d * gelu(g),
+// dg = d * v * (Phi(g) + g phi(g)), Phi / phi the standard normal CDF / density.  fp32, one rounding at the store.  The
+// index space is the (rows, I) grid flattened; kVec: I % VEC == 0 and 16-byte aligned tensors, so every 16-byte vector
+// lies inside one row; otherwise one element per step.
+__device__ __forceinline__ void geglu_grad(float v, float g, float d, float &dv, float &dg) {
+    const float cdf = 0.5f * (1.f + erff(g * 0.70710678118654752f));
+    const float pdf = 0.39894228040143268f * expf(-0.5f * g * g);
+    dv = d * g * cdf;
+    dg = d * v * fmaf(g, pdf, cdf);
+}
+
+template <typename T, bool kVec>
+__global__ void __launch_bounds__(256) geglu_bwd_kernel(const T *__restrict__ vg, const T *__restrict__ d_out,
+                                                        T *__restrict__ d_vg, long rows, int I) {
+    constexpr int VEC = kVec ? 16 / (int)sizeof(T) : 1;
+    const long per_row = I / VEC, n = rows * per_row;
+    const long stride = (long)gridDim.x * blockDim.x;
+    for (long t = (long)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
+        const long r = t / per_row, i = (t - r * per_row) * VEC;
+        const long v_at = r * 2 * I + i, g_at = v_at + I;
+        float v[VEC], g[VEC], d[VEC], dv[VEC], dg[VEC];
+        if constexpr (kVec) {
+            Vec16<T>::unpack(ldg_nc_v4(vg + v_at), v);
+            Vec16<T>::unpack(ldg_nc_v4(vg + g_at), g);
+            Vec16<T>::unpack(ldg_nc_v4(d_out + r * I + i), d);
+        } else {
+            v[0] = to_op(vg[v_at]);
+            g[0] = to_op(vg[g_at]);
+            d[0] = to_op(d_out[r * I + i]);
+        }
+#pragma unroll
+        for (int k = 0; k < VEC; ++k) geglu_grad(v[k], g[k], d[k], dv[k], dg[k]);
+        if constexpr (kVec) {
+            stg_v4(d_vg + v_at, Vec16<T>::pack(dv));
+            stg_v4(d_vg + g_at, Vec16<T>::pack(dg));
+        } else {
+            d_vg[v_at] = from_op<T>(dv[0]);
+            d_vg[g_at] = from_op<T>(dg[0]);
+        }
+    }
+}
+
+template <typename T>
+static int launch_geglu_bwd(const void *vg, const void *d_out, void *d_vg, long rows, int inter, bool vec, cudaStream_t st) {
+    const long items = rows * (vec ? inter / (16 / (int)sizeof(T)) : inter);
+    const int grid = capped_grid((items + 255) / 256, 8);
+    if (vec)
+        geglu_bwd_kernel<T, true><<<grid, 256, 0, st>>>((const T *)vg, (const T *)d_out, (T *)d_vg, rows, inter);
+    else
+        geglu_bwd_kernel<T, false><<<grid, 256, 0, st>>>((const T *)vg, (const T *)d_out, (T *)d_vg, rows, inter);
+    MMFS_CUDA(cudaGetLastError());
+    return MMFS_OK;
+}
+
 template <typename T>
 static int launch_rmsnorm_bwd(const void *x, const void *w, const void *dy, void *dx, void *dw, float *partials, long rows,
                               int cols, float eps, cudaStream_t st) {
@@ -751,6 +806,22 @@ extern "C" int mmfs_swiglu_backward(const void *gate_up, const void *d_out, void
     }
     return dispatch_dtype<kF16Types, MMFS_EUNSUPPORTED>(dtype, "swiglu_backward", [&](auto tag) {
         return launch_swiglu_bwd<typename decltype(tag)::type>(gate_up, d_out, d_gate_up, rows, inter, (cudaStream_t)stream);
+    });
+}
+
+extern "C" int mmfs_geglu_backward(const void *value_gate, const void *d_out, void *d_value_gate, long rows, int inter,
+                                   int dtype, void *stream) {
+    MMFS_CHECK_ARG(rows >= 0 && inter > 0, "geglu_backward: bad shape");
+    if (rows == 0) return MMFS_OK;
+    MMFS_CHECK_ARG(value_gate && d_out && d_value_gate, "geglu_backward: null pointer argument");
+    if (!(dtype == MMFS_BF16 || dtype == MMFS_F16)) {
+        set_error("geglu_backward: needs bf16 / f16 (got dtype=%d)", dtype);
+        return MMFS_EUNSUPPORTED;
+    }
+    const bool vec = inter % 8 == 0 && ((uintptr_t)value_gate | (uintptr_t)d_out | (uintptr_t)d_value_gate) % 16 == 0;
+    return dispatch_dtype<kF16Types, MMFS_EUNSUPPORTED>(dtype, "geglu_backward", [&](auto tag) {
+        return launch_geglu_bwd<typename decltype(tag)::type>(value_gate, d_out, d_value_gate, rows, inter, vec,
+                                                              (cudaStream_t)stream);
     });
 }
 

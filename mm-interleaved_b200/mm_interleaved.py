@@ -264,15 +264,19 @@ class StableDiffusion(nn.Module):
 
     def _encode_latents(self, image, dtype, generator=None):
         """sd.py:220-238: posterior samples of ``vae_encode_mini_bs`` images at a time, cast to ``dtype``, times the
-        scaling factor.  The VAE encodes in its own dtype (the reference casts it to fp32)."""
+        scaling factor.  The VAE encodes in its own dtype (the reference casts it to fp32), under ``torch.no_grad()`` as
+        there: the VAE is frozen and nothing upstream of the latents trains."""
         n = self.vae_encode_mini_bs if self.vae_encode_mini_bs > 0 else image.shape[0]
-        parts = [self.vae.encode(image[i:i + n]).latent_dist.sample(generator).to(dtype) for i in range(0, image.shape[0], n)]
+        with torch.no_grad():
+            parts = [self.vae.encode(image[i:i + n]).latent_dist.sample(generator).to(dtype)
+                     for i in range(0, image.shape[0], n)]
         return torch.cat(parts, dim=0) * self.vae_scaling_factor
 
     def forward(self, image, text_embeds, return_outputs=False, mmfs_features=None, mmfs_mask=None,
                 generator: Optional[torch.Generator] = None):
-        """The denoising loss of sd.py:240-316 (inference kernels: an evaluation loss, call under ``torch.no_grad()``).
-        ``image`` (B, 3, S, S) in [0, 1] with S = ``image_size``; returns the per-element
+        """The denoising loss of sd.py:240-316.  Under autograd its gradient reaches ``text_embeds``, the MMFS hook
+        (``mmfs_module``) and ``mmfs_features`` through the frozen UNet (``unet.requires_grad_(False)``; the UNet's own
+        weights have no backward here).  ``image`` (B, 3, S, S) in [0, 1] with S = ``image_size``; returns the per-element
         ``mse(unet(noisy, t), target)`` in fp32, shaped like the latents, or with ``return_outputs`` the reference's
         ``dict(loss, pred, target)`` plus ``latents`` and ``timesteps``.
 
@@ -350,7 +354,10 @@ class ImageDecoder(nn.Module):
         probability ``uncond_prob`` an image's prompt is replaced by ``neg_prompt_embeds`` (in eval mode too, as in the
         reference; that ``rand`` is drawn before the diffusion loss's draws, from ``generator`` when given); the
         per-element SD loss is zeroed for images whose context has <= 2 tokens (``<bos>``, ``<soi>``) and where
-        ``image_loss_mask`` is 0, then averaged over every element, zeroed ones included."""
+        ``image_loss_mask`` is 0, then averaged over every element, zeroed ones included.  Differentiable: under
+        autograd the gradient reaches the Q-Former, ``neg_prompt_embeds``, the MMFS hook, ``context_features`` and
+        ``mmfs_features`` through the frozen UNet (``decoder.unet.requires_grad_(False)``; its own weights have no
+        backward here)."""
         assert image_tensors.shape[0] == context_features.shape[0]
         if context_attention_mask is None:
             raise ValueError("ImageDecoder.forward needs context_attention_mask")
@@ -650,8 +657,11 @@ class MMInterleaved(InterleavedForward):
         then leaves the output, as there.  ``generator`` (keyword) seeds the image loss's random draws.
         Under autograd the text loss is differentiable (``freeze_like_reference``), down to the visual tokenizer's head
         (``pos_proj``, ``pos_ln``, ``post_ln``, the Q-Former, ``proj``) and its ViT-Adapter, through the frozen CLIP ViT
-        (``visual_tokenizer.freeze_like_reference()``); a trainable CLIP ViT weight or an image loss raises up front, as
-        neither has a backward here."""
+        (``visual_tokenizer.freeze_like_reference()``).  The image loss is differentiable too, through the frozen SD UNet
+        (``image_decoder.decoder.unet.requires_grad_(False)``): its gradient reaches the image decoder's Q-Former,
+        ``neg_prompt_embeds``, the MMFS hook, ``context_feat_proj`` and, through the context and the MMFS features, the
+        LLM and the visual tokenizer.  A trainable CLIP ViT weight or, with the image loss on, a trainable UNet weight
+        raises up front, as neither has a backward here."""
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             if any(p.requires_grad for n, p in self.visual_tokenizer.encoder.vision_model.named_parameters()
                    if not n.startswith("adapter")):
@@ -659,10 +669,11 @@ class MMInterleaved(InterleavedForward):
                                    "for its CLIP ViT weights (the reference freezes them, and trains the ViT-Adapter); "
                                    "call model.visual_tokenizer.freeze_like_reference(), or freeze the whole encoder "
                                    "(model.visual_tokenizer.encoder.requires_grad_(False)), or run under torch.no_grad()")
-            if self._has_image_loss():
-                raise RuntimeError("MMInterleaved.forward under autograd: the image-decoder loss has no backward here; "
-                                   "build the image decoder's VAE without an encoder (no image loss) or run under "
-                                   "torch.no_grad()")
+            if self._has_image_loss() and not self._image_loss_differentiable():
+                raise RuntimeError("MMInterleaved.forward under autograd: the image-decoder loss has no backward here "
+                                   "for the UNet's own weights (it trains what feeds the UNet); freeze them with "
+                                   "model.image_decoder.decoder.unet.requires_grad_(False), or build the image decoder's "
+                                   "VAE without an encoder (no image loss), or run under torch.no_grad()")
         return_loss = kwargs.pop("return_loss", True)
         generator = kwargs.pop("generator", None)
         out = self._prepare_mm_embeds(text_ids, image_tensors, num_image_per_seq, meta, kwargs.pop("max_num_image", None))
@@ -701,10 +712,13 @@ class MMInterleaved(InterleavedForward):
         The reference also trains the visual tokenizer's ViT-Adapter and Q-Former head and the image decoder.  This
         leaves the tokenizer's flags as they are.  Its head (``pos_proj``, ``pos_ln``, ``post_ln``, the Q-Former,
         ``proj``) and its ViT-Adapter have a backward here, its CLIP ViT weights do not: ``forward`` under autograd
-        raises while a CLIP ViT parameter requires grad or the image loss is on.  To train the text loss like the
-        reference, call ``model.freeze_like_reference(); model.visual_tokenizer.freeze_like_reference()``; to keep the
-        adapter frozen, freeze the encoder (``model.visual_tokenizer.encoder.requires_grad_(False)``); to train without
-        the tokenizer, freeze all of it (``model.visual_tokenizer.requires_grad_(False)``)."""
+        raises while a CLIP ViT parameter requires grad, or while the image loss is on and a UNet parameter requires
+        grad.  The image decoder's flags are left as they are too: its Q-Former, ``neg_prompt_embeds`` and MMFS hook
+        have a backward, the UNet's own weights do not (``model.image_decoder.decoder.unet.requires_grad_(False)``).
+        To train the text loss like the reference, call ``model.freeze_like_reference();
+        model.visual_tokenizer.freeze_like_reference()``; to keep the adapter frozen, freeze the encoder
+        (``model.visual_tokenizer.encoder.requires_grad_(False)``); to train without the tokenizer, freeze all of it
+        (``model.visual_tokenizer.requires_grad_(False)``)."""
         for name, p in self.mm_decoder.named_parameters():
             p.requires_grad_("llama_cross_attn" in name)
         self.text_decoder.requires_grad_(False)
@@ -715,6 +729,12 @@ class MMInterleaved(InterleavedForward):
     def _has_image_loss(self) -> bool:
         sd = getattr(self.image_decoder, "decoder", None)
         return getattr(getattr(sd, "vae", None), "encoder", None) is not None
+
+    def _image_loss_differentiable(self) -> bool:
+        """The image loss has a backward when the image decoder runs this repository's UNet with its weights frozen."""
+        from .unet_sd import UNet2DConditionModel, has_trainable_weights
+        unet = getattr(getattr(self.image_decoder, "decoder", None), "unet", None)
+        return isinstance(unet, UNet2DConditionModel) and not has_trainable_weights(unet)
 
     @torch.no_grad()
     def generate_texts(self, text_ids, image_tensors=None, num_image_per_seq=None, attention_mask=None, meta=None, **kwargs):

@@ -555,6 +555,22 @@ def swiglu_backward(gate_up: torch.Tensor, d_out: torch.Tensor) -> torch.Tensor:
     return d_gu
 
 
+def geglu_backward(value_gate: torch.Tensor, d_out: torch.Tensor) -> torch.Tensor:
+    """d(value_gate) of ``geglu``: [d value | d gate], computed in fp32 and rounded once."""
+    inference_only("geglu_backward", value_gate, d_out)
+    _require(value_gate.is_cuda and value_gate.is_contiguous() and d_out.is_contiguous() and value_gate.shape[-1] % 2 == 0
+             and d_out.shape == value_gate.shape[:-1] + (value_gate.shape[-1] // 2,) and d_out.dtype == value_gate.dtype
+             and d_out.device == value_gate.device, "geglu_backward: bad input")
+    inter = value_gate.shape[-1] // 2
+    d_vg = torch.empty_like(value_gate)
+    with torch.cuda.device(value_gate.device):
+        rc = _lib.lib().mmfs_geglu_backward(value_gate.data_ptr(), d_out.data_ptr(), d_vg.data_ptr(),
+                                            value_gate.numel() // (2 * inter), inter, _DTYPE_CODE[value_gate.dtype], _stream())
+    _lib.check(rc, "geglu_backward")
+    launch_counter[0] += 1
+    return d_vg
+
+
 def quick_gelu_backward(h: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
     """dh of CLIP's quick_gelu ``h * sigmoid(1.702 h)``, computed in fp32 and rounded once (csrc/vit_bwd_sm100.cu)."""
     inference_only("quick_gelu_backward", h, dy)
@@ -652,6 +668,29 @@ def fold_up2x_weights(weight: torch.Tensor) -> torch.Tensor:
     return w.reshape(4, *w.shape[2:]).to(weight.dtype).contiguous()
 
 
+def dgrad_weights_khwc(weight: torch.Tensor) -> torch.Tensor:
+    """The filter of the data gradient of a stride-1, 'same'-padded convolution, in ``conv2d``'s KHWC layout.
+
+    For y = conv(x, W) with a KxK filter and pad (K-1)/2, dx = conv(dy, W') with the same padding, where W' swaps the
+    channel roles and rotates the taps by 180 degrees: ``W'[ci, ky, kx, co] = W[co, ci, K-1-ky, K-1-kx]``.  A pure
+    re-indexing, so no rounding."""
+    return weight.flip(2, 3).permute(1, 2, 3, 0).contiguous()
+
+
+def fold_dgrad_down2x_weights(weight: torch.Tensor) -> torch.Tensor:
+    """A 3x3 / stride-2 / pad-1 filter (Cout, Cin, 3, 3) folded into the data gradient's phase filters for ``conv2d_up2x``:
+    (4, Cin, 2, 2, Cout), phase p = 2 py + px.
+
+    y[i] = sum_k w[k] x[2i + k - 1] along each axis, so dx at input row 2j (py = 0) is w[1] dy[j], and at row 2j + 1
+    (py = 1) w[2] dy[j] + w[0] dy[j + 1]: in ``conv2d_up2x``'s tap order (offsets {-1, 0} for py = 0, {0, +1} for py = 1)
+    the rows fold to {0, w1} or {w2, w0}, the columns alike, and the channels are transposed.  Summed in fp32 (fp64 stays
+    fp64) and rounded to the filter's dtype once (each tap is a single weight, so the fold is exact)."""
+    acc = torch.float64 if weight.dtype == torch.float64 else torch.float32
+    fold = torch.tensor([[[0, 0, 0], [0, 1, 0]], [[0, 0, 1], [1, 0, 0]]], dtype=acc, device=weight.device)   # (py, tap, k)
+    w = torch.einsum("pak,ockl,qbl->pqcabo", fold, weight.to(acc), fold)         # (py, px, Cin, 2, 2, Cout)
+    return w.reshape(4, *w.shape[2:]).to(weight.dtype).contiguous()
+
+
 def conv2d_up2x_supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
     """Whether ``conv2d_up2x`` can take ``conv3x3(interpolate(x, 2, "nearest"))`` for this (B, Cin, H, W) input and
     (Cout, Cin, 3, 3) filter."""
@@ -738,3 +777,32 @@ def group_norm_nhwc(x: torch.Tensor, groups: int, weight=None, bias=None, eps: f
     _lib.check(rc, "group_norm_nhwc")
     launch_counter[0] += 2
     return y
+
+
+def group_norm_nhwc_backward(x: torch.Tensor, dy: torch.Tensor, groups: int, weight=None, bias=None, eps: float = 1e-5,
+                             silu: bool = False) -> torch.Tensor:
+    """dx of ``group_norm_nhwc`` (csrc/groupnorm_nhwc_sm100.cu, three kernels): the statistics recomputed from x as the
+    forward computes them, the SiLU derivative taken at the forward's rounded pre-activation, every sum reduced in a
+    fixed order (run-to-run reproducible).  The affine parameters get no gradient.  ``x`` and ``dy`` channels_last
+    (B, C, H, W) of one dtype; returns dx channels_last."""
+    inference_only("group_norm_nhwc_backward", x, dy, weight, bias)
+    _require(group_norm_supported(x) and x.shape[1] * x.element_size() <= 8192,
+             "group_norm_nhwc_backward: need a CUDA channels_last f32/f16/bf16 tensor with C % (16/size) == 0 and "
+             "C * size <= 8 KiB")
+    _require(dy.shape == x.shape and dy.dtype == x.dtype and dy.device == x.device,
+             "group_norm_nhwc_backward: dy must match x in shape, dtype and device")
+    if not dy.is_contiguous(memory_format=torch.channels_last):
+        dy = dy.contiguous(memory_format=torch.channels_last)
+    B, C, H, W = x.shape
+    _require(groups > 0 and C % groups == 0, f"group_norm_nhwc_backward: {C} channels do not split into {groups} groups")
+    _check_affine("group_norm_nhwc_backward", x, C, weight, bias)
+    dx = torch.empty_like(x, memory_format=torch.channels_last)
+    scratch = torch.empty((2, B, 64, groups, 2), dtype=torch.float32, device=x.device)   # statistics, then (sum g, sum g xhat)
+    with torch.cuda.device(x.device):
+        rc = _lib.lib().mmfs_groupnorm_nhwc_backward(x.data_ptr(), weight.data_ptr() if weight is not None else None,
+                                                     bias.data_ptr() if bias is not None else None, dy.data_ptr(),
+                                                     dx.data_ptr(), scratch.data_ptr(), B, H * W, C, groups, float(eps),
+                                                     int(silu), _DTYPE_CODE[x.dtype], _stream())
+    _lib.check(rc, "group_norm_nhwc_backward")
+    launch_counter[0] += 3
+    return dx

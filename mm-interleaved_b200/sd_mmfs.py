@@ -11,6 +11,10 @@ unchanged.  Built for the denoise loop:
 * the zero-initialised 1x1 ``conv`` after MMFS is folded into ``output_proj`` (one GEMM instead of GEMM + conv);
 * the per-pixel reference grid and the resized sin-cos position embedding are cached per query size;
 * sampling runs in the fused MMFS kernel (pixel-grid reference points, 2-D image mask).
+
+Under autograd (the image loss) a block runs ``_forward_differentiable`` instead: the LayerNorm Function on the
+query and on the features (no feature cache), the frozen position embedding, ``MMFS.forward_differentiable`` on the
+pixel grid, then ``output_proj`` and the 1x1 ``conv`` as two maps -- the folded weight is inference-only.
 """
 from __future__ import annotations
 
@@ -120,9 +124,28 @@ class MMFSBlock(nn.Module):
         n = self.feat_norm                      # no memoisation here: the caller owns the result (PreparedSDFeatures)
         return self.mmfs.project_value(ops.layernorm(ms_feat.contiguous(), n.weight, n.bias, n.eps), cache=False)
 
+    def _records(self, sample, ms_feat) -> bool:
+        return torch.is_grad_enabled() and (sample.requires_grad or (ms_feat is not None and ms_feat.requires_grad)
+                                            or any(p.requires_grad for p in self.parameters()))
+
+    def _forward_differentiable(self, sample, ms_feat, ms_feat_mask, spatial_shapes):
+        from . import autograd_ops
+        B, C, H, W = sample.shape
+        n_images = ms_feat_mask.shape[-1]
+        ref, ss, starts, pos = self._geometry(sample.device, sample.dtype, H, W, n_images, spatial_shapes)
+        qn, fn = self.query_norm, self.feat_norm
+        query = sample.flatten(2).transpose(1, 2).contiguous()                       # b c h w -> b (h w) c
+        query = autograd_ops.layernorm(query, qn.weight, qn.bias, qn.eps) + pos
+        feat = autograd_ops.layernorm(ms_feat.contiguous(), fn.weight, fn.bias, fn.eps)
+        out = self.mmfs.forward_differentiable(query, ref, feat, ss, starts, ms_feat_mask)          # output_proj included
+        out = F.linear(out, self.conv.weight.view(C, C), self.conv.bias)                          # the 1x1 conv, per token
+        return out.transpose(1, 2).reshape(B, C, H, W)
+
     def forward(self, sample, ms_feat, ms_feat_mask, spatial_shapes, value=None):
         """sample (B, C_q, H, W); ms_feat (B, N, sum(H_l*W_l), C_v); ms_feat_mask (B, N); returns the residual (B, C_q, H, W).
         ``value`` (extension): ``project_features(ms_feat)`` computed by the caller (``ms_feat`` is then not read)."""
+        if value is None and self._records(sample, ms_feat):
+            return self._forward_differentiable(sample, ms_feat, ms_feat_mask, spatial_shapes)
         B, C, H, W = sample.shape
         n_images = ms_feat_mask.shape[-1]
         ref, ss, starts, pos = self._geometry(sample.device, sample.dtype, H, W, n_images, spatial_shapes)
@@ -192,6 +215,11 @@ class MMFSNet(nn.Module):
         """``mmfs_features``: the list of feature maps (reference signature) or a ``PreparedSDFeatures`` (extension)."""
         assert len(down_block_res_samples) == len(self.mmfs_down_blocks)
         if isinstance(mmfs_features, PreparedSDFeatures):
+            if torch.is_grad_enabled() and (any(t.requires_grad for t in (sample, *down_block_res_samples))
+                                            or any(p.requires_grad for p in self.parameters())):
+                raise RuntimeError("MMFSNet.forward under autograd: a PreparedSDFeatures was built under no_grad and "
+                                   "would cut the gradient to the feature maps and the feature-side weights; pass the "
+                                   "list of feature maps instead")
             pv = mmfs_features
             new_res = ()
             for res, blk, val in zip(down_block_res_samples, self.mmfs_down_blocks, pv.values):

@@ -18,6 +18,13 @@ when the model is bf16/f16 and channels-last) in the implicit-GEMM wgmma kernel 
 ResNet block's time-embedding add and residual add fused into its epilogue; GroupNorm(+SiLU) runs in an NHWC kernel
 (csrc/groupnorm_nhwc_sm100.cu) because torch's CUDA group_norm returns NCHW and would force a layout round trip
 around every convolution.
+
+Training path (the image loss): when autograd records, the convolutions, GroupNorms, GEGLUs, attentions and
+LayerNorms switch to the Functions of autograd_ops.py, whose forwards run the same kernels as the inference path and
+whose backwards carry the gradient to the UNet's inputs -- the context, the MMFS hook and what feeds them.  The UNet's
+own weights get no gradient here: ``UNet2DConditionModel.forward`` under autograd raises while any of them requires
+grad.  Nearest upsampling, ``cat``, the linears and ``conv_in`` / ``conv_out`` (library convolutions) stay on PyTorch
+autograd.
 """
 from __future__ import annotations
 
@@ -34,9 +41,23 @@ from ._cache import WeightCache
 USE_CONV_KERNEL = True      # tests flip this to compare against the cuDNN path on the same weights
 
 
+def _records(*tensors) -> bool:
+    """Whether autograd records an op on these tensors (the training path's switch)."""
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
+def has_trainable_weights(unet: nn.Module) -> bool:
+    """Whether a UNet parameter requires grad: the UNet's weights have no backward here, so its forward under autograd
+    (and ``MMInterleaved.forward`` with the image loss on) refuses to run then."""
+    return any(p.requires_grad for p in unet.parameters())
+
+
 def _gn(mod: nn.GroupNorm, x: torch.Tensor, silu: bool) -> torch.Tensor:
     """``silu(mod(x))`` / ``mod(x)`` kept in NHWC by this repo's kernel when x is channels-last on the GPU."""
     if USE_CONV_KERNEL and ops.group_norm_supported(x):
+        if _records(x, mod.weight, mod.bias):
+            from . import autograd_ops
+            return autograd_ops.group_norm_nhwc(x, mod.num_groups, mod.weight, mod.bias, mod.eps, silu=silu)
         return ops.group_norm_nhwc(x, mod.num_groups, mod.weight, mod.bias, mod.eps, silu=silu)
     h = mod(x)
     return F.silu(h) if silu else h
@@ -55,20 +76,42 @@ class Conv2d(nn.Conv2d):
     def weight_up2x(self) -> torch.Tensor:
         return self._derived.get(self.weight, lambda: ops.fold_up2x_weights(self.weight), key="up2x")
 
+    def weight_dgrad_khwc(self) -> torch.Tensor:
+        """The data gradient's filter of a stride-1 layer (``ops.dgrad_weights_khwc``)."""
+        return self._derived.get(self.weight, lambda: ops.dgrad_weights_khwc(self.weight.detach()), key="dgrad_khwc")
+
+    def weight_dgrad_down2x(self) -> torch.Tensor:
+        """The data gradient's phase filters of a 3x3 / stride-2 layer (``ops.fold_dgrad_down2x_weights``)."""
+        return self._derived.get(self.weight, lambda: ops.fold_dgrad_down2x_weights(self.weight.detach()), key="dgrad_down2x")
+
+    def uses_kernel(self, x: torch.Tensor) -> bool:
+        """Whether ``fused`` runs this layer on the wgmma implicit-GEMM kernel for input x."""
+        return (USE_CONV_KERNEL and x.is_contiguous(memory_format=torch.channels_last)
+                and ops.conv2d_supported(x, self.weight, self.stride[0], self.padding[0]))
+
+    def fused(self, x: torch.Tensor, add_bc: Optional[torch.Tensor] = None,
+              residual: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``self(x) [+ add_bc[:, :, None, None]] [+ residual]`` -- on the wgmma implicit-GEMM kernel when the layer
+        qualifies (``uses_kernel``), else on the library convolution."""
+        if self.uses_kernel(x):
+            if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
+                residual = residual.contiguous(memory_format=torch.channels_last)
+            return ops.conv2d(x, self.weight_khwc(), self.bias, self.stride[0], self.padding[0], add_bc=add_bc,
+                              residual=residual)
+        h = self(x)
+        if add_bc is not None:
+            h = h + add_bc[:, :, None, None]
+        return h if residual is None else h + residual
+
 
 def _conv(mod: Conv2d, x: torch.Tensor, add_bc: Optional[torch.Tensor] = None,
           residual: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``mod(x) [+ add_bc[:, :, None, None]] [+ residual]`` -- on the wgmma implicit-GEMM kernel when the layer
-    qualifies (ops.conv2d_supported), else on the library convolution."""
-    stride, pad = mod.stride[0], mod.padding[0]
-    if USE_CONV_KERNEL and x.is_contiguous(memory_format=torch.channels_last) and ops.conv2d_supported(x, mod.weight, stride, pad):
-        if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
-            residual = residual.contiguous(memory_format=torch.channels_last)
-        return ops.conv2d(x, mod.weight_khwc(), mod.bias, stride, pad, add_bc=add_bc, residual=residual)
-    h = mod(x)
-    if add_bc is not None:
-        h = h + add_bc[:, :, None, None]
-    return h if residual is None else h + residual
+    """``mod.fused(x, add_bc, residual)``; under autograd a layer on the kernel goes through ``ConvFunction`` (same
+    forward, dx and d residual in the backward)."""
+    if _records(x, residual, add_bc, mod.weight, mod.bias) and mod.uses_kernel(x):
+        from . import autograd_ops
+        return autograd_ops.conv(x, mod, add_bc, residual)
+    return mod.fused(x, add_bc, residual)
 
 
 def timestep_embedding(timesteps: torch.Tensor, dim: int, max_period: int = 10000) -> torch.Tensor:
@@ -127,6 +170,9 @@ class Attention(nn.Module):
         q = self.to_q(x).view(B, T, self.heads, self.dim_head)
         k = self.to_k(ctx).view(B, ctx.shape[1], self.heads, self.dim_head)
         v = self.to_v(ctx).view(B, ctx.shape[1], self.heads, self.dim_head)
+        if _records(q, k, v):          # LSE forward on the same wgmma kernel, general (hd 64, non-causal) backward
+            from . import autograd_ops
+            return self.to_out[0](autograd_ops.attention_general(q, k, v))
         return self.to_out[0](ops.attention(q, k, v, causal=False))
 
 
@@ -138,6 +184,9 @@ class GEGLU(nn.Module):
     def forward(self, x):
         hg = self.proj(x)
         if hg.is_cuda and hg.dtype != torch.float64 and (hg.shape[-1] // 2 * hg.element_size()) % 16 == 0:
+            if _records(hg):
+                from . import autograd_ops
+                return autograd_ops.geglu(hg)
             return ops.geglu(hg.contiguous())
         h, gate = hg.chunk(2, dim=-1)
         return h * F.gelu(gate)
@@ -164,6 +213,9 @@ class BasicTransformerBlock(nn.Module):
 
     @staticmethod
     def _ln(mod, x):
+        if _records(x, mod.weight, mod.bias):
+            from . import autograd_ops
+            return autograd_ops.layernorm(x, mod.weight, mod.bias, mod.eps)
         return ops.layernorm(x.contiguous(), mod.weight, mod.bias, mod.eps)
 
     def forward(self, x, context):
@@ -296,6 +348,17 @@ class UNet2DConditionModel(nn.Module):
 
     def forward(self, sample, timestep, encoder_hidden_states, mmfs_features: Optional[List[torch.Tensor]] = None,
                 mmfs_mask: Optional[torch.Tensor] = None, mmfs_module=None):
+        """Under autograd the gradient reaches ``encoder_hidden_states``, the MMFS hook and ``mmfs_features``; the
+        UNet's own weights must be frozen (``unet.requires_grad_(False)``)."""
+        if torch.is_grad_enabled() and has_trainable_weights(self):
+            raise RuntimeError("UNet2DConditionModel.forward under autograd: the UNet's own weights have no backward here "
+                               "(the image loss trains what feeds the UNet: the context, the MMFS hook and the features); "
+                               "freeze them with unet.requires_grad_(False), or run under torch.no_grad()")
+        if (self.conv_in.weight.is_cuda and self.conv_in.weight.dtype not in (torch.bfloat16, torch.float16)
+                and _records(sample, encoder_hidden_states, *(mmfs_features if isinstance(mmfs_features, (list, tuple)) else ()),
+                             *(mmfs_module.parameters() if isinstance(mmfs_module, nn.Module) else ()))):
+            from .llama_mmfs import check_training_dtype       # fail before the forward, not in loss.backward()
+            check_training_dtype("UNet2DConditionModel.forward under autograd", self.conv_in.weight)
         if not torch.is_tensor(timestep):
             timestep = torch.tensor([timestep], device=sample.device)
         t = timestep.reshape(-1).expand(sample.shape[0])
