@@ -1,8 +1,16 @@
-"""Autograd Functions over the decoder-layer kernels: the training path of the Llama decoder's self-attention layer,
-of the visual tokenizer, and of the image loss through the frozen SD UNet.
+"""The switch between the inference path and the training path, and the autograd Functions of the training path: the
+Llama decoder's self-attention layer, the visual tokenizer, and the image loss through the frozen SD UNet.
 
-Each forward runs the same sm_90a kernel as the inference wrapper in ops.py (a Function's forward runs with grad
-disabled, so the wrappers' ``inference_only`` guard does not fire there) and saves what its backward kernel reads:
+The entry points at the bottom (``layernorm``, ``rmsnorm``, ``swiglu``, ``geglu``, ``quick_gelu``, ``resize_bilinear``,
+``attention``, ``attention_general``, ``group_norm_nhwc``, ``conv``) are the one call a model module makes for the op.
+Each decides the path itself: unless autograd records the call (``msda.records``: grad mode on and a tensor argument or
+a parameter requires grad) it makes the inference call -- the ops.py kernel, or the torch expression the inference
+code computes -- and otherwise it refuses a dtype its backward kernels do not take (``check_training_dtype``, before
+any work rather than in ``loss.backward()``) and applies the Function.  ``rope_qkv`` is Function-only: its one caller
+is the Llama training forward.
+
+Each Function's forward runs the same sm_90a kernel as the inference wrapper in ops.py (a Function's forward runs with
+grad disabled, so the wrappers' ``inference_only`` guard does not fire there) and saves what its backward kernel reads:
 
 * ``RMSNormFunction``   -- ``mmfs_rmsnorm`` / ``mmfs_rmsnorm_backward`` (dweight only when the weight needs a gradient);
 * ``RoPEQKVFunction``   -- ``mmfs_rope_qk`` out of place on the (B, T, 3, H, hd) QKV projection output; the backward
@@ -25,9 +33,10 @@ disabled, so the wrappers' ``inference_only`` guard does not fire there) and sav
   frozen affine parameters;
 * ``GEGLUFunction`` -- ``mmfs_geglu`` / ``mmfs_geglu_backward`` on the [value | gate] buffer.
 
-The backward kernels take bf16 / fp16 only (the GroupNorm backward fp32 too), the causal attention backward head dim 128 without a KV cache and the
-general one head dim 64 or 128; other inputs are refused with the library's message.  Double backward is not
-supported.
+The backward kernels take bf16 / fp16 only, except the GroupNorm backward and the convolution's data gradient (cuDNN
+where the kernels do not apply), which take fp32 too; the causal attention backward takes head dim 128 without a KV
+cache and the general one head dim 64 or 128, other head dims are refused with the library's message.  Double
+backward is not supported.
 """
 from __future__ import annotations
 
@@ -37,6 +46,13 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from . import ops
+from .msda import records
+
+
+def check_training_dtype(what, t):
+    if t.dtype not in (torch.bfloat16, torch.float16):
+        raise RuntimeError(f"{what}: the backward kernels take bf16 / fp16 only (got {t.dtype}); cast the model, or run "
+                           "under torch.no_grad()")
 
 
 class RMSNormFunction(Function):
@@ -257,7 +273,10 @@ class GEGLUFunction(Function):
 
 
 def rmsnorm(x, weight, eps):
-    return RMSNormFunction.apply(x, weight, eps)
+    if not records(x, weight):
+        return ops.rmsnorm(x.contiguous(), weight, eps)
+    check_training_dtype("rmsnorm", x)
+    return RMSNormFunction.apply(x, weight.to(x.dtype), eps)
 
 
 def rope_qkv(qkv, cos, sin, position_ids):
@@ -265,36 +284,62 @@ def rope_qkv(qkv, cos, sin, position_ids):
 
 
 def attention(qkv, key_mask=None, scale=None, causal=True):
+    if not records(qkv):
+        return ops.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], key_mask=key_mask, scale=scale, causal=causal)
+    check_training_dtype("attention", qkv)
     return AttentionFunction.apply(qkv, key_mask, float(scale if scale is not None else qkv.shape[-1] ** -0.5), causal)
 
 
 def swiglu(gate_up):
+    if not records(gate_up):
+        return ops.swiglu(gate_up)
+    check_training_dtype("swiglu", gate_up)
     return SwiGLUFunction.apply(gate_up)
 
 
 def layernorm(x, weight, bias, eps):
+    if not records(x, weight, bias):
+        return ops.layernorm(x.contiguous(), weight, bias, eps)
+    check_training_dtype("layernorm", x)
     return LayerNormFunction.apply(x, weight, bias, eps)
 
 
 def attention_general(q, k, v, key_mask=None, scale=None):
+    if not records(q, k, v):
+        return ops.attention(q.contiguous(), k.contiguous(), v.contiguous(), key_mask=key_mask, scale=scale,
+                             causal=False)
+    check_training_dtype("attention_general", q)
     return GeneralAttentionFunction.apply(q, k, v, key_mask, float(scale if scale is not None else q.shape[-1] ** -0.5))
 
 
 def quick_gelu(h):
+    if not records(h):
+        return h * torch.sigmoid(1.702 * h)
+    check_training_dtype("quick_gelu", h)
     return QuickGELUFunction.apply(h)
 
 
 def resize_bilinear(x, scale_factor):
+    if not records(x):
+        return F.interpolate(x, scale_factor=scale_factor, mode="bilinear", align_corners=False)
+    check_training_dtype("resize_bilinear", x)
     return ResizeBilinearFunction.apply(x, scale_factor)
 
 
 def conv(x, conv_module, add_bc=None, residual=None):
+    if not records(x, residual, add_bc, conv_module):
+        return conv_module.fused(x, add_bc, residual)
     return ConvFunction.apply(x, residual, conv_module, add_bc)
 
 
 def group_norm_nhwc(x, groups, weight=None, bias=None, eps=1e-5, silu=False):
+    if not records(x, weight, bias):
+        return ops.group_norm_nhwc(x, groups, weight, bias, eps, silu=silu)
     return GroupNormNHWCFunction.apply(x, weight, bias, groups, float(eps), bool(silu))
 
 
 def geglu(value_gate):
+    if not records(value_gate):
+        return ops.geglu(value_gate.contiguous())
+    check_training_dtype("geglu", value_gate)
     return GEGLUFunction.apply(value_gate)

@@ -14,7 +14,10 @@ the forward is built for H100:
 * the MMFS cross-attention uses the fused sampler (mmfs.py); RMSNorm(vision) and
   value_proj(vision) are computed once per vision tensor and reused by every decode step
   (the reference recomputes both at each of the 10 cross layers at every generated token,
-  SURVEY.md 3.2).
+  SURVEY.md 3.2);
+* the same modules carry the text loss's training path: RMSNorm, SwiGLU and attention go through the entry points of
+  autograd_ops.py, which take the autograd Functions when autograd records the call and the inference kernels
+  otherwise; ``LlamaAttention`` and ``LlamaMMFSAttention`` switch to their training forwards on ``msda.records``.
 
 Plain library GEMMs (cuBLAS via torch) are used for the dense linears.
 """
@@ -34,6 +37,7 @@ import torch.utils.checkpoint
 from . import autograd_ops, ops
 from ._cache import SourceCache, WeightCache
 from .mmfs import MMFS
+from .msda import records
 
 
 @dataclass
@@ -55,28 +59,6 @@ class LlamaMMFSConfig:
     use_cache: bool = True
 
 
-def records_grad(module, *tensors) -> bool:
-    """Whether autograd records this call: grad mode is on and an input or a parameter of ``module`` requires grad.
-    Only then do the modules below take their training path (autograd_ops); otherwise they run the inference kernels."""
-    if not torch.is_grad_enabled():
-        return False
-    return (any(t is not None and torch.is_tensor(t) and t.requires_grad for t in tensors)
-            or any(p.requires_grad for p in module.parameters()))
-
-
-def check_training_dtype(what, t):
-    if t.dtype not in (torch.bfloat16, torch.float16):
-        raise RuntimeError(f"{what}: the backward kernels take bf16 / fp16 only (got {t.dtype}); cast the model, or run "
-                           "under torch.no_grad()")
-
-
-def _cat_weight(cat, linears):
-    """The concatenated weight, differentiable when a source weight is trainable (the cached copy is built without grad)."""
-    if any(l.weight.requires_grad for l in linears):
-        return torch.cat([l.weight for l in linears], 0)
-    return cat.get()
-
-
 class LlamaRMSNorm(nn.Module):
     def __init__(self, hidden_size, eps=1e-6):
         super().__init__()
@@ -84,10 +66,7 @@ class LlamaRMSNorm(nn.Module):
         self.variance_epsilon = eps
 
     def forward(self, hidden_states):
-        if records_grad(self, hidden_states):
-            check_training_dtype("LlamaRMSNorm", hidden_states)
-            return autograd_ops.rmsnorm(hidden_states, self.weight.to(hidden_states.dtype), self.variance_epsilon)
-        return ops.rmsnorm(hidden_states.contiguous(), self.weight, self.variance_epsilon)
+        return autograd_ops.rmsnorm(hidden_states, self.weight, self.variance_epsilon)
 
 
 def rotary_tables(dim: int, max_pos: int, base: float = 10000.0, device=None):
@@ -119,7 +98,8 @@ def shared_rotary_tables(dim: int, need_pos: int, min_pos: int, device):
 
 
 class _CatWeight:
-    """Concatenation of several Linear weights along the output dim, rebuilt when a source changes."""
+    """Concatenation of several Linear weights along the output dim, rebuilt when a source changes; differentiable, and
+    not cached, when autograd records a source weight (the cached copy is built without grad)."""
 
     def __init__(self, *linears):
         self.linears = linears
@@ -127,6 +107,8 @@ class _CatWeight:
 
     def get(self):
         ws = [l.weight for l in self.linears]
+        if records(*ws):
+            return torch.cat(ws, 0)
         return self._cache.get(ws, lambda: torch.cat(ws, 0).contiguous())
 
 
@@ -153,14 +135,8 @@ class LlamaMLP(nn.Module):
 
     def forward(self, x, residual=None, inplace=False):
         """``inplace``: accumulate into ``residual``'s storage (beta = 1 GEMM epilogue, no copy of the stream)."""
-        if records_grad(self, x, residual):
-            check_training_dtype("LlamaMLP", x)
-            act = autograd_ops.swiglu(F.linear(x, _cat_weight(self._gate_up, (self.gate_proj, self.up_proj))))
-            if residual is None:
-                return self.down_proj(act)
-            return _addmm_residual(residual, act, self.down_proj.weight, False)
         gu = F.linear(x, self._gate_up.get())                 # [gate | up] in one GEMM
-        act = ops.swiglu(gu)
+        act = autograd_ops.swiglu(gu)
         if residual is None:
             return self.down_proj(act)
         return _addmm_residual(residual, act, self.down_proj.weight, inplace)
@@ -239,7 +215,7 @@ class LlamaAttention(nn.Module):
             raise NotImplementedError("attention probabilities are never materialised by the fused kernel")
         B, T, _ = hidden_states.shape
         H, hd = self.num_heads, self.head_dim
-        if records_grad(self, hidden_states, residual):
+        if records(hidden_states, residual, self):
             return self._forward_training(hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual)
         qkv = F.linear(hidden_states, self._qkv.get()).view(B, T, 3, H, hd)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
@@ -284,13 +260,12 @@ class LlamaAttention(nn.Module):
         if past_key_value is not None or use_cache:
             raise RuntimeError("LlamaAttention under autograd runs the prefill without a KV cache: pass use_cache=False "
                                "and no past_key_values, or run under torch.no_grad()")
-        check_training_dtype("LlamaAttention", hidden_states)
+        autograd_ops.check_training_dtype("LlamaAttention", hidden_states)
         if self.head_dim != 128:
             raise RuntimeError(f"LlamaAttention under autograd needs head dim 128 (the attention backward kernel's), "
                                f"got {self.head_dim}")
         B, T, _ = hidden_states.shape
-        w = _cat_weight(self._qkv, (self.q_proj, self.k_proj, self.v_proj))
-        qkv = F.linear(hidden_states, w).view(B, T, 3, self.num_heads, self.head_dim)
+        qkv = F.linear(hidden_states, self._qkv.get()).view(B, T, 3, self.num_heads, self.head_dim)
         if position_ids is None:
             position_ids = torch.arange(T, device=hidden_states.device)
         cos, sin = self.rope_tables(hidden_states.device, T)
@@ -352,7 +327,7 @@ class LlamaMMFSAttention(nn.Module):
         return self.attn.project_value(self.norm2(vision_hidden_states))
 
     def forward(self, hidden_states, vision_hidden_states=None, cross_attention_mask=None, residual=None, inplace=False):
-        if records_grad(self, hidden_states, residual, vision_hidden_states if torch.is_tensor(vision_hidden_states) else None):
+        if records(hidden_states, residual, vision_hidden_states, self):
             return self._forward_training(hidden_states, vision_hidden_states, cross_attention_mask, residual)
         h = self.norm1(hidden_states)
         value = None
@@ -477,9 +452,9 @@ class LlamaModel(nn.Module):
     def forward(self, input_ids=None, attention_mask=None, position_ids=None, past_key_values=None,
                 inputs_embeds=None, vision_hidden_states=None, cross_attention_mask=None, use_cache=None,
                 output_attentions=None, output_hidden_states=None, return_dict=None):
+        training = records(inputs_embeds, vision_hidden_states, self)   # an embedding lookup below records through self
         if use_cache is None:   # under autograd the default is no cache, as HF's training path forces it
-            grad = records_grad(self, inputs_embeds, vision_hidden_states if torch.is_tensor(vision_hidden_states) else None)
-            use_cache = False if grad else self.config.use_cache
+            use_cache = False if training else self.config.use_cache
         return_dict = True if return_dict is None else return_dict
         if output_attentions:
             raise NotImplementedError("attention probabilities are never materialised")
@@ -504,12 +479,11 @@ class LlamaModel(nn.Module):
                 raise ValueError(f"attention_mask should be of size {(B, past + T)}, but is {tuple(attention_mask.shape)}")
             key_mask = attention_mask.to(torch.uint8)
 
-        training = records_grad(self, inputs_embeds, vision_hidden_states if torch.is_tensor(vision_hidden_states) else None)
         if training:
             if use_cache or past_key_values is not None:
                 raise RuntimeError("LlamaModel under autograd runs the prefill without a KV cache: pass use_cache=False "
                                    "and no past_key_values, or run under torch.no_grad()")
-            check_training_dtype("LlamaModel", inputs_embeds)
+            autograd_ops.check_training_dtype("LlamaModel", inputs_embeds)
         hidden_states = inputs_embeds
         inplace = not torch.is_grad_enabled() and not output_hidden_states
         if inplace:                      # one private copy of the stream; every layer then accumulates into it

@@ -18,6 +18,7 @@ from torch import nn
 from . import generation
 from ._cache import WeightCache
 from .llama_mmfs import LlamaMMFSConfig, LlamaModel
+from .msda import records
 
 # special-token convention of the reference (mm_interleaved.py:33-39; custom_datasets/wds_utils.py:186-215 appends
 # "<|beginofimage|>" = 32000 and "<|image|>" = 32001 to the 32000 Llama ids)
@@ -173,7 +174,7 @@ class TextDecoder(nn.Module):
         return w, b
 
     def logits(self, hidden_states):
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if records(self):
             logits = self.head(hidden_states)                                              # :155-157 as written
             tail = logits[..., self.orig_txt_vocab_size:] + self.head_new(hidden_states)
             return torch.cat([logits[..., :self.orig_txt_vocab_size], tail], dim=-1)
@@ -662,7 +663,7 @@ class MMInterleaved(InterleavedForward):
         ``neg_prompt_embeds``, the MMFS hook, ``context_feat_proj`` and, through the context and the MMFS features, the
         LLM and the visual tokenizer.  A trainable CLIP ViT weight or, with the image loss on, a trainable UNet weight
         raises up front, as neither has a backward here."""
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if records(self):
             if any(p.requires_grad for n, p in self.visual_tokenizer.encoder.vision_model.named_parameters()
                    if not n.startswith("adapter")):
                 raise RuntimeError("MMInterleaved.forward under autograd: the visual tokenizer has no backward here "

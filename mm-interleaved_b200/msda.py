@@ -19,9 +19,19 @@ def _require(cond: bool, msg: str) -> None:
         raise RuntimeError(msg)
 
 
+def records(*args) -> bool:
+    """Whether autograd records a call on ``args``: grad mode is on and a tensor argument, or a parameter of an
+    ``nn.Module`` argument, requires grad (``None`` and other arguments never do).  Exactly then the entry points of
+    autograd_ops.py take their autograd Functions, and the inference kernels refuse to run (``inference_only``)."""
+    if not torch.is_grad_enabled():
+        return False
+    return any(any(p.requires_grad for p in a.parameters()) if isinstance(a, torch.nn.Module)
+               else torch.is_tensor(a) and a.requires_grad for a in args)
+
+
 def inference_only(name: str, *tensors) -> None:
     """None of the ctypes kernels is autograd-aware: refuse to run where a gradient would be silently dropped."""
-    if torch.is_grad_enabled() and any(t is not None and torch.is_tensor(t) and t.requires_grad for t in tensors):
+    if records(*tensors):
         raise RuntimeError(f"{name}: this kernel is inference-only (no autograd support); call it under torch.no_grad() "
                            "or detach its inputs / freeze its parameters")
 

@@ -12,7 +12,7 @@ unchanged.  Built for the denoise loop:
 * the per-pixel reference grid and the resized sin-cos position embedding are cached per query size;
 * sampling runs in the fused MMFS kernel (pixel-grid reference points, 2-D image mask).
 
-Under autograd (the image loss) a block runs ``_forward_differentiable`` instead: the LayerNorm Function on the
+Under autograd (the image loss) a block runs ``_forward_differentiable`` instead: ``autograd_ops.layernorm`` on the
 query and on the features (no feature cache), the frozen position embedding, ``MMFS.forward_differentiable`` on the
 pixel grid, then ``output_proj`` and the 1x1 ``conv`` as two maps -- the folded weight is inference-only.
 """
@@ -27,9 +27,10 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from . import ops
+from . import autograd_ops, ops
 from ._cache import SourceCache, WeightCache
 from .mmfs import MMFS
+from .msda import records
 
 
 def sincos_pos_embed_2d(embed_dim: int, grid_size: int) -> torch.Tensor:
@@ -124,12 +125,7 @@ class MMFSBlock(nn.Module):
         n = self.feat_norm                      # no memoisation here: the caller owns the result (PreparedSDFeatures)
         return self.mmfs.project_value(ops.layernorm(ms_feat.contiguous(), n.weight, n.bias, n.eps), cache=False)
 
-    def _records(self, sample, ms_feat) -> bool:
-        return torch.is_grad_enabled() and (sample.requires_grad or (ms_feat is not None and ms_feat.requires_grad)
-                                            or any(p.requires_grad for p in self.parameters()))
-
     def _forward_differentiable(self, sample, ms_feat, ms_feat_mask, spatial_shapes):
-        from . import autograd_ops
         B, C, H, W = sample.shape
         n_images = ms_feat_mask.shape[-1]
         ref, ss, starts, pos = self._geometry(sample.device, sample.dtype, H, W, n_images, spatial_shapes)
@@ -144,7 +140,7 @@ class MMFSBlock(nn.Module):
     def forward(self, sample, ms_feat, ms_feat_mask, spatial_shapes, value=None):
         """sample (B, C_q, H, W); ms_feat (B, N, sum(H_l*W_l), C_v); ms_feat_mask (B, N); returns the residual (B, C_q, H, W).
         ``value`` (extension): ``project_features(ms_feat)`` computed by the caller (``ms_feat`` is then not read)."""
-        if value is None and self._records(sample, ms_feat):
+        if value is None and records(sample, ms_feat, self):
             return self._forward_differentiable(sample, ms_feat, ms_feat_mask, spatial_shapes)
         B, C, H, W = sample.shape
         n_images = ms_feat_mask.shape[-1]
@@ -215,8 +211,7 @@ class MMFSNet(nn.Module):
         """``mmfs_features``: the list of feature maps (reference signature) or a ``PreparedSDFeatures`` (extension)."""
         assert len(down_block_res_samples) == len(self.mmfs_down_blocks)
         if isinstance(mmfs_features, PreparedSDFeatures):
-            if torch.is_grad_enabled() and (any(t.requires_grad for t in (sample, *down_block_res_samples))
-                                            or any(p.requires_grad for p in self.parameters())):
+            if records(sample, *down_block_res_samples, self):
                 raise RuntimeError("MMFSNet.forward under autograd: a PreparedSDFeatures was built under no_grad and "
                                    "would cut the gradient to the feature maps and the feature-side weights; pass the "
                                    "list of feature maps instead")

@@ -19,12 +19,12 @@ ResNet block's time-embedding add and residual add fused into its epilogue; Grou
 (csrc/groupnorm_nhwc_sm100.cu) because torch's CUDA group_norm returns NCHW and would force a layout round trip
 around every convolution.
 
-Training path (the image loss): when autograd records, the convolutions, GroupNorms, GEGLUs, attentions and
-LayerNorms switch to the Functions of autograd_ops.py, whose forwards run the same kernels as the inference path and
-whose backwards carry the gradient to the UNet's inputs -- the context, the MMFS hook and what feeds them.  The UNet's
-own weights get no gradient here: ``UNet2DConditionModel.forward`` under autograd raises while any of them requires
-grad.  Nearest upsampling, ``cat``, the linears and ``conv_in`` / ``conv_out`` (library convolutions) stay on PyTorch
-autograd.
+Training path (the image loss): the convolutions on the kernel, GroupNorms, GEGLUs, attentions and LayerNorms call
+the entry points of autograd_ops.py, which take the autograd Functions when autograd records the call; their forwards
+run the same kernels as the inference path and their backwards carry the gradient to the UNet's inputs -- the context,
+the MMFS hook and what feeds them.  The UNet's own weights get no gradient here: ``UNet2DConditionModel.forward`` under
+autograd raises while any of them requires grad.  Nearest upsampling, ``cat``, the linears and ``conv_in`` /
+``conv_out`` (library convolutions) stay on PyTorch autograd.
 """
 from __future__ import annotations
 
@@ -35,15 +35,11 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from . import ops
+from . import autograd_ops, ops
 from ._cache import WeightCache
+from .msda import records
 
 USE_CONV_KERNEL = True      # tests flip this to compare against the cuDNN path on the same weights
-
-
-def _records(*tensors) -> bool:
-    """Whether autograd records an op on these tensors (the training path's switch)."""
-    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
 
 
 def has_trainable_weights(unet: nn.Module) -> bool:
@@ -55,10 +51,7 @@ def has_trainable_weights(unet: nn.Module) -> bool:
 def _gn(mod: nn.GroupNorm, x: torch.Tensor, silu: bool) -> torch.Tensor:
     """``silu(mod(x))`` / ``mod(x)`` kept in NHWC by this repo's kernel when x is channels-last on the GPU."""
     if USE_CONV_KERNEL and ops.group_norm_supported(x):
-        if _records(x, mod.weight, mod.bias):
-            from . import autograd_ops
-            return autograd_ops.group_norm_nhwc(x, mod.num_groups, mod.weight, mod.bias, mod.eps, silu=silu)
-        return ops.group_norm_nhwc(x, mod.num_groups, mod.weight, mod.bias, mod.eps, silu=silu)
+        return autograd_ops.group_norm_nhwc(x, mod.num_groups, mod.weight, mod.bias, mod.eps, silu=silu)
     h = mod(x)
     return F.silu(h) if silu else h
 
@@ -106,10 +99,9 @@ class Conv2d(nn.Conv2d):
 
 def _conv(mod: Conv2d, x: torch.Tensor, add_bc: Optional[torch.Tensor] = None,
           residual: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``mod.fused(x, add_bc, residual)``; under autograd a layer on the kernel goes through ``ConvFunction`` (same
-    forward, dx and d residual in the backward)."""
-    if _records(x, residual, add_bc, mod.weight, mod.bias) and mod.uses_kernel(x):
-        from . import autograd_ops
+    """``mod.fused(x, add_bc, residual)``; a layer on the kernel through ``autograd_ops.conv`` (under autograd: same
+    forward, dx and d residual in the backward), any other on the library convolution and PyTorch autograd."""
+    if mod.uses_kernel(x):
         return autograd_ops.conv(x, mod, add_bc, residual)
     return mod.fused(x, add_bc, residual)
 
@@ -170,10 +162,7 @@ class Attention(nn.Module):
         q = self.to_q(x).view(B, T, self.heads, self.dim_head)
         k = self.to_k(ctx).view(B, ctx.shape[1], self.heads, self.dim_head)
         v = self.to_v(ctx).view(B, ctx.shape[1], self.heads, self.dim_head)
-        if _records(q, k, v):          # LSE forward on the same wgmma kernel, general (hd 64, non-causal) backward
-            from . import autograd_ops
-            return self.to_out[0](autograd_ops.attention_general(q, k, v))
-        return self.to_out[0](ops.attention(q, k, v, causal=False))
+        return self.to_out[0](autograd_ops.attention_general(q, k, v))
 
 
 class GEGLU(nn.Module):
@@ -184,10 +173,7 @@ class GEGLU(nn.Module):
     def forward(self, x):
         hg = self.proj(x)
         if hg.is_cuda and hg.dtype != torch.float64 and (hg.shape[-1] // 2 * hg.element_size()) % 16 == 0:
-            if _records(hg):
-                from . import autograd_ops
-                return autograd_ops.geglu(hg)
-            return ops.geglu(hg.contiguous())
+            return autograd_ops.geglu(hg)
         h, gate = hg.chunk(2, dim=-1)
         return h * F.gelu(gate)
 
@@ -211,17 +197,11 @@ class BasicTransformerBlock(nn.Module):
         self.norm3 = nn.LayerNorm(dim)
         self.ff = FeedForward(dim)
 
-    @staticmethod
-    def _ln(mod, x):
-        if _records(x, mod.weight, mod.bias):
-            from . import autograd_ops
-            return autograd_ops.layernorm(x, mod.weight, mod.bias, mod.eps)
-        return ops.layernorm(x.contiguous(), mod.weight, mod.bias, mod.eps)
-
     def forward(self, x, context):
-        x = x + self.attn1(self._ln(self.norm1, x))
-        x = x + self.attn2(self._ln(self.norm2, x), context)
-        return x + self.ff(self._ln(self.norm3, x))
+        n1, n2, n3 = self.norm1, self.norm2, self.norm3
+        x = x + self.attn1(autograd_ops.layernorm(x, n1.weight, n1.bias, n1.eps))
+        x = x + self.attn2(autograd_ops.layernorm(x, n2.weight, n2.bias, n2.eps), context)
+        return x + self.ff(autograd_ops.layernorm(x, n3.weight, n3.bias, n3.eps))
 
 
 class Transformer2DModel(nn.Module):
@@ -354,11 +334,10 @@ class UNet2DConditionModel(nn.Module):
             raise RuntimeError("UNet2DConditionModel.forward under autograd: the UNet's own weights have no backward here "
                                "(the image loss trains what feeds the UNet: the context, the MMFS hook and the features); "
                                "freeze them with unet.requires_grad_(False), or run under torch.no_grad()")
-        if (self.conv_in.weight.is_cuda and self.conv_in.weight.dtype not in (torch.bfloat16, torch.float16)
-                and _records(sample, encoder_hidden_states, *(mmfs_features if isinstance(mmfs_features, (list, tuple)) else ()),
-                             *(mmfs_module.parameters() if isinstance(mmfs_module, nn.Module) else ()))):
-            from .llama_mmfs import check_training_dtype       # fail before the forward, not in loss.backward()
-            check_training_dtype("UNet2DConditionModel.forward under autograd", self.conv_in.weight)
+        feats = mmfs_features if isinstance(mmfs_features, (list, tuple)) else ()
+        if self.conv_in.weight.is_cuda and records(sample, encoder_hidden_states, *feats, mmfs_module):
+            # fail before the forward, not in loss.backward()
+            autograd_ops.check_training_dtype("UNet2DConditionModel.forward under autograd", self.conv_in.weight)
         if not torch.is_tensor(timestep):
             timestep = torch.tensor([timestep], device=sample.device)
         t = timestep.reshape(-1).expand(sample.shape[0])

@@ -28,20 +28,10 @@ from torch import nn
 
 from . import autograd_ops
 from . import msda as _msda
-from . import ops
 from ._cache import WeightCache
-from .llama_mmfs import check_training_dtype, records_grad
 from .functions import MSDeformAttnFunction
+from .msda import records
 from .sd_mmfs import resize_abs_pos, sincos_pos_embed_2d
-
-
-def _ln(mod: nn.LayerNorm, x):
-    """``mod(x)`` on the LayerNorm kernel; through its autograd Function when autograd records the call (the trainable
-    Q-Former head), otherwise on the inference path."""
-    if records_grad(mod, x):
-        check_training_dtype("LayerNorm", x)
-        return autograd_ops.layernorm(x, mod.weight, mod.bias, mod.eps)
-    return ops.layernorm(x.contiguous(), mod.weight, mod.bias, mod.eps)
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -100,18 +90,14 @@ class CLIPAttention(nn.Module):
         (the gradient of a trainable ViT-Adapter crosses the frozen CLIP layers): forward with the row log-sum-exp and
         the general attention backward into one (B, T, 3, H, hd) gradient, so the fused projection's backward is one
         GEMM.  The q / k / v weights are read through a cache built without grad, so they must be frozen there."""
+        if records(self.q_proj, self.k_proj, self.v_proj):
+            raise RuntimeError("CLIPAttention: the CLIP q / k / v projections have no weight gradient here (the "
+                               "reference freezes the CLIP ViT); freeze them, e.g. with "
+                               "VisualTokenizer.freeze_like_reference(), or run under torch.no_grad()")
         B, T, _ = x.shape
         w, b = self._fused()
         qkv = F.linear(x, w, b).view(B, T, 3, self.num_heads, self.head_dim)
-        if records_grad(self, x):
-            if any(m.weight.requires_grad or m.bias.requires_grad for m in (self.q_proj, self.k_proj, self.v_proj)):
-                raise RuntimeError("CLIPAttention: the CLIP q / k / v projections have no weight gradient here (the "
-                                   "reference freezes the CLIP ViT); freeze them, e.g. with "
-                                   "VisualTokenizer.freeze_like_reference(), or run under torch.no_grad()")
-            check_training_dtype("CLIPAttention", x)
-            return self.out_proj(autograd_ops.attention(qkv, causal=False))
-        ctx = ops.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], causal=False)
-        return self.out_proj(ctx)
+        return self.out_proj(autograd_ops.attention(qkv, causal=False))
 
 
 class CLIPMLP(nn.Module):
@@ -121,11 +107,7 @@ class CLIPMLP(nn.Module):
         self.fc2 = nn.Linear(config.intermediate_size, config.hidden_size)
 
     def forward(self, x):
-        h = self.fc1(x)
-        if records_grad(self, x):                                                   # same bits, backward on our kernel
-            check_training_dtype("CLIPMLP", h)
-            return self.fc2(autograd_ops.quick_gelu(h))
-        return self.fc2(h * torch.sigmoid(1.702 * h))                               # quick_gelu
+        return self.fc2(autograd_ops.quick_gelu(self.fc1(x)))
 
 
 class CLIPEncoderLayer(nn.Module):
@@ -137,8 +119,9 @@ class CLIPEncoderLayer(nn.Module):
         self.layer_norm2 = nn.LayerNorm(config.hidden_size, eps=config.layer_norm_eps)
 
     def forward(self, x):
-        x = x + self.self_attn(_ln(self.layer_norm1, x))
-        return x + self.mlp(_ln(self.layer_norm2, x))
+        n1, n2 = self.layer_norm1, self.layer_norm2
+        x = x + self.self_attn(autograd_ops.layernorm(x, n1.weight, n1.bias, n1.eps))
+        return x + self.mlp(autograd_ops.layernorm(x, n2.weight, n2.bias, n2.eps))
 
 
 class CLIPEncoder(nn.Module):
@@ -196,7 +179,7 @@ class MSDeformAttn(nn.Module):
             raise NotImplementedError("box reference points are not used on this path")
         normalizer = torch.stack([input_spatial_shapes[..., 1], input_spatial_shapes[..., 0]], -1)
         loc = reference_points[:, :, None, :, None, :] + off / normalizer[None, None, None, :, None, :]
-        if records_grad(self, query, input_flatten):        # deterministic backward to value, loc and attention weights
+        if records(query, input_flatten, self):             # deterministic backward to value, loc and attention weights
             out = MSDeformAttnFunction.apply(value, input_spatial_shapes.contiguous(), input_level_start_index.contiguous(),
                                              loc.to(value.dtype), aw.to(value.dtype), self.im2col_step)
             return self.output_proj(out)
@@ -215,12 +198,7 @@ class ChannelsFirstLayerNorm(nn.Module):
         self.eps = eps
 
     def forward(self, x):
-        B, C, H, W = x.shape
-        if records_grad(self, x):
-            check_training_dtype("ChannelsFirstLayerNorm", x)
-            return autograd_ops.layernorm(x.permute(0, 2, 3, 1), self.weight, self.bias, self.eps).permute(0, 3, 1, 2)
-        y = ops.layernorm(x.permute(0, 2, 3, 1).contiguous(), self.weight, self.bias, self.eps)
-        return y.permute(0, 3, 1, 2)
+        return autograd_ops.layernorm(x.permute(0, 2, 3, 1), self.weight, self.bias, self.eps).permute(0, 3, 1, 2)
 
 
 class SpatialPriorModule(nn.Module):
@@ -290,10 +268,13 @@ class Extractor(nn.Module):
             self.ffn_norm = nn.LayerNorm(dim, eps=1e-6)
 
     def forward(self, query, reference_points, feat, spatial_shapes, level_start_index, H, W):
-        query = query + self.attn(_ln(self.query_norm, query), reference_points, _ln(self.feat_norm, feat),
-                                  spatial_shapes, level_start_index, None)
+        qn, fn = self.query_norm, self.feat_norm
+        query = query + self.attn(autograd_ops.layernorm(query, qn.weight, qn.bias, qn.eps), reference_points,
+                                  autograd_ops.layernorm(feat, fn.weight, fn.bias, fn.eps), spatial_shapes,
+                                  level_start_index, None)
         if self.with_cffn:
-            query = query + self.ffn(_ln(self.ffn_norm, query), H, W)
+            n = self.ffn_norm
+            query = query + self.ffn(autograd_ops.layernorm(query, n.weight, n.bias, n.eps), H, W)
         return query
 
 
@@ -306,8 +287,10 @@ class Injector(nn.Module):
         self.gamma = nn.Parameter(init_values * torch.ones(dim), requires_grad=True)
 
     def forward(self, query, reference_points, feat, spatial_shapes, level_start_index):
-        attn = self.attn(_ln(self.query_norm, query), reference_points, _ln(self.feat_norm, feat), spatial_shapes,
-                         level_start_index, None)
+        qn, fn = self.query_norm, self.feat_norm
+        attn = self.attn(autograd_ops.layernorm(query, qn.weight, qn.bias, qn.eps), reference_points,
+                         autograd_ops.layernorm(feat, fn.weight, fn.bias, fn.eps), spatial_shapes, level_start_index,
+                         None)
         return query + self.gamma * attn
 
 
@@ -357,15 +340,6 @@ def adapter_deform_inputs(h, w, device):
     return [_grid_points([(h // 16, w // 16)], device), ss1, st1], [_grid_points(s3, device), ss2, st2]
 
 
-def _resize(x, scale_factor):
-    """Bilinear resize of an adapter stage output; under autograd through the Function with the same forward bits and a
-    deterministic backward straight into the stage's token layout."""
-    if torch.is_grad_enabled() and x.requires_grad:
-        check_training_dtype("CLIPVisionTransformerAdapter", x)
-        return autograd_ops.resize_bilinear(x, scale_factor)
-    return F.interpolate(x, scale_factor=scale_factor, mode="bilinear", align_corners=False)
-
-
 class CLIPVisionTransformerAdapter(nn.Module):
     def __init__(self, config, conv_inplane=64, n_points=4):
         super().__init__()
@@ -391,7 +365,8 @@ class CLIPVisionTransformerAdapter(nn.Module):
         cfg = self.config
         hidden, H, W = self.embeddings(pixel_values)
         bs, n, dim = hidden.shape
-        hidden = _ln(self.pre_layrnorm, hidden)
+        pre = self.pre_layrnorm
+        hidden = autograd_ops.layernorm(hidden, pre.weight, pre.bias, pre.eps)
         new_size = cfg.image_size // cfg.patch_size * 16                              # vit_adapter_hf.py:113-114
         resized = F.interpolate(pixel_values, size=(new_size, new_size), mode="bilinear", align_corners=False)
         gkey = (new_size, pixel_values.device)
@@ -414,7 +389,9 @@ class CLIPVisionTransformerAdapter(nn.Module):
         c1 = self.adapter_up(c2) + c1
         x1, x2, x3, x4 = outs
         last_hidden = torch.cat([cls, x4.flatten(2).transpose(1, 2)], dim=1)
-        x1, x2, x4 = _resize(x1, 4), _resize(x2, 2), _resize(x4, 0.5)
+        x1 = autograd_ops.resize_bilinear(x1, 4)
+        x2 = autograd_ops.resize_bilinear(x2, 2)
+        x4 = autograd_ops.resize_bilinear(x4, 0.5)
         return SimpleNamespace(last_hidden_state=last_hidden, pooler_output=cls,
                                hidden_states=[c1 + x1, c2 + x2, c3 + x3, c4 + x4])
 
@@ -453,12 +430,11 @@ class QFormerAttention(nn.Module):
         k = self.key(kv).view(B, kv.shape[1], H, hd)
         v = self.value(kv).view(B, kv.shape[1], H, hd)
         if isinstance(self.q_norm, nn.LayerNorm):
-            q, k = _ln(self.q_norm, q), _ln(self.k_norm, k)
+            qn, kn = self.q_norm, self.k_norm
+            q = autograd_ops.layernorm(q, qn.weight, qn.bias, qn.eps)
+            k = autograd_ops.layernorm(k, kn.weight, kn.bias, kn.eps)
         km = None if (encoder_attention_mask is None or encoder_hidden_states is None) else encoder_attention_mask.to(torch.uint8).contiguous()
-        if records_grad(self, hidden_states, kv):       # training: forward with LSE, general attention backward
-            check_training_dtype("QFormerAttention", hidden_states)
-            return autograd_ops.attention_general(q, k, v, key_mask=km)
-        return ops.attention(q.contiguous(), k.contiguous(), v.contiguous(), key_mask=km, causal=False)   # scores / sqrt(hd), softmax, @ v
+        return autograd_ops.attention_general(q, k, v, key_mask=km)      # scores / sqrt(hd), softmax, @ v
 
 
 class _SelfOutput(nn.Module):
@@ -468,7 +444,8 @@ class _SelfOutput(nn.Module):
         self.LayerNorm = nn.LayerNorm(hidden, eps=eps)
 
     def forward(self, ctx, residual):
-        return _ln(self.LayerNorm, self.dense(ctx) + residual)
+        n = self.LayerNorm
+        return autograd_ops.layernorm(self.dense(ctx) + residual, n.weight, n.bias, n.eps)
 
 
 class _AttnBlock(nn.Module):
@@ -497,7 +474,8 @@ class _Output(nn.Module):
         self.LayerNorm = nn.LayerNorm(hidden, eps=eps)
 
     def forward(self, x, residual):
-        return _ln(self.LayerNorm, self.dense(x) + residual)
+        n = self.LayerNorm
+        return autograd_ops.layernorm(self.dense(x) + residual, n.weight, n.bias, n.eps)
 
 
 class QFormerLayer(nn.Module):
@@ -534,7 +512,8 @@ class Blip2QFormerModel(nn.Module):
         self.encoder = _QFormerEncoder(cfg)
 
     def forward(self, query_embeds, encoder_hidden_states, encoder_attention_mask=None):
-        x = _ln(self.layernorm, query_embeds)
+        n = self.layernorm
+        x = autograd_ops.layernorm(query_embeds, n.weight, n.bias, n.eps)
         for layer in self.encoder.layer:
             x = layer(x, encoder_hidden_states, encoder_attention_mask)
         return x
@@ -637,8 +616,9 @@ class VisualTokenizer(nn.Module):
             feats.append(f + pe.to(f.dtype).view(f.size(2), f.size(3), -1).permute(2, 0, 1))
         n = image_embed.size(1)
         pe = torch.cat([self.pos_embed[:1], self.abs_pos(n - 1)], 0).to(image_embed.dtype)
-        q_in = _ln(self.pos_ln, self.pos_proj(image_embed)) + pe                          # :85-87
+        pn, qn = self.pos_ln, self.post_ln
+        q_in = autograd_ops.layernorm(self.pos_proj(image_embed), pn.weight, pn.bias, pn.eps) + pe      # :85-87
         image_embed = image_embed + pe
-        q_in = _ln(self.post_ln, q_in)
+        q_in = autograd_ops.layernorm(q_in, qn.weight, qn.bias, qn.eps)
         vis = self.perceiver_resampler(encoder_hidden_states=q_in)[0]
         return dict(vis_embed=self.proj(vis), image_embeds=image_embed[:, 1:, :], multiscale_features=feats)
