@@ -495,6 +495,18 @@ int mmfs_kv_beam_reorder(void *cache, int n_caches, long cache_stride, int rows,
                          long row_bytes, int num_beams, const int64_t *parent, const int64_t *cur, const int64_t *step,
                          const uint8_t *done, int max_positions, void *stream);
 
+/*
+ * A generated image re-entering the context: (N, 3, S, S) fp32 images in [0, 1] (contiguous) to the visual tokenizer's
+ * (N, 3, R, R) fp32 input (contiguous), bit-identical to the host path tensor_to_pil -> center_crop_arr(R) -> float32
+ * / 255 of the reference's inference loop: the uint8 quantisation x * 255 + 0.5 (fp32, clamped to [0, 255],
+ * truncated), PIL's BOX halvings while the size is >= 2R, PIL's BICUBIC resize to R with its antialiasing support and
+ * 8-bit fixed-point passes (horizontal then vertical, each rounded and clipped), the (empty) centre crop, then u / 255
+ * in fp32.  One launch; two runs are bit-identical.  A NaN pixel quantises to 0.
+ * N < 0, non-positive C / H / W / R, N > 65535, null pointers with N > 0: MMFS_EINVAL.  C != 3, H != W, S or R above
+ * 16384, or a resize whose rows do not fit in shared memory: MMFS_EUNSUPPORTED.
+ */
+int mmfs_image_reentry(const float *images, float *out, int N, int C, int H, int W, int R, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

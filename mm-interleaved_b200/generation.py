@@ -4,7 +4,7 @@ the eager beam loop (HF 4.31 ``beam_search`` and ``beam_sample``), and the CUDA-
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import List
+from typing import List, Optional
 
 import torch
 
@@ -17,13 +17,23 @@ _BEAM_SAMPLE_TOP_K = 50              # transformers 4.31 GenerationConfig.top_k,
 @dataclass
 class Prompt:
     """What every decoding path needs from the call's inputs: the decoder inputs of the prompt, its (defaulted)
-    attention mask, its position ids and the eos ids as a list."""
+    attention mask, its position ids and the eos ids as a list.
+
+    A prompt may continue a cached prefix (``interleaved.InterleavedSession``): ``cache`` (one ``StaticKV`` per layer)
+    already holds its first ``prefix`` positions, so the prefill runs over the rest only, appending to ``cache``;
+    ``vision`` is the ``PreparedVision`` of ``feats`` when the caller keeps one, and ``hidden`` (B, >= L, C), when given,
+    receives the decoder's last hidden state of every prefilled position.  The decoding paths then start from the
+    cached prompt instead of an empty cache, and leave ``cache`` at the prompt's length."""
     mm_embeds: torch.Tensor
     cross: torch.Tensor
     feats: torch.Tensor
     attention_mask: torch.Tensor
     position_ids: torch.Tensor
     eos_ids: List[int]
+    cache: Optional[list] = None
+    prefix: int = 0
+    vision: Optional[PreparedVision] = None
+    hidden: Optional[torch.Tensor] = None
 
 
 def prepare_prompt(model, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, eos_token_id):
@@ -37,22 +47,28 @@ def prepare_prompt(model, text_ids, visual_output, num_image_per_seq, max_num_im
 
 
 def _prefill(model, p: Prompt, past, vision):
-    """The decoder over the whole prompt into the cache ``past``; returns (the cache, the last position's logits)."""
-    out = model.mm_decoder(inputs_embeds=p.mm_embeds, attention_mask=p.attention_mask, position_ids=p.position_ids,
-                           past_key_values=past, vision_hidden_states=vision, cross_attention_mask=p.cross,
-                           use_cache=True, return_dict=True)
+    """The decoder over the prompt's positions from ``p.prefix`` on into the cache ``past`` (which holds the ones
+    before); returns (the cache, the last position's logits)."""
+    s = p.prefix
+    out = model.mm_decoder(inputs_embeds=p.mm_embeds[:, s:], attention_mask=p.attention_mask,
+                           position_ids=p.position_ids[:, s:], past_key_values=past, vision_hidden_states=vision,
+                           cross_attention_mask=p.cross[:, s:], use_cache=True, return_dict=True)
+    if p.hidden is not None:
+        p.hidden[:, s:p.mm_embeds.shape[1]].copy_(out.last_hidden_state)
     return out.past_key_values, model.text_decoder.logits(out.last_hidden_state[:, -1:])
 
 
 def _prefill_beams(model, p: Prompt, rep, past, vision):
-    """The prompt prefilled ONCE per sequence, its cache rows copied to the beam rows of ``past`` (``rep``: beam row ->
-    prompt); returns the beam rows' last logits, attention mask, last position id and last cross-attention row."""
+    """The prompt prefilled ONCE per sequence (into ``p.cache`` after its prefix, else into a fresh cache), its cache rows
+    copied to the beam rows of ``past`` (``rep``: beam row -> prompt); returns the beam rows' last logits, attention
+    mask, last position id and last cross-attention row."""
     B, L, _ = p.mm_embeds.shape
-    pre = model.mm_decoder.static_cache(B, L, dtype=p.mm_embeds.dtype, device=p.mm_embeds.device)
+    pre = p.cache if p.cache is not None else \
+        model.mm_decoder.static_cache(B, L, dtype=p.mm_embeds.dtype, device=p.mm_embeds.device)
     _, logits = _prefill(model, p, pre, vision)
     for dst, src in zip(past, pre):                                     # a copy of the prompt rows, no recompute
-        dst.k[:, :L].copy_(src.k.index_select(0, rep))
-        dst.v[:, :L].copy_(src.v.index_select(0, rep))
+        dst.k[:, :L].copy_(src.k[:, :L].index_select(0, rep))
+        dst.v[:, :L].copy_(src.v[:, :L].index_select(0, rep))
         dst.length = L
     return (t.index_select(0, rep) for t in (logits, p.attention_mask, p.position_ids[:, -1:], p.cross[:, -1:, :]))
 
@@ -60,11 +76,17 @@ def _prefill_beams(model, p: Prompt, rep, past, vision):
 def generate_texts(model, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, max_new_tokens,
                    eos_token_id, pad_token_id, static_cache, min_length, repetition_penalty, use_nucleus_sampling, top_p,
                    temperature, generator, num_beams, length_penalty, num_return_sequences):
-    """``InterleavedForward.generate_texts``: one prompt setup, then the graphed decoder where
-    ``enable_decode_graphs`` is on and the kernels take the shape, else the eager loop."""
+    """``InterleavedForward.generate_texts``: one prompt setup, then ``decode``."""
     p = prepare_prompt(model, text_ids, visual_output, num_image_per_seq, max_num_image, attention_mask, eos_token_id)
+    return decode(model, p, max_new_tokens, pad_token_id, static_cache, min_length, repetition_penalty,
+                  use_nucleus_sampling, top_p, temperature, generator, num_beams, length_penalty, num_return_sequences)
+
+
+def decode(model, p: Prompt, max_new_tokens, pad_token_id, static_cache, min_length, repetition_penalty,
+           use_nucleus_sampling, top_p, temperature, generator, num_beams, length_penalty, num_return_sequences):
+    """The graphed decoder where ``enable_decode_graphs`` is on and the kernels take the shape, else the eager loop."""
     V = model.text_decoder.head.weight.shape[0]
-    graphs = (model._decode_graphs is not None and text_ids.is_cuda and max_new_tokens > 0 and
+    graphs = (model._decode_graphs is not None and p.mm_embeds.is_cuda and max_new_tokens > 0 and
               (not use_nucleus_sampling or model._decode_graph_sampling))
     sample, warp = use_nucleus_sampling, (temperature, top_p, generator)
     if num_beams > 1:
@@ -87,9 +109,12 @@ def token_loop(model, p: Prompt, max_new_tokens, pad_token_id, static_cache, min
     mm_embeds, attention_mask, eos_ids = p.mm_embeds, p.attention_mask, p.eos_ids
     B, L, _ = mm_embeds.shape
     # the image-only half of the 10 cross-attention layers, once per call (PreparedVision)
-    feats = model.mm_decoder.prepare_vision(p.feats)
+    feats = p.vision if p.vision is not None else model.mm_decoder.prepare_vision(p.feats)
     # pre-allocated per-layer caches appended in place (the reference's cat-per-token re-copies every layer's cache)
-    past = model.mm_decoder.static_cache(B, L + max_new_tokens, dtype=mm_embeds.dtype, device=mm_embeds.device) if static_cache else None
+    if p.cache is not None:
+        past = p.cache
+    else:
+        past = model.mm_decoder.static_cache(B, L + max_new_tokens, dtype=mm_embeds.dtype, device=mm_embeds.device) if static_cache else None
     past, logits = _prefill(model, p, past, feats)
     new_ids = []
     finished = torch.zeros((B,), dtype=torch.bool, device=mm_embeds.device)
@@ -125,6 +150,9 @@ def token_loop(model, p: Prompt, max_new_tokens, pad_token_id, static_cache, min
                                 cross_attention_mask=last_cross, use_cache=True, return_dict=True)
         past = step.past_key_values
         logits = model.text_decoder.logits(step.last_hidden_state)
+    if p.cache is not None:                                          # the generated positions are not kept
+        for c in p.cache:
+            c.length = L
     return torch.stack(new_ids, dim=1)
 
 
@@ -150,7 +178,7 @@ def beam_search(model, p: Prompt, max_new_tokens, pad_token_id, min_length, num_
     B = B0 * expand                                                            # independent beam searches
     rep = torch.arange(B0, device=dev).repeat_interleave(expand * nb)         # beam row -> prompt
     past = model.mm_decoder.static_cache(B * nb, L + max_new_tokens, dtype=mm_embeds.dtype, device=dev)
-    logits, mask, pos, last_cross = _prefill_beams(model, p, rep, past, p.feats)
+    logits, mask, pos, last_cross = _prefill_beams(model, p, rep, past, p.vision if p.vision is not None else p.feats)
     feats_b = p.feats.index_select(0, rep)
 
     beam_scores = torch.zeros((B, nb), dtype=torch.float32, device=dev)
@@ -432,7 +460,11 @@ class TokenDecoder(_GraphedDecoder):
         self._start_call(L, generator, repetition_penalty, temperature, top_p)
         o.mm_decoder.prepare_vision(p.feats, out=self.pv)                   # eager, into the static buffers the graph reads
         self._set_graph_mode(False, 0)
-        _, logits = _prefill(o, p, self.past, self.pv)                      # prefill straight into the static cache
+        if p.cache is None:
+            _, logits = _prefill(o, p, self.past, self.pv)                  # prefill straight into the static cache
+        else:                                                               # after a cached prefix: copy the prompt rows
+            rows = torch.arange(p.mm_embeds.shape[0], device=p.mm_embeds.device)
+            logits = next(_prefill_beams(o, p, rows, self.past, self.pv))
         logits0 = logits[:, -1].float()
         self._prefill_done(L, lambda: self._reset(L, p.attention_mask, p.position_ids, p.cross, logits0))
         for _ in range(self.max_new):

@@ -806,6 +806,25 @@ class MMInterleaved(InterleavedForward):
             scores.append((logp * options_attn_masks[i]).sum(dim=-1))
         return {"scores": torch.stack(scores, dim=0)[:, None, :]}
 
+    @torch.no_grad()
+    def generate_interleaved(self, text_ids, image_tensors, num_image_per_seq, attention_mask=None,
+                             generate_mode="generate_texts", num_iter=2, auto_end=False, force_gen_image_next=False,
+                             force_replace_gen_text=False, generator: Optional[torch.Generator] = None, **kwargs):
+        """Interleaved image-text generation of ONE sample (batch 1) in one call: the turn loop of the reference's
+        ``inference.py::inference_all`` (text turns as ``generate_texts``, image turns as ``generate_images``,
+        ``update_texts`` / ``update_image`` between them, ``auto_end``, ``force_gen_image_next``) on an
+        ``interleaved.InterleavedSession`` that keeps the KV cache, the hidden states and the tokenizer outputs across
+        turns, so every position is prefilled once and every image tokenized once, and re-enters each generated image
+        on the device (``ops.image_reentry``).  ``kwargs``: the generation keywords of ``mm_inference.yaml``
+        (``max_length``, ``min_length``, ``num_beams``, ``use_nucleus_sampling``, ``top_p``, ``temperature``,
+        ``repetition_penalty``, ``length_penalty``, ``guidance_scale``, ``num_inference_steps``,
+        ``num_validation_images``), ``max_cache_length`` (refuse samples that could outgrow it) and ``return_session``.
+        Needs an image decoder with a VAE decoder; ``force_replace_gen_text`` (a text tokenizer's job) raises.
+        Returns ``turns`` and the final ``text_ids``, ``attention_mask``, ``image_tensors``, ``num_image_per_seq``."""
+        from .interleaved import generate_interleaved
+        return generate_interleaved(self, text_ids, image_tensors, num_image_per_seq, attention_mask, generate_mode,
+                                    num_iter, auto_end, force_gen_image_next, force_replace_gen_text, generator, **kwargs)
+
     def generate(self, mode="generate_images", **kwargs):
         """mm_interleaved.py:745-763."""
         if mode in ("generate_images", "generate_segm"):

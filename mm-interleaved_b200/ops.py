@@ -585,6 +585,27 @@ def quick_gelu_backward(h: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
     return dh
 
 
+def image_reentry(images: torch.Tensor, size: int = 224, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """A generated (N, 3, S, S) fp32 image in [0, 1] as the visual tokenizer's (N, 3, size, size) fp32 input, on the
+    device and bit-identical to the reference's host path (``tensor_to_pil``, ``center_crop_arr``, ``/ 255``; see
+    csrc/image_reentry_sm100.cu).  ``out`` (contiguous, e.g. a slot of the sample's image tensor) receives the result.
+    Non-square or non-RGB images raise."""
+    _require(images.is_cuda and images.dim() == 4 and images.dtype == torch.float32,
+             "image_reentry: images must be a (N, 3, S, S) fp32 CUDA tensor")
+    images = images.contiguous()
+    N, C, H, W = images.shape
+    if out is None:
+        out = torch.empty((N, C, size, size), dtype=torch.float32, device=images.device)
+    _require(out.is_cuda and out.is_contiguous() and out.dtype == torch.float32 and out.device == images.device and
+             tuple(out.shape) == (N, C, size, size), "image_reentry: out must be a contiguous (N, 3, size, size) fp32 "
+             "tensor on the images' device")
+    with torch.cuda.device(images.device):
+        rc = _lib.lib().mmfs_image_reentry(images.data_ptr(), out.data_ptr(), N, C, H, W, int(size), _stream())
+    _lib.check(rc, "image_reentry")
+    launch_counter[0] += 1
+    return out
+
+
 def _pixel_stride(t: torch.Tensor):
     """The one stride that steps pixel p = y * W + x of a (B, C, H, W) tensor, or None when H and W are not laid out
     as one flattened pixel axis.  The stride of a size-1 dim is arbitrary in PyTorch and is not used."""
