@@ -507,6 +507,19 @@ int mmfs_kv_beam_reorder(void *cache, int n_caches, long cache_stride, int rows,
  */
 int mmfs_image_reentry(const float *images, float *out, int N, int C, int H, int W, int R, void *stream);
 
+/*
+ * Weight-only FP8 linear of a decode step: out = x * (w8 * scale)^T [+ bias] [+ residual], rounded once to x's type.
+ * x (M, K), bias (N), residual (M, N), out (M, N): contiguous, dtype MMFS_BF16 or MMFS_F16; w8 (N, K) contiguous
+ * float8 e4m3 (OCP "e4m3fn") bytes; scale (N) fp32, one per output channel.  bias and residual may be NULL; out may be
+ * residual (accumulated in place).  Products are exact in the MMA's 16-bit type, sums are fp32; the K slices of an
+ * output tile are reduced in a fixed order, so two calls give bit-identical outputs.  No workspace, no host
+ * synchronisation (capturable in a CUDA graph).  x and w8 must be 16-byte aligned.
+ * Non-positive M / N / K, null x / w8 / scale / out or misaligned x / w8: MMFS_EINVAL.  M > 64, K not a multiple of 16
+ * or another dtype: MMFS_EUNSUPPORTED.
+ */
+int mmfs_linear_fp8(const void *x, const uint8_t *w8, const float *scale, const void *bias, const void *residual,
+                    void *out, int M, int N, int K, int dtype, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -64,8 +64,10 @@ SIGNATURES = {
     "mmfs_beam_sample": (_I, [_P, _L] + [_P] * 14 + [_I, _L, _I, _I, _P] + [_I] * 4 + [_P]),
     "mmfs_kv_beam_reorder": (_I, [_P, _I, _L, _I, _L, _L, _L, _I] + [_P] * 4 + [_I, _P]),
     "mmfs_image_reentry": (_I, [_P, _P] + [_I] * 5 + [_P]),
+    "mmfs_linear_fp8": (_I, [_P] * 6 + [_I] * 4 + [_P]),
 }
 BEAM_MAX_BEAMS, BEAM_MAX_EOS = 8, 4                  # limits of mmfs_beam_select / mmfs_beam_sample / mmfs_kv_beam_reorder
+LINEAR_FP8_MAX_M = 64                                # rows of x mmfs_linear_fp8 takes
 RMSNORM_BWD_PARTS = 256                              # MMFS_RMSNORM_BWD_PARTS: dweight partial rows of mmfs_rmsnorm_backward
 
 

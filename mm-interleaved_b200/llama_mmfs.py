@@ -123,6 +123,29 @@ def _addmm_residual(residual, x, weight, inplace):
     return torch.addmm(r2, x2, weight.t()).view_as(residual)
 
 
+# Where ops.linear_fp8 beat the bf16 cuBLAS GEMM on an H100 80GB HBM3 at 700 W (tools/fp8_decode_bench.py, DESIGN.md
+# sections 4.9 and 6): at most 5 rows, and only the wide linears (N >= 2K: fused QKV, fused gate/up, the head).  At 20 rows and
+# on o_proj / down_proj it was slower, so those calls keep the 16-bit weights.
+FP8_DECODE_MAX_ROWS = 5
+
+
+def decode_linear(x, weight, fp8, key, bias=None, residual=None, inplace=False):
+    """``x @ weight^T [+ bias] [+ residual]``: the one place the decode-time linears (fused QKV, o_proj, fused gate/up,
+    down_proj, the folded text head) choose their weights.  ``fp8`` is the module's ``WeightCache`` of FP8 copies while
+    ``InterleavedForward.enable_fp8_decode`` is on, else None; ``key`` names the copy in it.  A decode-step call -- one
+    position per row (x is (B, 1, K)), at most ``FP8_DECODE_MAX_ROWS`` rows, autograd not recording -- of a wide linear
+    (N >= 2K, where the kernel wins) then runs ``ops.linear_fp8`` on the per-channel E4M3 copy of ``weight`` (``ops.quantize_fp8_per_channel``, built on first
+    use and rebuilt when ``weight`` changes).  Every other call runs the 16-bit GEMM: ``F.linear``, or with
+    ``residual`` the beta = 1 ``addmm`` (``inplace``: into ``residual``'s storage)."""
+    if (fp8 is not None and x.dim() == 3 and x.shape[1] == 1 and x.shape[0] <= FP8_DECODE_MAX_ROWS
+            and weight.shape[0] >= 2 * weight.shape[1] and not records(x, residual)):
+        w8, scale = fp8.get(weight, lambda: ops.quantize_fp8_per_channel(weight), key)
+        return ops.linear_fp8(x, w8, scale, bias, residual, out=residual if inplace else None)
+    if residual is None:
+        return F.linear(x, weight, bias)
+    return _addmm_residual(residual, x, weight, inplace)
+
+
 class LlamaMLP(nn.Module):
     def __init__(self, hidden_size: int, intermediate_size: int, hidden_act: str):
         super().__init__()
@@ -132,14 +155,13 @@ class LlamaMLP(nn.Module):
         self.down_proj = nn.Linear(intermediate_size, hidden_size, bias=False)
         self.up_proj = nn.Linear(hidden_size, intermediate_size, bias=False)
         self._gate_up = _CatWeight(self.gate_proj, self.up_proj)
+        self._fp8 = None                                       # FP8 decode copies (enable_fp8_decode)
 
     def forward(self, x, residual=None, inplace=False):
         """``inplace``: accumulate into ``residual``'s storage (beta = 1 GEMM epilogue, no copy of the stream)."""
-        gu = F.linear(x, self._gate_up.get())                 # [gate | up] in one GEMM
+        gu = decode_linear(x, self._gate_up.get(), self._fp8, "gate_up")       # [gate | up] in one GEMM
         act = autograd_ops.swiglu(gu)
-        if residual is None:
-            return self.down_proj(act)
-        return _addmm_residual(residual, act, self.down_proj.weight, inplace)
+        return decode_linear(act, self.down_proj.weight, self._fp8, "down", residual=residual, inplace=inplace)
 
 
 class StaticKV:
@@ -198,6 +220,7 @@ class LlamaAttention(nn.Module):
         self.o_proj = nn.Linear(self.hidden_size, self.hidden_size, bias=False)
         self._qkv = _CatWeight(self.q_proj, self.k_proj, self.v_proj)
         self._rope = None   # (device, max_pos, cos, sin)
+        self._fp8 = None    # FP8 decode copies (enable_fp8_decode)
 
     def rope_tables(self, device, need_pos):
         if self._rope is None or self._rope[0] != device or self._rope[1] < need_pos:
@@ -217,7 +240,7 @@ class LlamaAttention(nn.Module):
         H, hd = self.num_heads, self.head_dim
         if records(hidden_states, residual, self):
             return self._forward_training(hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual)
-        qkv = F.linear(hidden_states, self._qkv.get()).view(B, T, 3, H, hd)
+        qkv = decode_linear(hidden_states, self._qkv.get(), self._fp8, "qkv").view(B, T, 3, H, hd)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
         static = isinstance(past_key_value, StaticKV)
         past = 0 if past_key_value is None else (past_key_value.length if static else past_key_value[0].shape[1])
@@ -251,7 +274,7 @@ class LlamaAttention(nn.Module):
             else:
                 key_mask = attention_mask
         ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)       # (B, T, H*hd)
-        out = self.o_proj(ctx) if residual is None else _addmm_residual(residual, ctx, self.o_proj.weight, inplace)
+        out = decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace)
         return out, None, present
 
     def _forward_training(self, hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual):

@@ -17,7 +17,7 @@ from torch import nn
 
 from . import generation
 from ._cache import WeightCache
-from .llama_mmfs import LlamaMMFSConfig, LlamaModel
+from .llama_mmfs import LlamaAttention, LlamaMLP, LlamaMMFSConfig, LlamaModel, decode_linear
 from .msda import records
 
 # special-token convention of the reference (mm_interleaved.py:33-39; custom_datasets/wds_utils.py:186-215 appends
@@ -154,6 +154,7 @@ class TextDecoder(nn.Module):
         self.head = nn.Linear(hidden_size, vocab_size, bias=True)
         self.head_new = nn.Linear(hidden_size, vocab_size - orig_vocab_size, bias=True)
         self._fused_cache = WeightCache()
+        self._fp8 = None                  # FP8 copy of the folded head for decode steps (enable_fp8_decode)
 
     _PAD = 128   # a vocabulary of 32002+ rows is not a multiple of 8: cuBLAS drops to an unaligned legacy kernel (5x slower)
 
@@ -179,7 +180,7 @@ class TextDecoder(nn.Module):
             tail = logits[..., self.orig_txt_vocab_size:] + self.head_new(hidden_states)
             return torch.cat([logits[..., :self.orig_txt_vocab_size], tail], dim=-1)
         w, b = self._fused()
-        return F.linear(hidden_states, w, b)[..., :self.head.weight.shape[0]]
+        return decode_linear(hidden_states, w, self._fp8, "head", bias=b)[..., :self.head.weight.shape[0]]
 
     def forward(self, inputs_embeds, attention_mask=None, position_ids=None, past_key_values=None, use_cache=None,
                 output_attentions=None, output_hidden_states=None, return_dict=None, **kwargs):
@@ -437,6 +438,30 @@ class InterleavedForward(nn.Module):
         its draws from the kernel's Philox stream keyed by a per-call seed, so again not the eager loop's tokens."""
         self._decode_graphs = {} if enabled else None
         self._decode_graph_sampling = bool(enabled and sampling)
+        return self
+
+    def enable_fp8_decode(self, enabled: bool = True) -> "InterleavedForward":
+        """Decode with FP8 weights: a decode step's wide linears -- the fused QKV, the fused gate/up and the folded text
+        head -- run on ``ops.linear_fp8`` with per-channel E4M3 copies of their weights (``ops.quantize_fp8_per_channel``)
+        where that kernel beat bf16 cuBLAS (``llama_mmfs.decode_linear``: one new position per row, at most
+        ``FP8_DECODE_MAX_ROWS`` rows, autograd not recording), in the eager token loop, beam search, the graphed decoders
+        and ``generate_interleaved`` alike.  A decode step streams every weight once per token, so fewer bytes per weight
+        is what can still shorten it.
+
+        This selects different numerics, not another route to the same result: the step computes exactly what the
+        16-bit model with those weights replaced by ``w8 * scale`` would (the scales are powers of two), up to the order
+        of the fp32 sums, so tokens may differ from the 16-bit decode.  Off by default.  o_proj and down_proj, the prefill
+        (more than one position; the head on the prefill's last position is a one-position call and takes FP8),
+        ``forward``, ``generate_scores``, the training path and the MMFS cross-attention linears keep the 16-bit
+        weights, so those stay resident; the FP8 copies, built on a layer's first decode step and kept per weight tensor
+        (``_cache.WeightCache``), add about 9 GB at the 13B sizes.  ``enabled=False`` drops them.  Toggling drops the
+        captured decode graphs, so no graph replays the other path."""
+        cache = WeightCache if enabled else (lambda: None)
+        for m in [*self.mm_decoder.modules(), self.text_decoder]:
+            if isinstance(m, (LlamaAttention, LlamaMLP, TextDecoder)):
+                m._fp8 = cache()
+        if self._decode_graphs is not None:
+            self._decode_graphs = {}
         return self
 
     def prepare(self, text_ids, visual_output, num_image_per_seq, max_num_image: int):

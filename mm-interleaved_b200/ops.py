@@ -827,3 +827,71 @@ def group_norm_nhwc_backward(x: torch.Tensor, dy: torch.Tensor, groups: int, wei
     _lib.check(rc, "group_norm_nhwc_backward")
     launch_counter[0] += 3
     return dx
+
+
+E4M3_MAX = 448.0                                      # largest finite float8_e4m3fn
+LINEAR_FP8_MAX_M = _lib.LINEAR_FP8_MAX_M
+
+
+def quantize_fp8_per_channel(w: torch.Tensor):
+    """(w8, scale) of a (N, K) weight: ``w8`` float8_e4m3fn (N, K), ``scale`` fp32 (N,) with ``w ~= w8 * scale[:, None]``.
+
+    Each scale is the least power of two with ``amax_n / scale <= 448`` (``2^ceil(log2(amax_n / 448))``), 1 for an
+    all-zero row.  The division by it is exact and the cast rounds to nearest even without ever saturating.  Powers of
+    two make ``w8 * scale`` exactly representable in bf16 and fp16's range, so the FP8 model is exactly the 16-bit
+    model with weights ``w8 * scale``.  The cost against a scale of exactly ``amax / 448``: at most one bit of e4m3
+    range per channel (the row's largest entry may land in [224, 448] instead of at 448)."""
+    _require(w.dim() == 2 and w.dtype in (torch.float16, torch.bfloat16, torch.float32),
+             "quantize_fp8_per_channel: w must be a 2-D fp16 / bf16 / fp32 tensor")
+    wf = w.detach().float()
+    amax = wf.abs().amax(dim=1)
+    scale = torch.exp2(torch.ceil(torch.log2(amax / E4M3_MAX)))
+    # log2 and the division round: settle on the least power of two that keeps amax within range
+    scale = torch.where(amax / scale > E4M3_MAX, scale * 2, scale)
+    scale = torch.where(amax / (scale * 0.5) <= E4M3_MAX, scale * 0.5, scale)
+    scale = torch.where(amax > 0, scale, torch.ones_like(scale)).contiguous()
+    w8 = (wf / scale[:, None]).to(torch.float8_e4m3fn)
+    return w8, scale
+
+
+def linear_fp8_supported(x: torch.Tensor, w8: torch.Tensor) -> bool:
+    """Whether ``linear_fp8`` takes ``x`` (..., K) against ``w8`` (N, K): CUDA bf16 / fp16 x with at most
+    ``LINEAR_FP8_MAX_M`` rows and K a multiple of 16."""
+    K = x.shape[-1]
+    return (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16) and w8.dtype == torch.float8_e4m3fn
+            and w8.dim() == 2 and w8.shape[1] == K and K % 16 == 0 and 0 < x.numel() // max(K, 1) <= LINEAR_FP8_MAX_M)
+
+
+def linear_fp8(x: torch.Tensor, w8: torch.Tensor, scale: torch.Tensor, bias=None, residual=None, out=None):
+    """``x @ (w8 * scale[:, None])^T [+ bias] [+ residual]`` on the weight-streaming kernel
+    (csrc/linear_fp8_sm100.cu): x (..., K) bf16 / fp16 with at most ``LINEAR_FP8_MAX_M`` rows, ``w8`` float8_e4m3fn
+    (N, K), ``scale`` fp32 (N,), ``bias`` (N,) and ``residual`` (..., N) in x's dtype.  The result is rounded once;
+    ``out`` (..., N) may be ``residual`` (accumulated in place).  One launch, no host synchronisation."""
+    inference_only("linear_fp8", x, residual)
+    K = x.shape[-1]
+    _require(x.is_cuda and x.dtype in (torch.bfloat16, torch.float16), "linear_fp8: x must be a CUDA bf16 / fp16 tensor")
+    _require(w8.dtype == torch.float8_e4m3fn and w8.dim() == 2 and w8.shape[1] == K and w8.is_contiguous()
+             and w8.device == x.device, f"linear_fp8: w8 must be a contiguous float8_e4m3fn (N, {K}) tensor on {x.device}")
+    N = w8.shape[0]
+    _require(scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == N and scale.device == x.device,
+             f"linear_fp8: scale must be a contiguous fp32 tensor of {N} elements on {x.device}")
+    _check_affine("linear_fp8", x, N, bias)
+    x2 = x.reshape(-1, K)
+    if not x2.is_contiguous() or x2.data_ptr() % 16:
+        x2 = x2.clone(memory_format=torch.contiguous_format)
+    M = x2.shape[0]
+    shape = tuple(x.shape[:-1]) + (N,)
+    for t, name in ((residual, "residual"), (out, "out")):
+        if t is not None:
+            _require(tuple(t.shape) == shape and t.dtype == x.dtype and t.is_contiguous() and t.device == x.device,
+                     f"linear_fp8: {name} must be a contiguous {x.dtype} tensor of shape {shape}")
+    if out is None:
+        out = torch.empty(shape, dtype=x.dtype, device=x.device)
+    with torch.cuda.device(x.device):
+        rc = _lib.lib().mmfs_linear_fp8(x2.data_ptr(), w8.data_ptr(), scale.data_ptr(),
+                                        bias.data_ptr() if bias is not None else None,
+                                        residual.data_ptr() if residual is not None else None, out.data_ptr(),
+                                        M, N, K, _DTYPE_CODE[x.dtype], _stream())
+    _lib.check(rc, "linear_fp8")
+    launch_counter[0] += 1
+    return out
