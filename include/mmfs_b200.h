@@ -216,6 +216,20 @@ long mmfs_attn_decode_scratch_floats(int B, int H, int Tkv, int hd);
 int mmfs_attn_decode(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask, float *scratch,
                      int B, int H, int Tkv, int hd, long q_bs, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs,
                      float scale, int causal, int past, int dtype, void *stream);
+/* mmfs_attn_decode over a prompt stored once per group of rows (graphed beam search): R = P * G query rows q (R, 1, H, hd)
+ * in groups of G consecutive rows, one group per prompt.  Row r's key / value at position p (0 <= p < Tkv) is
+ * k_prefix / v_prefix[r / G][p] when p < *prefix_len, with k_prefix / v_prefix (P, Tp, H, hd); otherwise
+ * k_gen / v_gen[r][min(p - *prefix_len, max_new - 1)], with k_gen / v_gen (R, max_new, H, hd).  prefix_len is a (1,)
+ * int64 DEVICE value (one captured graph serves every prompt length), read clamped to [0, Tp].  key_mask (R, Tkv),
+ * causal, past, scale, strides (elements, 16-byte aligned rows) and scratch (mmfs_attn_decode_scratch_floats(R, H, Tkv,
+ * hd) floats) mean what they mean in mmfs_attn_decode, and the output is bit-identical to mmfs_attn_decode's over the
+ * equivalent replicated (R, Tkv, H, hd) cache.  MMFS_EINVAL: null pointers, R % G != 0, max_new < 1, a bad shape;
+ * MMFS_EUNSUPPORTED: mmfs_attn_decode's dtype / hd / alignment limits, R / G > 65535. */
+int mmfs_attn_decode_shared(const void *q, const void *k_prefix, const void *v_prefix, const void *k_gen, const void *v_gen,
+                            void *out, const uint8_t *key_mask, const long long *prefix_len, float *scratch,
+                            int R, int G, int H, int Tkv, int Tp, int max_new, int hd, long q_bs,
+                            long kp_bs, long kp_ts, long vp_bs, long vp_ts, long kg_bs, long kg_ts, long vg_bs, long vg_ts,
+                            long o_bs, float scale, int causal, int past, int dtype, void *stream);
 
 /*
  * softmax(q k^T * scale + mask) v on the tensor cores (wgmma, register accumulators, TMA tiles):

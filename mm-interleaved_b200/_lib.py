@@ -49,6 +49,7 @@ SIGNATURES = {
     "mmfs_conv2d_down2x_nhwc": (_I, [_P] * 4 + [_I] * 6 + [_P]),
     "mmfs_attn_decode_scratch_floats": (_L, [_I] * 4),
     "mmfs_attn_decode": (_I, [_P] * 6 + [_I] * 4 + [_L] * 6 + [_F, _I, _I, _I, _P]),
+    "mmfs_attn_decode_shared": (_I, [_P] * 9 + [_I] * 7 + [_L] * 10 + [_F, _I, _I, _I, _P]),
     "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
     "mmfs_attn_forward_lse": (_I, [_P] * 6 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
     "mmfs_attn_backward": (_I, [_P] * 11 + [_I] * 4 + [_L] * 16 + [_F, _I, _P]),

@@ -111,16 +111,46 @@ attn_generic_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *_
 constexpr int kDecKeys = 256;     // keys per CTA
 constexpr int kDecWarps = 4;      // 64 keys per warp, two passes of 32
 
+// Shared-prefix layout (mmfs_attn_decode_shared, the graphed beam search): the R query rows come in groups of G, one
+// group per prompt; the kernels' k / v (with k_bs, k_ts, v_bs, v_ts) are then the (P, Tp, H, hd) prefix, one row per
+// prompt, and row r's key / value at position j is prefix[r / G][j] below *prefix_len (clamped to [0, Tp]) and
+// gen[r][min(j - prefix_len, max_new - 1)] from there on.  A SHARED instantiation launches grid (n_split * G, H, P) with
+// blockIdx.x = split * G + g, so the G rows that read the same prefix tile are adjacent in launch order and share it
+// through L2.  Only the addressing differs: the arithmetic, the splits and the merge order are the replicated
+// kernels', so the output is bit-identical to mmfs_attn_decode over the replicated cache.
 template <typename T>
+struct SharedPrefix {
+    const T *k_gen, *v_gen;                           // (R, max_new, H, hd)
+    long kg_bs, kg_ts, vg_bs, vg_ts;
+    const long long *prefix_len;                      // (1,) device
+    int G, Tp, max_new;
+};
+
+template <typename T>
+__device__ __forceinline__ int shared_prefix_len(const SharedPrefix<T> &sp) {
+    return (int)min(max(*sp.prefix_len, 0ll), (long long)sp.Tp);
+}
+
+// position j of row b: prefix row `pre` (already offset to the prompt, head and lane) or generated row `gen`
+template <typename T>
+__device__ __forceinline__ const T *shared_kv_row(const T *pre, long pre_ts, const T *gen, long gen_ts, int j, int plen,
+                                                  int max_new) {
+    return j < plen ? pre + (long)j * pre_ts : gen + (long)min(j - plen, max_new - 1) * gen_ts;
+}
+
+template <typename T, bool SHARED = false>
 __global__ void __launch_bounds__(32 * kDecWarps)
 attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *__restrict__ v,
                          const uint8_t *__restrict__ key_mask, float *__restrict__ part, int H, int Tkv, int hd,
-                         long q_bs, long k_bs, long k_ts, long v_bs, long v_ts, float scale, int last_key) {
+                         long q_bs, long k_bs, long k_ts, long v_bs, long v_ts, float scale, int last_key,
+                         SharedPrefix<T> sp) {
     constexpr int VEC = 16 / (int)sizeof(T);
     extern __shared__ float s_dec[];                  // q[hd] | per-warp partials [kDecWarps][hd + 2]
     float *s_q = s_dec, *s_red = s_dec + hd;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z, n_split = gridDim.x;
+    const int split = SHARED ? blockIdx.x / sp.G : blockIdx.x, h = blockIdx.y,
+              b = SHARED ? blockIdx.z * sp.G + blockIdx.x % sp.G : blockIdx.z, n_split = SHARED ? gridDim.x / sp.G : gridDim.x;
+    const int plen = SHARED ? shared_prefix_len(sp) : 0;
     const int cpl = hd / 32;                          // channels per lane in the P V phase (host: hd % 32 == 0, <= 8)
     const T *qp = q + b * q_bs + (long)h * hd;
     for (int d = threadIdx.x; d < hd; d += blockDim.x) s_q[d] = to_op(qp[d]) * scale;
@@ -138,7 +168,12 @@ attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const
         const int j = j0 + lane;
         float sc = -INFINITY;
         if (j <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + j])) {
-            const T *kp = k + b * k_bs + (long)j * k_ts + (long)h * hd;
+            const T *kp;
+            if constexpr (SHARED)
+                kp = shared_kv_row(k + blockIdx.z * k_bs + (long)h * hd, k_ts, sp.k_gen + b * sp.kg_bs + (long)h * hd, sp.kg_ts,
+                                   j, plen, sp.max_new);
+            else
+                kp = k + b * k_bs + (long)j * k_ts + (long)h * hd;
             float dot = 0.f;
             for (int d0 = 0; d0 < hd; d0 += VEC) {
                 float f[VEC];
@@ -170,7 +205,12 @@ attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const
         for (int jj = 0; jj < 32; ++jj) {
             const float pw = __shfl_sync(0xffffffffu, pj, jj);
             if (pw == 0.f) continue;                  // warp-uniform
-            const T *vp = vb + (long)(j0 + jj) * v_ts;
+            const T *vp;
+            if constexpr (SHARED)
+                vp = shared_kv_row(v + blockIdx.z * v_bs + (long)h * hd + lane * cpl, v_ts,
+                                   sp.v_gen + b * sp.vg_bs + (long)h * hd + lane * cpl, sp.vg_ts, j0 + jj, plen, sp.max_new);
+            else
+                vp = vb + (long)(j0 + jj) * v_ts;
             bool done = false;
             if constexpr (sizeof(T) == 2) {
                 if (cpl == 4) {                        // hd = 128, 16-bit: one 8-byte load per lane, 256 B per warp
@@ -245,12 +285,13 @@ __device__ __forceinline__ float dot16_mixed(const uint4 &ka, const uint4 &kb, c
     return d0 + d1;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(32 * kDecWarps, 5)
+// SHARED: 4 CTAs per SM (128 registers), which holds the generated rows' pointers without spilling
+template <typename T, bool SHARED = false>
+__global__ void __launch_bounds__(32 * kDecWarps, SHARED ? 4 : 5)
 attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *__restrict__ v,
                             const uint8_t *__restrict__ key_mask, float *__restrict__ part, unsigned *__restrict__ tickets,
                             T *__restrict__ out, int H, int Tkv, long q_bs, long k_bs, long k_ts, long v_bs, long v_ts,
-                            long o_bs, float scale, int last_key) {
+                            long o_bs, float scale, int last_key, SharedPrefix<T> sp) {
     constexpr int WARPS = kDecWarps, HD = 128, KPW = kDecKeys / WARPS;
     static_assert(KPW == 64, "the pipeline below walks a warp's keys in four batches of 16");
     static_assert(32 * WARPS >= HD, "one thread per channel in the combine / merge steps");
@@ -259,7 +300,9 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
     __shared__ float s_m[WARPS], s_l[WARPS];
     __shared__ int s_is_last;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z, n_split = gridDim.x;
+    const int split = SHARED ? blockIdx.x / sp.G : blockIdx.x, h = blockIdx.y,
+              b = SHARED ? blockIdx.z * sp.G + blockIdx.x % sp.G : blockIdx.z, n_split = SHARED ? gridDim.x / sp.G : gridDim.x;
+    const int plen = SHARED ? shared_prefix_len(sp) : 0;
     const int k0 = split * kDecKeys + warp * KPW;
     const int half = lane >> 4, ch = (lane & 15) * 8;
     float m = -INFINITY, l = 0.f;
@@ -288,14 +331,27 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
         auto load_k = [&](uint4 (&r)[8], int bt) {
 #pragma unroll
             for (int s = 0; s < 4; ++s) {
-                const T *kp = kb + (long)min(k0 + bt * 16 + s * 4 + grp, last_key) * k_ts;
+                const T *kp;
+                if constexpr (SHARED)
+                    kp = shared_kv_row(k + blockIdx.z * k_bs + (long)h * HD + sub * 16, k_ts,
+                                       sp.k_gen + b * sp.kg_bs + (long)h * HD + sub * 16, sp.kg_ts,
+                                       min(k0 + bt * 16 + s * 4 + grp, last_key), plen, sp.max_new);
+                else
+                    kp = kb + (long)min(k0 + bt * 16 + s * 4 + grp, last_key) * k_ts;
                 r[2 * s] = ldg_nc_v4(kp);
                 r[2 * s + 1] = ldg_nc_v4(kp + 8);
             }
         };
         auto load_v = [&](uint4 (&r)[8], int bt) {
 #pragma unroll
-            for (int s = 0; s < 8; ++s) r[s] = ldg_nc_v4(vb + (long)min(k0 + bt * 16 + s * 2 + half, last_key) * v_ts);
+            for (int s = 0; s < 8; ++s) {
+                if constexpr (SHARED)
+                    r[s] = ldg_nc_v4(shared_kv_row(v + blockIdx.z * v_bs + (long)h * HD + ch, v_ts,
+                                                   sp.v_gen + b * sp.vg_bs + (long)h * HD + ch, sp.vg_ts,
+                                                   min(k0 + bt * 16 + s * 2 + half, last_key), plen, sp.max_new));
+                else
+                    r[s] = ldg_nc_v4(vb + (long)min(k0 + bt * 16 + s * 2 + half, last_key) * v_ts);
+            }
         };
         auto scores = [&](const uint4 (&r)[8], int bt) {          // 4 steps of 4 keys
             const unsigned okw = (bt < 2 ? ok_lo : ok_hi) >> ((bt & 1) * 16);
@@ -428,27 +484,29 @@ __global__ void attn_decode_merge_kernel(const float *__restrict__ part, T *__re
 
 static inline long decode_ticket_floats(int B, int H) { return ((long)B * H + 3) / 4 * 4; }   // keeps the partials 16-byte aligned
 
-template <typename T>
+// B query rows; SHARED: B = P * sp.G rows over the shared-prefix layout (k / v = the prefix)
+template <typename T, bool SHARED = false>
 static int launch_attn_decode(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask, float *scratch,
                               int B, int H, int Tkv, int hd, long q_bs, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs,
-                              float scale, int last_key, cudaStream_t st) {
+                              float scale, int last_key, cudaStream_t st, SharedPrefix<T> sp = {}) {
     const int n_split = (last_key + kDecKeys) / kDecKeys;           // keys 0 .. last_key
-    dim3 grid(n_split, H, B);
+    dim3 grid = SHARED ? dim3(n_split * sp.G, H, B / sp.G) : dim3(n_split, H, B);
     if constexpr (sizeof(T) == 2) {
         if (hd == 128 && ((uintptr_t)q % 16 == 0) && (q_bs % 8 == 0) && ((uintptr_t)scratch % 16 == 0)) {
             unsigned *tickets = reinterpret_cast<unsigned *>(scratch);          // [B * H], then the partials
             float *part = scratch + decode_ticket_floats(B, H);
             if (n_split > 1) MMFS_CUDA(cudaMemsetAsync(tickets, 0, sizeof(unsigned) * (size_t)B * H, st));
-            attn_decode_split128_kernel<T><<<grid, 32 * kDecWarps, 0, st>>>((const T *)q, (const T *)k, (const T *)v, key_mask, part,
-                                                                          tickets, (T *)out, H, Tkv, q_bs, k_bs, k_ts, v_bs, v_ts,
-                                                                          o_bs, scale, last_key);
+            attn_decode_split128_kernel<T, SHARED><<<grid, 32 * kDecWarps, 0, st>>>(
+                (const T *)q, (const T *)k, (const T *)v, key_mask, part, tickets, (T *)out, H, Tkv, q_bs, k_bs, k_ts, v_bs, v_ts,
+                o_bs, scale, last_key, sp);
             MMFS_CUDA(cudaGetLastError());
             return MMFS_OK;
         }
     }
     const size_t smem = (size_t)(hd + kDecWarps * (hd + 2)) * sizeof(float);
-    attn_decode_split_kernel<T><<<grid, 32 * kDecWarps, smem, st>>>((const T *)q, (const T *)k, (const T *)v, key_mask, scratch, H,
-                                                                   Tkv, hd, q_bs, k_bs, k_ts, v_bs, v_ts, scale, last_key);
+    attn_decode_split_kernel<T, SHARED><<<grid, 32 * kDecWarps, smem, st>>>((const T *)q, (const T *)k, (const T *)v, key_mask,
+                                                                           scratch, H, Tkv, hd, q_bs, k_bs, k_ts, v_bs, v_ts,
+                                                                           scale, last_key, sp);
     attn_decode_merge_kernel<T><<<dim3(H, B), hd < 128 ? 64 : 128, 0, st>>>(scratch, (T *)out, H, hd, n_split, o_bs);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
@@ -510,5 +568,36 @@ extern "C" int mmfs_attn_decode(const void *q, const void *k, const void *v, voi
     return dispatch_dtype<kF32Types>(dtype, "attn_decode", [&](auto tag) {
         return launch_attn_decode<typename decltype(tag)::type>(q, k, v, out, key_mask, scratch, B, H, Tkv, hd, q_bs, k_bs, k_ts,
                                                                 v_bs, v_ts, o_bs, scale, last_key, st);
+    });
+}
+
+extern "C" int mmfs_attn_decode_shared(const void *q, const void *k_prefix, const void *v_prefix, const void *k_gen,
+                                       const void *v_gen, void *out, const uint8_t *key_mask, const long long *prefix_len,
+                                       float *scratch, int R, int G, int H, int Tkv, int Tp, int max_new, int hd, long q_bs,
+                                       long kp_bs, long kp_ts, long vp_bs, long vp_ts, long kg_bs, long kg_ts, long vg_bs,
+                                       long vg_ts, long o_bs, float scale, int causal, int past, int dtype, void *stream) {
+    MMFS_CHECK_ARG(R >= 0 && G > 0 && H > 0 && Tkv > 0 && Tp > 0 && hd > 0, "attn_decode_shared: bad shape");
+    MMFS_CHECK_ARG(R % G == 0, "attn_decode_shared: R = %d rows are not whole groups of G = %d", R, G);
+    MMFS_CHECK_ARG(max_new >= 1, "attn_decode_shared: max_new must be >= 1");
+    if (R == 0) return MMFS_OK;
+    MMFS_CHECK_ARG(q && k_prefix && v_prefix && k_gen && v_gen && out && prefix_len && scratch,
+                   "attn_decode_shared: null pointer argument");
+    const size_t es = dtype_size(dtype);
+    const long strides[8] = {kp_bs, kp_ts, vp_bs, vp_ts, kg_bs, kg_ts, vg_bs, vg_ts};
+    bool aligned = (((uintptr_t)k_prefix | (uintptr_t)v_prefix | (uintptr_t)k_gen | (uintptr_t)v_gen) % 16 == 0);
+    for (long s : strides) aligned = aligned && (s * (long)es) % 16 == 0;
+    if (dtype == MMFS_F64 || es == 0 || hd % 32 != 0 || hd > 256 || R / G > 65535 || H > 65535 || !aligned ||
+        (hd * es) % 16 != 0) {
+        set_error("attn_decode_shared: needs f32/f16/bf16, hd %% 32 == 0 (<= 256), 16-byte aligned prefix / gen rows, R / G <= 65535");
+        return MMFS_EUNSUPPORTED;
+    }
+    const int last_key = causal ? (past < Tkv - 1 ? past : Tkv - 1) : Tkv - 1;
+    MMFS_CHECK_ARG(last_key >= 0, "attn_decode_shared: negative past");
+    cudaStream_t st = (cudaStream_t)stream;
+    return dispatch_dtype<kF32Types>(dtype, "attn_decode_shared", [&](auto tag) {
+        using T = typename decltype(tag)::type;
+        const SharedPrefix<T> sp{(const T *)k_gen, (const T *)v_gen, kg_bs, kg_ts, vg_bs, vg_ts, prefix_len, G, Tp, max_new};
+        return launch_attn_decode<T, true>(q, k_prefix, v_prefix, out, key_mask, scratch, R, H, Tkv, hd, q_bs, kp_bs, kp_ts,
+                                           vp_bs, vp_ts, o_bs, scale, last_key, st, sp);
     });
 }

@@ -9,7 +9,7 @@ from typing import List, Optional
 import torch
 
 from . import ops
-from .llama_mmfs import PreparedVision, StaticKV
+from .llama_mmfs import PreparedVision, SharedPrefixKV, StaticKV
 
 _BEAM_SAMPLE_TOP_K = 50              # transformers 4.31 GenerationConfig.top_k, which the reference never overrides
 
@@ -399,11 +399,15 @@ class _GraphedDecoder:
         self.cross_last.copy_(cross[:, -1:, :])
         self.logits.copy_(logits0)
 
-    def _prefill_done(self, L, reset):
-        """After the prefill: zero the unused cache slots, capture the step graph once, reset the per-call state."""
-        for c in self.past:                                                 # masked slots must hold finite numbers
+    def _clear_unused(self, L):
+        """Zero the cache positions from ``L`` on: masked slots must hold finite numbers."""
+        for c in self.past:
             c.k[:, L:].zero_()
             c.v[:, L:].zero_()
+
+    def _prefill_done(self, L, reset):
+        """After the prefill: zero the unused cache slots, capture the step graph once, reset the per-call state."""
+        self._clear_unused(L)
         self._set_graph_mode(True)
         if self.graph is None:
             reset()
@@ -423,9 +427,7 @@ class _GraphedDecoder:
             # the graph reads the RoPE tables by address: keep the captured storage alive even if an eager decode grows
             # (and so replaces) the shared tables later
             self._captured_rope = [l.self_attn._rope for l in self.owner.mm_decoder.layers]
-            for c in self.past:                                             # the warm-up steps wrote slots L, L+1
-                c.k[:, L:].zero_()
-                c.v[:, L:].zero_()
+            self._clear_unused(L)                                           # the warm-up steps wrote the first new slot
         reset()
 
     def _replayed(self, L, n):
@@ -475,20 +477,31 @@ class TokenDecoder(_GraphedDecoder):
 
 class BeamDecoder(_GraphedDecoder):
     """Beam search over B * num_beams rows: the step is ``ops.beam_select`` (scores, hypotheses, done flags, history)
-    -> ``ops.kv_beam_reorder`` (the generated positions of every layer's K and V, held in one tensor ``kv``) -> the
+    -> ``ops.kv_beam_reorder`` (the generated positions of every layer's K and V, held in one tensor ``gen``) -> the
     decoder on the next tokens, with the repetition and length penalties in a device buffer; ``finished`` holds the
     per-sequence done flags.  With ``sample`` the step uses ``ops.beam_sample`` instead (temperature and top_p in the
-    device buffer too, one seed per call, a sticky error flag) and every beam starts at score 0."""
+    device buffer too, one seed per call, a sticky error flag) and every beam starts at score 0.
+
+    The KV cache stores each prompt once: ``prefix`` (2·layers, P, T_p, H, hd), T_p = t_max - max_new, holds the P
+    prompts' positions, which are the same for all G = R / P rows of a prompt (its beams, and with beam sample its
+    independent searches); ``gen`` (2·layers, R, max_new, H, hd) holds every row's generated positions.  The decoder
+    steps over ``SharedPrefixKV`` views of both (``ops.attention_decode_shared``)."""
 
     def __init__(self, model, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, sample,
                  num_beams):
         nb = self.nb = int(num_beams)
         R = B * nb                                                          # decoder rows: one per beam
+        P = feats_shape[0]                                                  # prompts: the features have one row each
         cfg, layers = model.mm_decoder.config, model.mm_decoder.layers
-        H = cfg.num_attention_heads
-        self.kv = torch.zeros((2 * len(layers), R, t_max, H, cfg.hidden_size // H), dtype=dtype, device=device)
-        self.past = [StaticKV.over(self.kv[2 * i], self.kv[2 * i + 1]) for i in range(len(layers))]
+        n, H = 2 * len(layers), cfg.num_attention_heads
+        hd = cfg.hidden_size // H
+        self.prefix = torch.zeros((n, P, t_max - max_new, H, hd), dtype=dtype, device=device)
+        self.gen = torch.zeros((n, R, max_new, H, hd), dtype=dtype, device=device)
+        self.prefix_kv = [StaticKV.over(self.prefix[2 * i], self.prefix[2 * i + 1]) for i in range(len(layers))]
+        self.prefix_len = torch.zeros((1,), dtype=torch.long, device=device)
         super().__init__(model, B, R, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, sample)
+        self.past = [SharedPrefixKV(self.prefix[2 * i], self.prefix[2 * i + 1], self.gen[2 * i], self.gen[2 * i + 1],
+                                    self.prefix_len, self.step) for i in range(len(layers))]
         # repetition_penalty, length_penalty (+ temperature, top_p when sampling)
         self.params = torch.ones((4 if sample else 2,), dtype=torch.float64, device=device)
         self.beam_scores = torch.zeros((R,), dtype=torch.float32, device=device)
@@ -513,7 +526,14 @@ class BeamDecoder(_GraphedDecoder):
             ops.beam_select(self.logits, self.step, self.params, self.beam_scores, self.history, self.next_ids,
                             self.parent, self.finished, self.hyp_scores, self.hyp_ids, self.hyp_meta, self.scratch,
                             self.nb, eos=self.eos, pad_id=self.pad_id, min_length=self.min_length)
-        ops.kv_beam_reorder(self.kv, self.parent, self.cur, self.step, self.nb, self.max_new, done=self.finished)
+        ops.kv_beam_reorder(self.gen, self.parent, self.step, self.step, self.nb, self.max_new, done=self.finished)
+
+    def _set_graph_mode(self, on: bool, length: int = 0):
+        pass                                                               # SharedPrefixKV is graph-only: slot = step
+
+    def _clear_unused(self, L):
+        self.prefix[:, :, L:].zero_()
+        self.gen.zero_()
 
     def _step(self):
         super()._step()
@@ -532,8 +552,9 @@ class BeamDecoder(_GraphedDecoder):
         self.hyp_meta.fill_(-1)
 
     def generate(self, p: Prompt, repetition_penalty, length_penalty, num_return, temperature, top_p, generator):
-        """The prompt is prefilled once per sequence and its cache rows, the ``PreparedVision`` values, key mask,
-        position ids and last cross-attention row are replicated to the beams (beam sample: to the ``self.B // B``
+        """The prompt is prefilled once per sequence, straight into ``prefix`` (after an interleaved session's cached
+        prefix: into the session's cache, whose B prompt rows are then copied), and the ``PreparedVision`` values, key
+        mask, position ids and last cross-attention row are replicated to the beams (beam sample: to the ``self.B // B``
         independent searches of each prompt, then to their beams); then one replay per step.  At most two replays are
         in flight: before enqueuing replay t the host waits for replay t - 2 and reads the "all sequences done" flag it
         copied to pinned memory, so decoding stops at most two steps after the eager loop would (done sequences are
@@ -546,8 +567,16 @@ class BeamDecoder(_GraphedDecoder):
         pv = o.mm_decoder.prepare_vision(p.feats)                           # the prefill's B rows, then one per beam
         for idx, val in pv.values.items():
             torch.index_select(val, 0, rep, out=self.pv.values[idx])
-        logits, mask_r, pos_r, cross_r = _prefill_beams(o, p, rep, self.past, pv)
+        for c in self.prefix_kv:
+            c.length = 0
+        if p.cache is None:
+            _, logits = _prefill(o, p, self.prefix_kv, pv)
+        else:
+            logits = next(_prefill_beams(o, p, torch.arange(B, device=rep.device), self.prefix_kv, pv))
         del pv
+        self.prefix_len.fill_(L)
+        logits, mask_r, pos_r, cross_r = (t.index_select(0, rep) for t in (logits, p.attention_mask,
+                                                                           p.position_ids[:, -1:], p.cross[:, -1:, :]))
         logits0 = logits[:, -1].float()
         self._prefill_done(L, lambda: self._reset(L, mask_r, pos_r, cross_r, logits0))
         torch.cuda.current_stream().synchronize()                           # no copy into all_done is pending

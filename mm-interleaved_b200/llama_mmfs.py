@@ -189,6 +189,28 @@ class StaticKV:
         return c
 
 
+class SharedPrefixKV:
+    """Graph-decode cache of one layer whose rows come in groups of ``G`` that share a prompt (the graphed beam search,
+    ``generation.BeamDecoder``): ``k``, ``v`` (P, T_p, H, hd) hold each prompt's positions once; ``k_gen``, ``v_gen``
+    (P·G, max_new, H, hd) hold every row's generated positions.  Row r's position p lies in ``k[r // G, p]`` below
+    ``prefix_len`` and in ``k_gen[r, p - prefix_len]`` from there on.  ``prefix_len`` and ``slot`` (where the next
+    token's key / value go in ``k_gen``) are (1,) int64 DEVICE tensors, so one captured step serves every prompt length
+    and step.  A step appends one token per row and attends over all ``length + 1`` = T_p + max_new positions under the
+    caller's key mask (``ops.attention_decode_shared``); there is no eager use."""
+
+    __slots__ = ("k", "v", "k_gen", "v_gen", "G", "prefix_len", "slot")
+
+    def __init__(self, k, v, k_gen, v_gen, prefix_len, slot):
+        self.k, self.v, self.k_gen, self.v_gen = k, v, k_gen, v_gen
+        self.G = k_gen.shape[0] // k.shape[0]
+        self.prefix_len, self.slot = prefix_len, slot
+
+    @property
+    def length(self):
+        """Positions before the step's query, as ``StaticKV.length`` in graph decode (pinned at the last position)."""
+        return self.k.shape[1] + self.k_gen.shape[1] - 1
+
+
 class PreparedVision:
     """Image-side state of the MMFS cross-attention layers for ONE batch of images: per layer, ``value`` =
     value_proj(RMSNorm(vision)) (modeling_llama_mmfs.py:353, mmfs.py:165-172) -- everything those layers derive from
@@ -242,12 +264,20 @@ class LlamaAttention(nn.Module):
             return self._forward_training(hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual)
         qkv = decode_linear(hidden_states, self._qkv.get(), self._fp8, "qkv").view(B, T, 3, H, hd)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-        static = isinstance(past_key_value, StaticKV)
+        shared = isinstance(past_key_value, SharedPrefixKV)
+        static = shared or isinstance(past_key_value, StaticKV)
         past = 0 if past_key_value is None else (past_key_value.length if static else past_key_value[0].shape[1])
         if position_ids is None:
             position_ids = torch.arange(past, past + T, device=hidden_states.device)
         cos, sin = self.rope_tables(hidden_states.device, past + T)
-        if static and past_key_value.slot is not None:          # graph decode: device-side slot, whole buffer visible
+        if shared:                                              # graph decode over a shared prompt: append to the row's gen
+            if T != 1:
+                raise RuntimeError("SharedPrefixKV is a graph-decode cache (one token per step): prefill into its prefix "
+                                   "through StaticKV.over, and decode eagerly over a StaticKV")
+            ops.rope_qk_append_(q, k, v, cos, sin, position_ids, past_key_value.k_gen, past_key_value.v_gen,
+                                past_key_value.slot)
+            present = past_key_value
+        elif static and past_key_value.slot is not None:          # graph decode: device-side slot, whole buffer visible
             if T != 1:
                 raise RuntimeError("StaticKV.slot (graph decode) takes one token per step")
             ops.rope_qk_append_(q, k, v, cos, sin, position_ids, past_key_value.k, past_key_value.v, past_key_value.slot)
@@ -273,7 +303,11 @@ class LlamaAttention(nn.Module):
                 key_mask = attention_mask[:, 0, -1, :] > (torch.finfo(attention_mask.dtype).min / 2)
             else:
                 key_mask = attention_mask
-        ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)       # (B, T, H*hd)
+        if shared:
+            c = past_key_value
+            ctx = ops.attention_decode_shared(q, c.k, c.v, c.k_gen, c.v_gen, c.prefix_len, key_mask=key_mask, past=past)
+        else:
+            ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)   # (B, T, H*hd)
         out = decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace)
         return out, None, present
 
@@ -491,7 +525,8 @@ class LlamaModel(nn.Module):
         if past_key_values is None:
             past = 0
         else:
-            past = past_key_values[0].length if isinstance(past_key_values[0], StaticKV) else past_key_values[0][0].shape[1]
+            past = (past_key_values[0].length if isinstance(past_key_values[0], (StaticKV, SharedPrefixKV))
+                    else past_key_values[0][0].shape[1])
         if position_ids is None:
             position_ids = torch.arange(past, past + T, dtype=torch.long, device=inputs_embeds.device)
         else:

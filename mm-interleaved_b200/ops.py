@@ -392,6 +392,49 @@ def attention(q, k, v, key_mask=None, causal=True, past=0, scale=None, force_gen
     return out.view(B, Tq, H * hd)
 
 
+def attention_decode_shared(q, k_prefix, v_prefix, k_gen, v_gen, prefix_len, key_mask=None, causal=True, past=0,
+                            scale=None) -> torch.Tensor:
+    """The decode branch of ``attention`` over a prompt stored once per group of rows (``mmfs_attn_decode_shared``):
+    q (R, 1, H, hd) in P groups of G = R / P consecutive rows; row r's key / value at position p is
+    ``k_prefix[r // G, p]`` (k_prefix / v_prefix (P, T_p, H, hd)) for p < ``prefix_len`` and
+    ``k_gen[r, p - prefix_len]`` (k_gen / v_gen (R, max_new, H, hd)) after it, over Tkv = T_p + max_new positions.
+    ``prefix_len`` is a (1,) int64 device tensor; key_mask (R, Tkv), causal, past and scale as in ``attention``.  The
+    output (R, 1, H*hd) is bit-identical to ``attention`` over the equivalent replicated (R, Tkv, H, hd) cache."""
+    R, Tq, H, hd = q.shape
+    P, Tp = k_prefix.shape[:2]
+    max_new = k_gen.shape[1]
+    Tkv = Tp + max_new
+    inference_only("attention_decode_shared", q, k_prefix, v_prefix, k_gen, v_gen)
+    _require(Tq == 1, "attention_decode_shared: one query position per row")
+    for t in (q, k_prefix, v_prefix, k_gen, v_gen):
+        _require(t.is_cuda and t.dim() == 4 and t.dtype == q.dtype and t.device == q.device and tuple(t.shape[2:]) == (H, hd)
+                 and t.stride(3) == 1 and t.stride(2) == hd,
+                 "attention_decode_shared: q / prefix / gen must be (rows, T, H, hd) CUDA tensors of q's dtype, heads dense")
+    _require(v_prefix.shape == k_prefix.shape and tuple(k_gen.shape) == (R, max_new, H, hd) and v_gen.shape == k_gen.shape,
+             "attention_decode_shared: prefix must be (P, T_p, H, hd) and gen (R, max_new, H, hd)")
+    _require(P > 0 and R % P == 0, "attention_decode_shared: the rows must be whole groups, one per prefix row")
+    _require(prefix_len.device == q.device and prefix_len.dtype == torch.int64 and prefix_len.numel() == 1,
+             "attention_decode_shared: prefix_len must be a (1,) int64 device tensor")
+    scale = float(scale if scale is not None else hd ** -0.5)
+    out = torch.empty((R, 1, H, hd), dtype=q.dtype, device=q.device)
+    km = None
+    if key_mask is not None:
+        km = key_mask.to(torch.uint8).contiguous()
+        _require(tuple(km.shape) == (R, Tkv), "attention_decode_shared: key_mask must be (R, T_p + max_new)")
+    lib = _lib.lib()
+    scratch = torch.empty((lib.mmfs_attn_decode_scratch_floats(R, H, Tkv, hd),), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        rc = lib.mmfs_attn_decode_shared(q.data_ptr(), k_prefix.data_ptr(), v_prefix.data_ptr(), k_gen.data_ptr(),
+                                         v_gen.data_ptr(), out.data_ptr(), km.data_ptr() if km is not None else None,
+                                         prefix_len.data_ptr(), scratch.data_ptr(), R, R // P, H, Tkv, Tp, max_new, hd,
+                                         q.stride(0), k_prefix.stride(0), k_prefix.stride(1), v_prefix.stride(0),
+                                         v_prefix.stride(1), k_gen.stride(0), k_gen.stride(1), v_gen.stride(0), v_gen.stride(1),
+                                         out.stride(0), scale, 1 if causal else 0, int(past), _DTYPE_CODE[q.dtype], _stream())
+    _lib.check(rc, "attention_decode_shared")
+    launch_counter[0] += 2                      # as attention's decode branch counts itself
+    return out.view(R, 1, H * hd)
+
+
 # ---- training path: backward kernels (csrc/attn_bwd_sm100.cu, csrc/llama_ops_sm100.cu).  autograd_ops.py wraps them in
 # autograd Functions; like the forward wrappers they refuse to run where autograd would record them.
 

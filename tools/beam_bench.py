@@ -3,16 +3,20 @@
 ``generation.BeamDecoder``, ``ops.beam_select`` + ``ops.kv_beam_reorder`` + the decoder in one graph replay), on two
 prompt shapes:
   caption: 1 image (64 image tokens) in an 80-token prompt, the reference's captioning setting, B in {1, 4};
-  long:    the 2048-token 4-image prompt of tools/decode_bench.py, B in {1, 2}.  At B = 4 its 20 beam rows need a
-           34 GB cache (38 GB graphed) next to the 26 GB of weights, their ~18 GB of fused copies and the prefill
-           cache: more than an 80 GB card holds, in either loop.
+  long:    the 2048-token 4-image prompt of tools/decode_bench.py, B in {1, 2, 4}.  At B = 4 only the graphed loops run:
+           the eager loop's 20 beam rows each hold a copy of the prompt's cache, 34 GB next to the 26 GB of weights and
+           their ~18 GB of fused copies, more than an 80 GB card holds.  The graphed decoder stores the prompt once per
+           prompt (7.5 GB at B = 4).
 The same for beam sample (``use_nucleus_sampling=True``, top_p 0.9, temperature 1: the same eager loop with ``sample`` against
 the graphed ``ops.beam_sample`` step under ``enable_decode_graphs(True, sampling=True)``; their draws differ by design,
 so those ids are not compared).  With random weights eos is practically never chosen, so every step decodes.  ms per
 token = (time of a 20-token call - time of a 1-token call) / 19, each the best of 2 runs; the ids of the eager and
-graphed beam searches are compared.  Then the kernels alone (beam_select, beam_sample, the cache reorder) at the step
-in the middle of a run (step 10), CUDA events over many launches.  Prints one JSON object with the card name, its
-power limit and SM clock read in the same run.
+graphed beam searches are compared.  Beside each ms per token: the peak memory allocated by torch during the 20-token
+calls, the model's weights included (GB, 2^30 bytes).  Then the kernels alone (beam_select, beam_sample, the cache
+reorder) at the step in the middle of a run (step 10), CUDA events over many launches, and one layer's decode attention
+of that step, replayed from a CUDA graph, over the replicated cache (``ops.attention``) and over the shared prefix
+(``ops.attention_decode_shared``).
+Prints one JSON object with the card name, its power limit and SM clock read in the same run.
 
     python tools/beam_bench.py
 """
@@ -58,6 +62,18 @@ def timed(fn, iters):
     return 1e3 * e0.elapsed_time(e1) / iters
 
 
+def graph_timed(fn, per_graph=20, iters=20):
+    """us per call of ``fn`` replayed from a CUDA graph of ``per_graph`` calls: the device time of a graphed step's
+    kernels, without the Python enqueue cost that ``timed`` includes."""
+    fn()
+    torch.cuda.synchronize()
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        for _ in range(per_graph):
+            fn()
+    return timed(graph.replay, iters) / per_graph
+
+
 def kernel_rows(rows, step=MAX_NEW // 2):
     g = torch.Generator(device="cuda").manual_seed(0)
     eos = torch.tensor([2, 32000], device="cuda")
@@ -91,6 +107,23 @@ def kernel_rows(rows, step=MAX_NEW // 2):
         rows[f"kv_beam_reorder_B{B}_bytes"] = 2 * 2 * LAYERS * R * step * HIDDEN * 2          # read + write, K and V
         del kv
         torch.cuda.empty_cache()
+        # one layer's decode attention of the graphed step, replayed from a graph: over the replicated cache
+        # (ops.attention, the layout before the shared prefix) and over the shared prefix (ops.attention_decode_shared)
+        hd = HIDDEN // HEADS
+        for name, L in (("caption", 80), ("long", 2048)):
+            t_max = (L + MAX_NEW + 255) // 256 * 256
+            rnd = lambda *shape: torch.randn(shape, device="cuda", generator=g).to(torch.bfloat16)
+            q = rnd(R, 1, 3, HEADS, hd)[:, :, 0]
+            kr, vr = rnd(R, t_max, HEADS, hd), rnd(R, t_max, HEADS, hd)
+            kp, vp = kr[::NB, :t_max - MAX_NEW].contiguous(), vr[::NB, :t_max - MAX_NEW].contiguous()
+            kg, vg = kr[:, L:L + MAX_NEW].contiguous(), vr[:, L:L + MAX_NEW].contiguous()
+            mask = torch.zeros((R, t_max), dtype=torch.uint8, device="cuda")
+            mask[:, :L + step + 1] = 1
+            plen = torch.tensor([L], device="cuda")
+            rep_us = graph_timed(lambda: ops.attention(q, kr, vr, key_mask=mask, past=t_max - 1))
+            sh_us = graph_timed(lambda: ops.attention_decode_shared(q, kp, vp, kg, vg, plen, key_mask=mask, past=t_max - 1))
+            rows[f"attn_decode_{name}_B{B}_replicated_us"], rows[f"attn_decode_{name}_B{B}_shared_us"] = rep_us, sh_us
+            del kr, vr, kp, vp, kg, vg
 
 
 def caption_inputs(B):
@@ -117,7 +150,7 @@ kernel_rows(rows)
 model = workloads.full_model(with_image_decoder=False)
 eos = [2, workloads.InterleavedCfg3.SOI_ID]
 with torch.no_grad():
-    for shape, make, batches in (("caption", caption_inputs, (1, 4)), ("long", long_inputs, (1, 2))):
+    for shape, make, batches in (("caption", caption_inputs, (1, 4)), ("long", long_inputs, (1, 2, 4))):
         for B in batches:
             ids, img, nimg, n_img = make(B)
             ids, img, nimg = ids.cuda(), img.cuda(), nimg.cuda()
@@ -130,6 +163,7 @@ with torch.no_grad():
                     model, ids, vis, nimg, n_img, max_new_tokens=n, eos_token_id=eos, min_length=MIN_LEN, num_beams=NB,
                     use_nucleus_sampling=sample, top_p=0.9, generator=torch.Generator(device="cuda").manual_seed(0))
                 best, out = {}, None
+                torch.cuda.reset_peak_memory_stats()
                 for n in (MAX_NEW, 1):
                     model.enable_decode_graphs(graphed, sampling=sample)
                     for _ in range(2):
@@ -138,17 +172,23 @@ with torch.no_grad():
                         torch.cuda.synchronize(); dt = time.time() - t0
                         best[n] = min(best.get(n, dt), dt)
                         out = o if n == MAX_NEW else out
+                    if n == MAX_NEW:
+                        peak = torch.cuda.max_memory_allocated() / 2**30
                     model.enable_decode_graphs(False)
                     torch.cuda.empty_cache()
-                return 1e3 * (best[MAX_NEW] - best[1]) / (MAX_NEW - 1), out
+                return 1e3 * (best[MAX_NEW] - best[1]) / (MAX_NEW - 1), out, peak
 
             key = f"{shape}_B{B}"
             rows[f"{key}_prompt_tokens"] = ids.shape[1]
-            rows[f"{key}_eager_ms_per_token"], out_e = per_token(False)
-            rows[f"{key}_graphed_ms_per_token"], out_g = per_token(True)
-            rows[f"{key}_ids_equal"] = bool(torch.equal(out_e, out_g))
-            rows[f"{key}_sample_eager_ms_per_token"], _ = per_token(False, sample=True)
-            rows[f"{key}_sample_graphed_ms_per_token"], _ = per_token(True, sample=True)
+            eager = not (shape == "long" and B == 4)                    # the eager loop's cache does not fit
+            outs = {}
+            for sample, name in ((False, ""), (True, "sample_")):
+                for graphed in (False, True) if eager else (True,):
+                    run = name + ("graphed" if graphed else "eager")
+                    ms, outs[run], peak = per_token(graphed, sample=sample)
+                    rows[f"{key}_{run}_ms_per_token"], rows[f"{key}_{run}_peak_gb"] = ms, peak
+            if eager:
+                rows[f"{key}_ids_equal"] = bool(torch.equal(outs["eager"], outs["graphed"]))
             del vis
             torch.cuda.empty_cache()
 rows.update(beams=NB, new_tokens=MAX_NEW, min_length=MIN_LEN)
