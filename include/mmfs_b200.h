@@ -534,6 +534,53 @@ int mmfs_image_reentry(const float *images, float *out, int N, int C, int H, int
 int mmfs_linear_fp8(const void *x, const uint8_t *w8, const float *scale, const void *bias, const void *residual,
                     void *out, int M, int N, int K, int dtype, void *stream);
 
+/*
+ * FP8 KV cache.  K and V are stored as float8 e4m3 ("e4m3fn") bytes, (rows, T_max, H, hd), with one fp32 scale per
+ * (row, position, head) in (rows, T_max, >= H) scale tensors.  A head vector x is stored as x8 = e4m3(x / s), round to
+ * nearest even, with s the least power of two such that max |x| / s <= 448 (1 for an all-zero vector); x8 * s is exact
+ * in bf16 and fp16.  dtype (of q, k, v and the outputs) is MMFS_F32, MMFS_BF16 or MMFS_F16 (others:
+ * MMFS_EUNSUPPORTED).  Strides are in elements.
+ *
+ * mmfs_rope_qk_append_fp8: mmfs_rope_qk_append writing to an FP8 cache.  q is rotated in place, bit-identical to
+ * mmfs_rope_qk_append; each (token, head) vector of rotated k, and of v, is quantised; the bytes go to
+ * k_cache / v_cache[b, slot + t] and the scales to k_scale / v_scale[b, slot + t, h] (scale_bs / scale_ts: scale row and
+ * position strides); k and v are overwritten in place with x8 * s.  hd even and <= 256, scale_ts >= H.
+ */
+int mmfs_rope_qk_append_fp8(void *q, void *k, void *v, const float *cos_table, const float *sin_table,
+                            const int64_t *position_ids, uint8_t *k_cache, uint8_t *v_cache, float *k_scale, float *v_scale,
+                            const int64_t *slot_dev, long slot_host, long n_tokens, int T_len, int H, int hd, int q_stride,
+                            int k_stride, int v_stride, long cache_bs, long cache_ts, long scale_bs, long scale_ts,
+                            int pos_per_batch, int dtype, void *stream);
+/*
+ * mmfs_attn_decode over an FP8 cache: score_j = (q . k8_j) * (k_scale[j] * scale), and P V accumulates
+ * (p_j * v_scale[j]) * v8_j, all sums fp32.  K and V share strides (kv_bs, kv_ts), and so do their scales (s_bs,
+ * s_ts).  key_mask, causal, past and scratch (mmfs_attn_decode_scratch_floats(B, H, Tkv, hd) floats) as in
+ * mmfs_attn_decode; a fully masked row gives zeros and a masked slot is never read into the sums.  Two calls give
+ * bit-identical outputs; capturable in a CUDA graph.  MMFS_EINVAL: null pointers, bad shapes, negative past;
+ * MMFS_EUNSUPPORTED: hd % 32 != 0 or > 256, misaligned q / K / V rows (16 bytes), s_ts < H, B or H > 65535.
+ */
+int mmfs_attn_decode_fp8(const void *q, const uint8_t *k, const uint8_t *v, const float *k_scale, const float *v_scale,
+                         void *out, const uint8_t *key_mask, float *scratch, int B, int H, int Tkv, int hd, long q_bs,
+                         long kv_bs, long kv_ts, long s_bs, long s_ts, long o_bs, float scale, int causal, int past,
+                         int dtype, void *stream);
+/*
+ * mmfs_attn_decode_shared over FP8 prefix and gen caches, each with its scales (prefix: p_* and ps_* strides; gen: g_*
+ * and gs_*).  The output is bit-identical to mmfs_attn_decode_fp8's over the equivalent replicated cache.  Refusals as
+ * mmfs_attn_decode_shared and mmfs_attn_decode_fp8.
+ */
+int mmfs_attn_decode_shared_fp8(const void *q, const uint8_t *k_prefix, const uint8_t *v_prefix, const float *ks_prefix,
+                                const float *vs_prefix, const uint8_t *k_gen, const uint8_t *v_gen, const float *ks_gen,
+                                const float *vs_gen, void *out, const uint8_t *key_mask, const long long *prefix_len,
+                                float *scratch, int R, int G, int H, int Tkv, int Tp, int max_new, int hd, long q_bs,
+                                long p_bs, long p_ts, long ps_bs, long ps_ts, long g_bs, long g_ts, long gs_bs, long gs_ts,
+                                long o_bs, float scale, int causal, int past, int dtype, void *stream);
+/*
+ * out[b, t, h, :] = x8[b, t, h, :] * scale[b, t, h] for (B, T, H, hd) e4m3 x8, into f32 / bf16 / fp16 out (exact).  hd % 16
+ * == 0, 16-byte aligned rows, s_ts >= H (MMFS_EUNSUPPORTED otherwise).
+ */
+int mmfs_kv_dequantize_fp8(const uint8_t *x8, const float *scale, void *out, int B, int T_len, int H, int hd, long x_bs,
+                           long x_ts, long s_bs, long s_ts, long o_bs, long o_ts, int dtype, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -66,6 +66,10 @@ SIGNATURES = {
     "mmfs_kv_beam_reorder": (_I, [_P, _I, _L, _I, _L, _L, _L, _I] + [_P] * 4 + [_I, _P]),
     "mmfs_image_reentry": (_I, [_P, _P] + [_I] * 5 + [_P]),
     "mmfs_linear_fp8": (_I, [_P] * 6 + [_I] * 4 + [_P]),
+    "mmfs_rope_qk_append_fp8": (_I, [_P] * 11 + [_L, _L] + [_I] * 6 + [_L] * 4 + [_I, _I, _P]),
+    "mmfs_attn_decode_fp8": (_I, [_P] * 8 + [_I] * 4 + [_L] * 6 + [_F, _I, _I, _I, _P]),
+    "mmfs_attn_decode_shared_fp8": (_I, [_P] * 13 + [_I] * 7 + [_L] * 10 + [_F, _I, _I, _I, _P]),
+    "mmfs_kv_dequantize_fp8": (_I, [_P] * 3 + [_I] * 4 + [_L] * 6 + [_I, _P]),
 }
 BEAM_MAX_BEAMS, BEAM_MAX_EOS = 8, 4                  # limits of mmfs_beam_select / mmfs_beam_sample / mmfs_kv_beam_reorder
 LINEAR_FP8_MAX_M = 64                                # rows of x mmfs_linear_fp8 takes

@@ -9,7 +9,7 @@ from typing import List, Optional
 import torch
 
 from . import ops
-from .llama_mmfs import PreparedVision, SharedPrefixKV, StaticKV
+from .llama_mmfs import PreparedVision, SharedPrefixKV, StaticKV, kv_storage
 
 _BEAM_SAMPLE_TOP_K = 50              # transformers 4.31 GenerationConfig.top_k, which the reference never overrides
 
@@ -64,11 +64,10 @@ def _prefill_beams(model, p: Prompt, rep, past, vision):
     mask, last position id and last cross-attention row."""
     B, L, _ = p.mm_embeds.shape
     pre = p.cache if p.cache is not None else \
-        model.mm_decoder.static_cache(B, L, dtype=p.mm_embeds.dtype, device=p.mm_embeds.device)
+        model.mm_decoder.static_cache(B, L, dtype=p.mm_embeds.dtype, device=p.mm_embeds.device, kv_fp8=model._kv_fp8)
     _, logits = _prefill(model, p, pre, vision)
     for dst, src in zip(past, pre):                                     # a copy of the prompt rows, no recompute
-        dst.k[:, :L].copy_(src.k[:, :L].index_select(0, rep))
-        dst.v[:, :L].copy_(src.v[:, :L].index_select(0, rep))
+        dst.copy_rows_(src, rep, L)
         dst.length = L
     return (t.index_select(0, rep) for t in (logits, p.attention_mask, p.position_ids[:, -1:], p.cross[:, -1:, :]))
 
@@ -85,6 +84,9 @@ def generate_texts(model, text_ids, visual_output, num_image_per_seq, max_num_im
 def decode(model, p: Prompt, max_new_tokens, pad_token_id, static_cache, min_length, repetition_penalty,
            use_nucleus_sampling, top_p, temperature, generator, num_beams, length_penalty, num_return_sequences):
     """The graphed decoder where ``enable_decode_graphs`` is on and the kernels take the shape, else the eager loop."""
+    if model._kv_fp8 and not static_cache:
+        raise ValueError("static_cache=False keeps a 16-bit torch.cat cache: it cannot hold the FP8 KV cache that "
+                         "enable_fp8_kv_cache() selects")
     V = model.text_decoder.head.weight.shape[0]
     graphs = (model._decode_graphs is not None and p.mm_embeds.is_cuda and max_new_tokens > 0 and
               (not use_nucleus_sampling or model._decode_graph_sampling))
@@ -114,7 +116,8 @@ def token_loop(model, p: Prompt, max_new_tokens, pad_token_id, static_cache, min
     if p.cache is not None:
         past = p.cache
     else:
-        past = model.mm_decoder.static_cache(B, L + max_new_tokens, dtype=mm_embeds.dtype, device=mm_embeds.device) if static_cache else None
+        past = model.mm_decoder.static_cache(B, L + max_new_tokens, dtype=mm_embeds.dtype, device=mm_embeds.device,
+                                             kv_fp8=model._kv_fp8) if static_cache else None
     past, logits = _prefill(model, p, past, feats)
     new_ids = []
     finished = torch.zeros((B,), dtype=torch.bool, device=mm_embeds.device)
@@ -177,7 +180,8 @@ def beam_search(model, p: Prompt, max_new_tokens, pad_token_id, min_length, num_
     expand = num_return if sample else 1
     B = B0 * expand                                                            # independent beam searches
     rep = torch.arange(B0, device=dev).repeat_interleave(expand * nb)         # beam row -> prompt
-    past = model.mm_decoder.static_cache(B * nb, L + max_new_tokens, dtype=mm_embeds.dtype, device=dev)
+    past = model.mm_decoder.static_cache(B * nb, L + max_new_tokens, dtype=mm_embeds.dtype, device=dev,
+                                         kv_fp8=model._kv_fp8)
     logits, mask, pos, last_cross = _prefill_beams(model, p, rep, past, p.vision if p.vision is not None else p.feats)
     feats_b = p.feats.index_select(0, rep)
 
@@ -234,8 +238,7 @@ def beam_search(model, p: Prompt, max_new_tokens, pad_token_id, min_length, num_
         if all(done) or step_idx == max_new_tokens - 1:
             break
         for c in past:                                                        # _reorder_cache
-            n = c.length
-            c.k[:, :n].copy_(c.k.index_select(0, row_t)[:, :n]); c.v[:, :n].copy_(c.v.index_select(0, row_t)[:, :n])
+            c.reorder_rows_(row_t, c.length)
         mask = torch.cat([mask.index_select(0, row_t), torch.ones((B * nb, 1), dtype=mask.dtype, device=dev)], dim=1)
         pos = pos.index_select(0, row_t) + 1
         step = model.mm_decoder(inputs_embeds=model.mm_decoder.embed_tokens(tok_t[:, None]), attention_mask=mask,
@@ -317,7 +320,7 @@ def _graphed_decoder(model, p: Prompt, max_new_tokens, pad_id, min_length, sampl
     t_max = ((L + max_new_tokens + 255) // 256) * 256                  # cache-length bucket: one graph serves nearby prompts
     mode = ("beam_sample" if sample else "beam") if num_beams > 1 else ("sample" if sample else "greedy")
     key = (B, t_max, tuple(p.feats.shape), p.mm_embeds.dtype, p.mm_embeds.device, tuple(p.eos_ids), int(pad_id),
-           int(min_length), int(max_new_tokens), int(num_beams), mode)
+           int(min_length), int(max_new_tokens), bool(model._kv_fp8), int(num_beams), mode)
     dec = model._decode_graphs.get(key)
     if dec is None:
         if len(model._decode_graphs) >= 4:
@@ -402,8 +405,7 @@ class _GraphedDecoder:
     def _clear_unused(self, L):
         """Zero the cache positions from ``L`` on: masked slots must hold finite numbers."""
         for c in self.past:
-            c.k[:, L:].zero_()
-            c.v[:, L:].zero_()
+            c.zero_from_(L)
 
     def _prefill_done(self, L, reset):
         """After the prefill: zero the unused cache slots, capture the step graph once, reset the per-call state."""
@@ -443,7 +445,7 @@ class TokenDecoder(_GraphedDecoder):
     sampling, one seed per call from ``seed``.  ``generate`` replays the graph ``max_new`` times."""
 
     def __init__(self, model, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, sample):
-        self.past = model.mm_decoder.static_cache(B, t_max, dtype=dtype, device=device)
+        self.past = model.mm_decoder.static_cache(B, t_max, dtype=dtype, device=device, kv_fp8=model._kv_fp8)
         super().__init__(model, B, B, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, sample)
         self.out_ids = torch.zeros((B, max_new), dtype=torch.long, device=device)
         self.params = torch.ones((3,), dtype=torch.float32, device=device)   # penalty, temperature, top_p
@@ -495,13 +497,18 @@ class BeamDecoder(_GraphedDecoder):
         cfg, layers = model.mm_decoder.config, model.mm_decoder.layers
         n, H = 2 * len(layers), cfg.num_attention_heads
         hd = cfg.hidden_size // H
-        self.prefix = torch.zeros((n, P, t_max - max_new, H, hd), dtype=dtype, device=device)
-        self.gen = torch.zeros((n, R, max_new, H, hd), dtype=dtype, device=device)
-        self.prefix_kv = [StaticKV.over(self.prefix[2 * i], self.prefix[2 * i + 1]) for i in range(len(layers))]
+        fp8 = model._kv_fp8
+        self.prefix, self.prefix_scale = kv_storage(n, P, t_max - max_new, H, hd, dtype, device, fp8)
+        self.gen, self.gen_scale = kv_storage(n, R, max_new, H, hd, dtype, device, fp8)
+        ps, gs = (self.prefix_scale, self.gen_scale) if fp8 else ([None] * n, [None] * n)
+        self.prefix_kv = [StaticKV.over(self.prefix[2 * i], self.prefix[2 * i + 1], ps[2 * i], ps[2 * i + 1])
+                          for i in range(len(layers))]
         self.prefix_len = torch.zeros((1,), dtype=torch.long, device=device)
         super().__init__(model, B, R, t_max, feats_shape, dtype, device, eos_ids, pad_id, min_length, max_new, sample)
         self.past = [SharedPrefixKV(self.prefix[2 * i], self.prefix[2 * i + 1], self.gen[2 * i], self.gen[2 * i + 1],
-                                    self.prefix_len, self.step) for i in range(len(layers))]
+                                    self.prefix_len, self.step,
+                                    (ps[2 * i], ps[2 * i + 1], gs[2 * i], gs[2 * i + 1]) if fp8 else None)
+                     for i in range(len(layers))]
         # repetition_penalty, length_penalty (+ temperature, top_p when sampling)
         self.params = torch.ones((4 if sample else 2,), dtype=torch.float64, device=device)
         self.beam_scores = torch.zeros((R,), dtype=torch.float32, device=device)
@@ -527,6 +534,8 @@ class BeamDecoder(_GraphedDecoder):
                             self.parent, self.finished, self.hyp_scores, self.hyp_ids, self.hyp_meta, self.scratch,
                             self.nb, eos=self.eos, pad_id=self.pad_id, min_length=self.min_length)
         ops.kv_beam_reorder(self.gen, self.parent, self.step, self.step, self.nb, self.max_new, done=self.finished)
+        if self.gen_scale is not None:
+            ops.kv_beam_reorder(self.gen_scale, self.parent, self.step, self.step, self.nb, self.max_new, done=self.finished)
 
     def _set_graph_mode(self, on: bool, length: int = 0):
         pass                                                               # SharedPrefixKV is graph-only: slot = step
@@ -534,6 +543,9 @@ class BeamDecoder(_GraphedDecoder):
     def _clear_unused(self, L):
         self.prefix[:, :, L:].zero_()
         self.gen.zero_()
+        if self.gen_scale is not None:
+            self.prefix_scale[:, :, L:].zero_()
+            self.gen_scale.zero_()
 
     def _step(self):
         super()._step()

@@ -109,7 +109,7 @@ class InterleavedSession:
         self.n_img = int(num_image_per_seq.reshape(-1)[0])
         self.capacity = int(capacity)
         w = model.mm_decoder.embed_tokens.weight
-        self.cache = model.mm_decoder.static_cache(1, self.capacity, dtype=w.dtype, device=dev)
+        self.cache = model.mm_decoder.static_cache(1, self.capacity, dtype=w.dtype, device=dev, kv_fp8=model._kv_fp8)
         self.hidden = torch.zeros((1, self.capacity, w.shape[1]), dtype=w.dtype, device=dev)
         self.cached = 0
         self.vis_embed, self.ms = None, None

@@ -167,13 +167,18 @@ class LlamaMLP(nn.Module):
 class StaticKV:
     """Pre-allocated key / value cache of one layer (extension): ``k``, ``v`` (B, T_max, H, hd) and the number of valid
     positions.  Passing it as ``past_key_value`` makes the layer append IN PLACE instead of the reference's
-    ``torch.cat`` (modeling_llama_mmfs.py:236-239), which re-copies the whole cache of every layer for every token."""
+    ``torch.cat`` (modeling_llama_mmfs.py:236-239), which re-copies the whole cache of every layer for every token.
 
-    __slots__ = ("k", "v", "length", "slot")
+    With ``kv_fp8`` (``InterleavedForward.enable_fp8_kv_cache``) ``k`` and ``v`` hold float8_e4m3fn bytes and
+    ``k_scale`` / ``v_scale`` (B, T_max, ``ops.kv_scale_heads(H)``) fp32 one scale per (row, position, head)
+    (``ops.quantize_kv_fp8``); for a 16-bit cache they are None.  The row operations below carry the scales along."""
 
-    def __init__(self, batch, max_len, heads, head_dim, dtype, device):
-        self.k = torch.empty((batch, max_len, heads, head_dim), dtype=dtype, device=device)
-        self.v = torch.empty_like(self.k)
+    __slots__ = ("k", "v", "k_scale", "v_scale", "length", "slot")
+
+    def __init__(self, batch, max_len, heads, head_dim, dtype, device, kv_fp8=False):
+        kv, scales = kv_storage(2, batch, max_len, heads, head_dim, dtype, device, kv_fp8, torch.empty)
+        self.k, self.v = kv[0], kv[1]
+        self.k_scale, self.v_scale = (None, None) if scales is None else (scales[0], scales[1])
         self.length = 0
         # CUDA-graph decode (the graphed decoders of generation.py): a (1,) int64 DEVICE tensor holding the slot the
         # next token is written to.  While set, a step appends at ``slot`` (index_copy_, no host integer involved),
@@ -181,12 +186,48 @@ class StaticKV:
         self.slot = None
 
     @classmethod
-    def over(cls, k, v) -> "StaticKV":
+    def over(cls, k, v, k_scale=None, v_scale=None) -> "StaticKV":
         """An empty cache over existing (B, T_max, H, hd) storage, e.g. views of one tensor holding every layer's k and v
         (the graphed beam search reorders all of them in one launch)."""
         c = cls.__new__(cls)
-        c.k, c.v, c.length, c.slot = k, v, 0, None
+        c.k, c.v, c.k_scale, c.v_scale, c.length, c.slot = k, v, k_scale, v_scale, 0, None
         return c
+
+    @property
+    def fp8(self) -> bool:
+        return self.k_scale is not None
+
+    def _tensors(self):
+        if self.k_scale is None:
+            return self.k, self.v
+        return self.k.view(torch.uint8), self.v.view(torch.uint8), self.k_scale, self.v_scale   # bytes: moved as they are
+
+    def copy_rows_(self, src: "StaticKV", rows: torch.Tensor, n: int) -> None:
+        """Positions ``[:n]`` of row i become those of ``src``'s row ``rows[i]`` (the prompt's rows copied to its beams)."""
+        if src.fp8 != self.fp8:
+            raise RuntimeError("StaticKV.copy_rows_: an FP8 and a 16-bit cache do not mix")
+        for dst, s in zip(self._tensors(), src._tensors()):
+            dst[:, :n].copy_(s[:, :n].index_select(0, rows))
+
+    def reorder_rows_(self, rows: torch.Tensor, n: int) -> None:
+        """Positions ``[:n]`` of row i become those of row ``rows[i]`` (beam search's ``_reorder_cache``)."""
+        for t in self._tensors():
+            t[:, :n].copy_(t.index_select(0, rows)[:, :n])
+
+    def zero_from_(self, n: int) -> None:
+        """Zero positions ``n`` on: masked slots must hold finite numbers."""
+        for t in self._tensors():
+            t[:, n:].zero_()
+
+
+def kv_storage(n, rows, max_len, heads, head_dim, dtype, device, kv_fp8=False, alloc=torch.zeros):
+    """(data, scales) of ``n`` K or V caches in one tensor each (one launch of ``ops.kv_beam_reorder`` moves them all):
+    data (n, rows, max_len, H, hd) of ``dtype``, or with ``kv_fp8`` float8_e4m3fn bytes and scales fp32
+    (n, rows, max_len, ``ops.kv_scale_heads(H)``), else None."""
+    data = alloc((n, rows, max_len, heads, head_dim), dtype=torch.float8_e4m3fn if kv_fp8 else dtype, device=device)
+    if not kv_fp8:
+        return data, None
+    return data, torch.ones((n, rows, max_len, ops.kv_scale_heads(heads)), dtype=torch.float32, device=device)
 
 
 class SharedPrefixKV:
@@ -196,14 +237,18 @@ class SharedPrefixKV:
     ``prefix_len`` and in ``k_gen[r, p - prefix_len]`` from there on.  ``prefix_len`` and ``slot`` (where the next
     token's key / value go in ``k_gen``) are (1,) int64 DEVICE tensors, so one captured step serves every prompt length
     and step.  A step appends one token per row and attends over all ``length + 1`` = T_p + max_new positions under the
-    caller's key mask (``ops.attention_decode_shared``); there is no eager use."""
+    caller's key mask (``ops.attention_decode_shared``); there is no eager use.
 
-    __slots__ = ("k", "v", "k_gen", "v_gen", "G", "prefix_len", "slot")
+    An FP8 cache (``StaticKV``'s format) also carries the prefix's ``k_scale`` / ``v_scale`` and the generated
+    positions' ``ks_gen`` / ``vs_gen``, and attends through ``ops.attention_decode_shared_fp8``."""
 
-    def __init__(self, k, v, k_gen, v_gen, prefix_len, slot):
+    __slots__ = ("k", "v", "k_gen", "v_gen", "G", "prefix_len", "slot", "k_scale", "v_scale", "ks_gen", "vs_gen")
+
+    def __init__(self, k, v, k_gen, v_gen, prefix_len, slot, scales=None):
         self.k, self.v, self.k_gen, self.v_gen = k, v, k_gen, v_gen
         self.G = k_gen.shape[0] // k.shape[0]
         self.prefix_len, self.slot = prefix_len, slot
+        self.k_scale, self.v_scale, self.ks_gen, self.vs_gen = scales if scales is not None else (None,) * 4
 
     @property
     def length(self):
@@ -270,6 +315,9 @@ class LlamaAttention(nn.Module):
         if position_ids is None:
             position_ids = torch.arange(past, past + T, device=hidden_states.device)
         cos, sin = self.rope_tables(hidden_states.device, past + T)
+        if static and past_key_value.k_scale is not None:
+            return self._forward_fp8(q, k, v, cos, sin, position_ids, past_key_value, past, attention_mask, residual,
+                                     inplace)
         if shared:                                              # graph decode over a shared prompt: append to the row's gen
             if T != 1:
                 raise RuntimeError("SharedPrefixKV is a graph-decode cache (one token per step): prefill into its prefix "
@@ -310,6 +358,43 @@ class LlamaAttention(nn.Module):
             ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)   # (B, T, H*hd)
         out = decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace)
         return out, None, present
+
+    def _forward_fp8(self, q, k, v, cos, sin, position_ids, c, past, attention_mask, residual, inplace):
+        """The layer over an FP8 cache (``StaticKV`` / ``SharedPrefixKV`` with scales).  ``ops.rope_qk_append_fp8_``
+        appends the rotated keys and the values as E4M3 and rewrites the k / v views with ``x8 * scale``; then a decode
+        step (T == 1) attends over the FP8 cache directly, a prefill from position 0 runs the 16-bit attention on the
+        rewritten views, and a prefill after cached positions runs it on the cache's first ``past + T`` positions
+        dequantised into a workspace.  Every path sees the keys and values ``x8 * scale``."""
+        B, T = q.shape[:2]
+        shared = isinstance(c, SharedPrefixKV)
+        if (shared or c.slot is not None) and T != 1:
+            raise RuntimeError("a graph-decode cache (SharedPrefixKV, StaticKV.slot) takes one token per step")
+        key_mask = attention_mask
+        if attention_mask is not None and attention_mask.dim() == 4:
+            key_mask = attention_mask[:, 0, -1, :] > (torch.finfo(attention_mask.dtype).min / 2)
+        if shared:
+            ops.rope_qk_append_fp8_(q, k, v, cos, sin, position_ids, c.k_gen, c.v_gen, c.ks_gen, c.vs_gen, c.slot)
+            ctx = ops.attention_decode_shared_fp8(q, c.k, c.v, c.k_scale, c.v_scale, c.k_gen, c.v_gen, c.ks_gen, c.vs_gen,
+                                                  c.prefix_len, key_mask=key_mask, past=past)
+        else:
+            if c.slot is not None:                              # graph decode: device-side slot, whole buffer visible
+                slot, n, past = c.slot, c.k.shape[1], c.k.shape[1] - 1
+            else:
+                if past + T > c.k.shape[1]:
+                    raise RuntimeError(f"StaticKV of {c.k.shape[1]} positions cannot take {past} + {T}")
+                slot, n = past, past + T
+                c.length = n
+            ops.rope_qk_append_fp8_(q, k, v, cos, sin, position_ids, c.k, c.v, c.k_scale, c.v_scale, slot)
+            if T == 1:
+                ctx = ops.attention_decode_fp8(q, c.k[:, :n], c.v[:, :n], c.k_scale[:, :n], c.v_scale[:, :n],
+                                               key_mask=key_mask, past=past)
+            else:
+                if past > 0:
+                    k = ops.kv_dequantize_fp8(c.k[:, :n], c.k_scale[:, :n], q.dtype)
+                    v = ops.kv_dequantize_fp8(c.v[:, :n], c.v_scale[:, :n], q.dtype)
+                ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)
+        out = decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace)
+        return out, None, c
 
     def _forward_training(self, hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual):
         """The prefill under autograd: QKV GEMM -> RoPE -> causal attention (saving O and the row log-sum-exp) -> o_proj,
@@ -477,11 +562,12 @@ class LlamaModel(nn.Module):
         self.norm = LlamaRMSNorm(config.hidden_size, eps=config.rms_norm_eps)
         self.gradient_checkpointing = False
 
-    def static_cache(self, batch: int, max_len: int, dtype=None, device=None):
-        """One ``StaticKV`` per layer, to be passed as ``past_key_values`` (prefill with length 0, then decode)."""
+    def static_cache(self, batch: int, max_len: int, dtype=None, device=None, kv_fp8: bool = False):
+        """One ``StaticKV`` per layer, to be passed as ``past_key_values`` (prefill with length 0, then decode);
+        ``kv_fp8``: E4M3 keys and values with per-head scales (see ``StaticKV``)."""
         p = self.embed_tokens.weight
         H = self.config.num_attention_heads
-        return [StaticKV(batch, max_len, H, self.config.hidden_size // H, dtype or p.dtype, device or p.device)
+        return [StaticKV(batch, max_len, H, self.config.hidden_size // H, dtype or p.dtype, device or p.device, kv_fp8)
                 for _ in self.layers]
 
     @torch.no_grad()

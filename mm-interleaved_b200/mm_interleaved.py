@@ -415,6 +415,7 @@ class InterleavedForward(nn.Module):
         self.image_decoder = image_decoder                                                # ImageDecoder or None
         self._decode_graphs = None                                                        # enable_decode_graphs()
         self._decode_graph_sampling = False
+        self._kv_fp8 = False                                                              # enable_fp8_kv_cache()
 
     def enable_decode_graphs(self, enabled: bool = True, sampling: bool = False) -> "InterleavedForward":
         """Greedy ``generate_texts`` then replays ONE captured CUDA graph per generated token (embedding -> 40 layers ->
@@ -460,6 +461,23 @@ class InterleavedForward(nn.Module):
         for m in [*self.mm_decoder.modules(), self.text_decoder]:
             if isinstance(m, (LlamaAttention, LlamaMLP, TextDecoder)):
                 m._fp8 = cache()
+        if self._decode_graphs is not None:
+            self._decode_graphs = {}
+        return self
+
+    def enable_fp8_kv_cache(self, enabled: bool = True) -> "InterleavedForward":
+        """Store the decoder's KV cache in FP8: every key (after RoPE) and value enters the cache as E4M3 bytes with one
+        power-of-two fp32 scale per (row, position, head) (``ops.quantize_kv_fp8``), which halves the cache's memory and
+        the bytes a decode step's attention reads.  The eager token and beam loops, the graphed decoders and
+        ``generate_interleaved`` all allocate FP8 caches while it is on.
+
+        This selects different numerics: generation computes exactly what the 16-bit model computes when every key and
+        value is replaced by ``x8 * scale`` on entering the cache (the prefill's attention over its own positions
+        included), up to the order of the fp32 sums, so tokens may differ from the 16-bit cache's.  ``forward``,
+        ``generate_scores``, ``generate_images``, the training path and the MMFS cross-attention keep no cache and stay
+        16-bit.  ``generate_texts(static_cache=False)`` raises ``ValueError`` while it is on.  Off by default and
+        independent of ``enable_fp8_decode``; toggling drops the captured decode graphs."""
+        self._kv_fp8 = bool(enabled)
         if self._decode_graphs is not None:
             self._decode_graphs = {}
         return self

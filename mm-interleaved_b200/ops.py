@@ -938,3 +938,176 @@ def linear_fp8(x: torch.Tensor, w8: torch.Tensor, scale: torch.Tensor, bias=None
     _lib.check(rc, "linear_fp8")
     launch_counter[0] += 1
     return out
+
+
+# ---- FP8 KV cache (csrc/kv_fp8_sm100.cu) ------------------------------------------------------------------------------
+
+_KV_FP8_DTYPES = (torch.float32, torch.bfloat16, torch.float16)    # of the model's q / k / v next to an FP8 cache
+
+
+def kv_scale_heads(H: int) -> int:
+    """Heads in a scale row of an FP8 KV cache: H rounded up to a multiple of 4, so that every position's scale row is a
+    multiple of 16 bytes (``kv_beam_reorder`` moves whole 16-byte rows)."""
+    return (H + 3) // 4 * 4
+
+
+def quantize_kv_fp8(x: torch.Tensor):
+    """(x8, scale) of keys or values ``x`` (..., H, hd): ``x8`` float8_e4m3fn (..., H, hd), ``scale`` fp32 (..., H), one per
+    head vector, with ``x ~= x8 * scale[..., None]``.  Runs on the CPU too, and is the reference of the cache kernels.
+
+    The rule of ``quantize_fp8_per_channel``: each scale is the least power of two with ``amax / scale <= 448``, 1 for an
+    all-zero vector.  ``x / scale`` is then exact, the cast rounds to nearest even and never saturates, and
+    ``x8 * scale`` is exactly representable in bf16, and in fp16 wherever the scale is at least 2^-15 (a head vector of
+    fp16 values all below 2^-7 may fall into fp16's subnormal range)."""
+    _require(x.dim() >= 2 and x.dtype in (torch.float16, torch.bfloat16, torch.float32),
+             "quantize_kv_fp8: x must be a (..., H, hd) fp16 / bf16 / fp32 tensor")
+    xf = x.detach().float()
+    amax = xf.abs().amax(dim=-1)
+    m, e = torch.frexp(amax)                                         # amax = m * 2^e, m in [0.5, 1); 448 = 0.875 * 2^9
+    e = torch.where(m <= 0.875, e - 9, e - 8)
+    scale = torch.exp2(e.double()).float()                           # exact: a power of two in fp32's range
+    scale = torch.where(amax > 0, scale, torch.ones_like(scale)).contiguous()
+    x8 = (xf / scale[..., None]).to(torch.float8_e4m3fn)
+    return x8, scale
+
+
+def _check_fp8_cache(what, k8, v8, ks, vs, rows, H, hd, dev):
+    """An FP8 K / V pair (rows, T, H, hd) with dense heads and shared strides, and its fp32 (rows, T, >= H) scales."""
+    for t in (k8, v8):
+        _require(t.is_cuda and t.device == dev and t.dtype == torch.float8_e4m3fn and t.dim() == 4 and t.shape[0] == rows
+                 and tuple(t.shape[2:]) == (H, hd) and t.stride(3) == 1 and t.stride(2) == hd,
+                 f"{what}: K / V must be float8_e4m3fn ({rows}, T, {H}, {hd}) CUDA tensors with dense heads")
+    _require(k8.shape == v8.shape and k8.stride() == v8.stride(), f"{what}: K and V must share their shape and strides")
+    for t in (ks, vs):
+        _require(t.is_cuda and t.device == dev and t.dtype == torch.float32 and t.dim() == 3
+                 and tuple(t.shape[:2]) == tuple(k8.shape[:2]) and t.shape[2] >= H and t.stride(2) == 1,
+                 f"{what}: scales must be fp32 ({rows}, T, >= {H}) CUDA tensors")
+    _require(ks.stride() == vs.stride(), f"{what}: K and V scales must share their strides")
+
+
+def rope_qk_append_fp8_(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor,
+                        position_ids: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, k_scale: torch.Tensor,
+                        v_scale: torch.Tensor, slot) -> None:
+    """``rope_qk_append_`` writing to an FP8 cache: q rotated in place (bit-identical to ``rope_qk_append_``); each
+    (token, head) vector of rotated k, and of v, quantised as ``quantize_kv_fp8`` does, its bytes written to
+    ``k_cache`` / ``v_cache[b, slot + t]`` and its scale to ``k_scale`` / ``v_scale[b, slot + t, h]``; k and v are
+    overwritten in place with ``x8 * scale``, so an attention over them reads what the cache holds.  ``slot``: int or a
+    (1,) int64 CUDA tensor (graphed decode)."""
+    B, T, H, hd = q.shape
+    inference_only("rope_qk_append_fp8_", q, k, v)
+    _require(q.dtype in _KV_FP8_DTYPES, "rope_qk_append_fp8_: q / k / v must be fp32 / bf16 / fp16")
+    for t in (q, k, v):
+        _require(t.is_cuda and t.dtype == q.dtype and tuple(t.shape) == (B, T, H, hd) and t.stride(3) == 1
+                 and t.stride(2) == hd and t.stride(0) == T * t.stride(1),
+                 "rope_qk_append_fp8_: q / k / v must be (B,T,H,hd) with dense heads and uniform token stride")
+    _check_fp8_cache("rope_qk_append_fp8_", k_cache, v_cache, k_scale, v_scale, B, H, hd, q.device)
+    _require(cos.dtype == torch.float32 and sin.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous()
+             and cos.shape[-1] == hd, "rope_qk_append_fp8_: cos / sin must be contiguous fp32 (max_pos, hd)")
+    pos = position_ids.to(torch.int64).contiguous()
+    per_batch = 1 if pos.numel() == B * T else 0
+    _require(per_batch or pos.numel() == T, "rope_qk_append_fp8_: position_ids must have B*T or T entries")
+    if isinstance(slot, torch.Tensor):
+        _require(slot.is_cuda and slot.dtype == torch.int64 and slot.numel() == 1,
+                 "rope_qk_append_fp8_: slot tensor must be (1,) int64 on the device")
+        slot_dev, slot_host = slot.data_ptr(), 0
+    else:
+        slot_dev, slot_host = None, int(slot)
+        _require(0 <= slot_host and slot_host + T <= k_cache.shape[1], "rope_qk_append_fp8_: slot + T exceeds the cache")
+    with torch.cuda.device(q.device):
+        rc = _lib.lib().mmfs_rope_qk_append_fp8(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), cos.data_ptr(), sin.data_ptr(), pos.data_ptr(), k_cache.data_ptr(),
+            v_cache.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(), slot_dev, slot_host, B * T, T, H, hd, q.stride(1),
+            k.stride(1), v.stride(1), k_cache.stride(0), k_cache.stride(1), k_scale.stride(0), k_scale.stride(1), per_batch,
+            _DTYPE_CODE[q.dtype], _stream())
+    _lib.check(rc, "rope_qk_append_fp8_")
+    launch_counter[0] += 1
+
+
+def _check_decode_q(what, q, rows, key_mask, Tkv):
+    _require(q.is_cuda and q.dtype in _KV_FP8_DTYPES and q.dim() == 4 and q.shape[0] == rows
+             and q.shape[1] == 1 and q.stride(3) == 1 and q.stride(2) == q.shape[3],
+             f"{what}: q must be an fp32 / bf16 / fp16 CUDA (rows, 1, H, hd) tensor with dense heads")
+    if key_mask is None:
+        return None
+    km = key_mask.to(torch.uint8).contiguous()
+    _require(tuple(km.shape) == (rows, Tkv), f"{what}: key_mask must be ({rows}, {Tkv})")
+    return km
+
+
+def attention_decode_fp8(q, k8, v8, k_scale, v_scale, key_mask=None, causal=True, past=0, scale=None) -> torch.Tensor:
+    """The decode branch of ``attention`` over an FP8 cache (``mmfs_attn_decode_fp8``): q (B, 1, H, hd) fp32 / bf16 / fp16,
+    k8 / v8 float8_e4m3fn (B, Tkv, H, hd) with their fp32 (B, Tkv, >= H) scales; key_mask, causal, past and scale as in
+    ``attention``.  Returns (B, 1, H*hd): softmax over ``(q . k8_j) * k_scale_j * scale``, then ``sum_j p_j * v_scale_j *
+    v8_j``, i.e. the 16-bit attention over keys and values ``x8 * scale`` up to the order of the fp32 sums."""
+    B, _, H, hd = q.shape
+    Tkv = k8.shape[1] if k8.dim() == 4 else 0
+    inference_only("attention_decode_fp8", q)
+    km = _check_decode_q("attention_decode_fp8", q, B, key_mask, Tkv)
+    _check_fp8_cache("attention_decode_fp8", k8, v8, k_scale, v_scale, B, H, hd, q.device)
+    scale = float(scale if scale is not None else hd ** -0.5)
+    out = torch.empty((B, 1, H, hd), dtype=q.dtype, device=q.device)
+    lib = _lib.lib()
+    scratch = torch.empty((lib.mmfs_attn_decode_scratch_floats(B, H, Tkv, hd),), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        rc = lib.mmfs_attn_decode_fp8(q.data_ptr(), k8.data_ptr(), v8.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
+                                      out.data_ptr(), km.data_ptr() if km is not None else None, scratch.data_ptr(), B, H,
+                                      Tkv, hd, q.stride(0), k8.stride(0), k8.stride(1), k_scale.stride(0), k_scale.stride(1),
+                                      out.stride(0), scale, 1 if causal else 0, int(past), _DTYPE_CODE[q.dtype], _stream())
+    _lib.check(rc, "attention_decode_fp8")
+    launch_counter[0] += 1
+    return out.view(B, 1, H * hd)
+
+
+def attention_decode_shared_fp8(q, k_prefix, v_prefix, ks_prefix, vs_prefix, k_gen, v_gen, ks_gen, vs_gen, prefix_len,
+                                key_mask=None, causal=True, past=0, scale=None) -> torch.Tensor:
+    """``attention_decode_shared`` over FP8 prefix (P, T_p, H, hd) and gen (R, max_new, H, hd) caches, each with its
+    fp32 scales (P, T_p, >= H) / (R, max_new, >= H).  Bit-identical to ``attention_decode_fp8`` over the equivalent
+    replicated cache."""
+    R, _, H, hd = q.shape
+    P = k_prefix.shape[0] if k_prefix.dim() == 4 else 0
+    Tp = k_prefix.shape[1] if k_prefix.dim() == 4 else 0
+    max_new = k_gen.shape[1] if k_gen.dim() == 4 else 0
+    Tkv = Tp + max_new
+    inference_only("attention_decode_shared_fp8", q)
+    km = _check_decode_q("attention_decode_shared_fp8", q, R, key_mask, Tkv)
+    _require(P > 0 and R % P == 0, "attention_decode_shared_fp8: the rows must be whole groups, one per prefix row")
+    _check_fp8_cache("attention_decode_shared_fp8", k_prefix, v_prefix, ks_prefix, vs_prefix, P, H, hd, q.device)
+    _check_fp8_cache("attention_decode_shared_fp8", k_gen, v_gen, ks_gen, vs_gen, R, H, hd, q.device)
+    _require(prefix_len.device == q.device and prefix_len.dtype == torch.int64 and prefix_len.numel() == 1,
+             "attention_decode_shared_fp8: prefix_len must be a (1,) int64 device tensor")
+    scale = float(scale if scale is not None else hd ** -0.5)
+    out = torch.empty((R, 1, H, hd), dtype=q.dtype, device=q.device)
+    lib = _lib.lib()
+    scratch = torch.empty((lib.mmfs_attn_decode_scratch_floats(R, H, Tkv, hd),), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        rc = lib.mmfs_attn_decode_shared_fp8(
+            q.data_ptr(), k_prefix.data_ptr(), v_prefix.data_ptr(), ks_prefix.data_ptr(), vs_prefix.data_ptr(),
+            k_gen.data_ptr(), v_gen.data_ptr(), ks_gen.data_ptr(), vs_gen.data_ptr(), out.data_ptr(),
+            km.data_ptr() if km is not None else None, prefix_len.data_ptr(), scratch.data_ptr(), R, R // P, H, Tkv, Tp,
+            max_new, hd, q.stride(0), k_prefix.stride(0), k_prefix.stride(1), ks_prefix.stride(0), ks_prefix.stride(1),
+            k_gen.stride(0), k_gen.stride(1), ks_gen.stride(0), ks_gen.stride(1), out.stride(0), scale, 1 if causal else 0,
+            int(past), _DTYPE_CODE[q.dtype], _stream())
+    _lib.check(rc, "attention_decode_shared_fp8")
+    launch_counter[0] += 1
+    return out.view(R, 1, H * hd)
+
+
+def kv_dequantize_fp8(x8: torch.Tensor, scale: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """``x8 * scale[..., None]`` of an FP8 cache slice x8 (B, T, H, hd) with scales (B, T, >= H), as a new contiguous
+    fp32 / bf16 / fp16 (B, T, H, hd) tensor (exact)."""
+    _require(dtype in _KV_FP8_DTYPES, "kv_dequantize_fp8: dtype must be fp32 / bf16 / fp16")
+    _require(x8.dim() == 4, "kv_dequantize_fp8: x8 must be (B, T, H, hd)")
+    B, T, H, hd = x8.shape
+    _require(x8.is_cuda and x8.dtype == torch.float8_e4m3fn and x8.stride(3) == 1 and x8.stride(2) == hd,
+             "kv_dequantize_fp8: x8 must be a float8_e4m3fn CUDA tensor with dense heads")
+    _require(scale.is_cuda and scale.device == x8.device and scale.dtype == torch.float32 and scale.dim() == 3
+             and tuple(scale.shape[:2]) == (B, T) and scale.shape[2] >= H and scale.stride(2) == 1,
+             f"kv_dequantize_fp8: scale must be fp32 ({B}, {T}, >= {H}) on x8's device")
+    out = torch.empty((B, T, H, hd), dtype=dtype, device=x8.device)
+    with torch.cuda.device(x8.device):
+        rc = _lib.lib().mmfs_kv_dequantize_fp8(x8.data_ptr(), scale.data_ptr(), out.data_ptr(), B, T, H, hd, x8.stride(0),
+                                               x8.stride(1), scale.stride(0), scale.stride(1), out.stride(0), out.stride(1),
+                                               _DTYPE_CODE[dtype], _stream())
+    _lib.check(rc, "kv_dequantize_fp8")
+    launch_counter[0] += 1
+    return out
