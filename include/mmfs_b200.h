@@ -249,6 +249,24 @@ int mmfs_attn_forward(const void *q, const void *k, const void *v, void *out, co
                       float scale, int causal, int past, int dtype, unsigned *work_counter, void *stream);
 
 /*
+ * Answer options scored against one stored context: prefix-shared, segment-causal attention.  q, k, v (P, Tq, H, hd):
+ * batch entry p holds Tq = G * seg_len queries, G segments of seg_len positions, and k / v are the segments' own keys
+ * and values; k_prefix, v_prefix (P, Tp, H, hd) the stored context.  Query i of entry p sees every prefix key j < Tp
+ * with prefix_mask[p, j] != 0 (prefix_mask (P, Tp) uint8, or NULL: all), and every own key j of its segment
+ * (j / seg_len == i / seg_len) with j <= i and key_mask[p, j] != 0 (key_mask (P, Tq) uint8, or NULL); a row that sees
+ * no key outputs 0.  out (P, Tq, H, hd).  Strides in elements, heads dense.  Routed like ops.attention: bf16 / f16 at
+ * hd 64 / 128 with Tq >= 16, 16-byte aligned pointers and strides and P, H <= 65535 run a variant of the wgmma kernel of
+ * mmfs_attn_forward (work_counter as there); everything else the generic kernel's variant (hd <= 256, f32 too).
+ * MMFS_EINVAL: a bad shape, seg_len < 1, Tq % seg_len != 0, null pointers, a misaligned work_counter;
+ * MMFS_EUNSUPPORTED: a dtype other than f32 / f16 / bf16, pointers not aligned to their element size.
+ */
+int mmfs_attn_prefix_shared(const void *q, const void *k, const void *v, const void *k_prefix, const void *v_prefix,
+                            void *out, const uint8_t *prefix_mask, const uint8_t *key_mask, int P, int H, int Tq, int Tp,
+                            int seg_len, int hd, long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts,
+                            long kp_bs, long kp_ts, long vp_bs, long vp_ts, long o_bs, long o_ts, float scale, int dtype,
+                            unsigned *work_counter, void *stream);
+
+/*
  * mmfs_attn_forward that also writes the row log-sum-exp the backward pass needs (training path).  Same arguments,
  * requirements and output (O is bit-identical to mmfs_attn_forward's), plus
  *   lse  (B, H, Tq) fp32, contiguous: lse[b,h,i] = ln sum_j exp(scale * q_i . k_j) over the keys row i sees, in

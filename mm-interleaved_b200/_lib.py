@@ -51,6 +51,7 @@ SIGNATURES = {
     "mmfs_attn_decode": (_I, [_P] * 6 + [_I] * 4 + [_L] * 6 + [_F, _I, _I, _I, _P]),
     "mmfs_attn_decode_shared": (_I, [_P] * 9 + [_I] * 7 + [_L] * 10 + [_F, _I, _I, _I, _P]),
     "mmfs_attn_forward": (_I, [_P] * 5 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
+    "mmfs_attn_prefix_shared": (_I, [_P] * 8 + [_I] * 6 + [_L] * 12 + [_F, _I, _P, _P]),
     "mmfs_attn_forward_lse": (_I, [_P] * 6 + [_I] * 5 + [_L] * 8 + [_F, _I, _I, _I, _P, _P]),
     "mmfs_attn_backward": (_I, [_P] * 11 + [_I] * 4 + [_L] * 16 + [_F, _I, _P]),
     "mmfs_attn_backward_general": (_I, [_P] * 11 + [_I] * 5 + [_L] * 16 + [_F, _I, _I, _P]),

@@ -33,13 +33,26 @@ constexpr int kConsumers = 256;
 //   Q [HD/64 boxes][128 rows][128 B] | K [2 stages][HD/64][64][128 B] | V [2][HD/64][64][128 B] | barriers | items [2]
 template <int HD> constexpr int attn_ctas_per_sm() { return HD == 64 ? 2 : 1; }
 
+// Prefix-shared segments (mmfs_attn_prefix_shared, option scoring over one stored context): batch entry b's Tq queries
+// are Tq / seg_len segments of seg_len positions.  Query i sees every prefix key j < Tp with prefix_mask[b, j] != 0, and
+// the own keys j of its segment with j <= i and key_mask[b, j] != 0 (p.key_mask, p.Tkv = Tq).  A 128-query item streams
+// its n_pre = ceil(Tp / 64) prefix tiles from map_kp / map_vp, then the own keys [segment start of its first query, its
+// last query] from map_k / map_v, 64 rows at a time from that (not tile-aligned) row.
+struct PrefixParams {
+    const uint8_t *prefix_mask;   // (B, Tp) or null
+    int Tp, seg_len, n_pre;
+};
+
 // LSE: also write the row log-sum-exp for the backward pass to `lse` (B, H, Tq), natural log (mmfs_attn_forward_lse).
 // The argument comes last so that the inference instantiation (LSE = false) compiles to the same code as before it.
-template <typename T, int HD, bool LSE>
+// PREFIX: the prefix-shared segment variant above; its arguments follow lse for the same reason, and the other
+// instantiations do not read them.
+template <typename T, int HD, bool LSE, bool PREFIX = false>
 __global__ void __launch_bounds__(kAttnThreads, attn_ctas_per_sm<HD>())
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const AttnParams p, unsigned *__restrict__ sched, int n_work,
-                float *__restrict__ lse) {
+                float *__restrict__ lse, const __grid_constant__ CUtensorMap map_kp,
+                const __grid_constant__ CUtensorMap map_vp, const PrefixParams pp) {
     constexpr int NBOX = HD / 64;
     constexpr uint32_t QBOX_BYTES = kBM * 128, KBOX_BYTES = kBN * 128;
     constexpr uint32_t Q_BYTES = NBOX * QBOX_BYTES, KV_BYTES = NBOX * KBOX_BYTES;
@@ -67,6 +80,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         int kv_end = p.Tkv;
         if (p.causal) kv_end = min(p.Tkv, p.past + min(q0 + kBM, p.Tq));
         n_tiles = (kv_end + kBN - 1) / kBN;
+        if constexpr (PREFIX)      // p.causal = 0: prefix tiles, then the own keys from the first query's segment start
+            n_tiles = pp.n_pre + (min(q0 + kBM, p.Tq) - q0 / pp.seg_len * pp.seg_len + kBN - 1) / kBN;
     };
 
     if (threadIdx.x == 0) {
@@ -102,16 +117,32 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
                 for (int j = 0; j < n_tiles; ++j, ++g) {
                     const int s = g & 1;
                     const uint32_t ph = (g >> 1) & 1;
-                    bar_wait(k_empty + s, ph ^ 1);
-                    bar_expect_tx(k_full + s, KV_BYTES);
+                    if constexpr (PREFIX) {
+                        const bool own = j >= pp.n_pre;
+                        const CUtensorMap *mk = own ? &map_k : &map_kp, *mv = own ? &map_v : &map_vp;
+                        const int row = own ? q0 / pp.seg_len * pp.seg_len + (j - pp.n_pre) * kBN : j * kBN;
+                        bar_wait(k_empty + s, ph ^ 1);
+                        bar_expect_tx(k_full + s, KV_BYTES);
 #pragma unroll
-                    for (int bx = 0; bx < NBOX; ++bx)
-                        tma_load_4d(sK + s * KV_BYTES + bx * KBOX_BYTES, &map_k, k_full + s, bx * 64, h, j * kBN, b);
-                    bar_wait(v_empty + s, ph ^ 1);
-                    bar_expect_tx(v_full + s, KV_BYTES);
+                        for (int bx = 0; bx < NBOX; ++bx)
+                            tma_load_4d(sK + s * KV_BYTES + bx * KBOX_BYTES, mk, k_full + s, bx * 64, h, row, b);
+                        bar_wait(v_empty + s, ph ^ 1);
+                        bar_expect_tx(v_full + s, KV_BYTES);
 #pragma unroll
-                    for (int bx = 0; bx < NBOX; ++bx)
-                        tma_load_4d(sV + s * KV_BYTES + bx * KBOX_BYTES, &map_v, v_full + s, bx * 64, h, j * kBN, b);
+                        for (int bx = 0; bx < NBOX; ++bx)
+                            tma_load_4d(sV + s * KV_BYTES + bx * KBOX_BYTES, mv, v_full + s, bx * 64, h, row, b);
+                    } else {
+                        bar_wait(k_empty + s, ph ^ 1);
+                        bar_expect_tx(k_full + s, KV_BYTES);
+#pragma unroll
+                        for (int bx = 0; bx < NBOX; ++bx)
+                            tma_load_4d(sK + s * KV_BYTES + bx * KBOX_BYTES, &map_k, k_full + s, bx * 64, h, j * kBN, b);
+                        bar_wait(v_empty + s, ph ^ 1);
+                        bar_expect_tx(v_full + s, KV_BYTES);
+#pragma unroll
+                        for (int bx = 0; bx < NBOX; ++bx)
+                            tma_load_4d(sV + s * KV_BYTES + bx * KBOX_BYTES, &map_v, v_full + s, bx * 64, h, j * kBN, b);
+                    }
                 }
                 w = w_next;
             }
@@ -134,6 +165,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         int h, b, q0, n_tiles;
         decode(w, h, b, q0, n_tiles);
         const int r0 = q0 + row_in_tile;             // rows r0 and r0 + 8
+        int own0 = 0, seg0[2] = {0, 0};              // PREFIX: first own key of the item, segment start of each row
+        if constexpr (PREFIX) {
+            own0 = q0 / pp.seg_len * pp.seg_len;
+            seg0[0] = r0 / pp.seg_len * pp.seg_len;
+            seg0[1] = (r0 + 8) / pp.seg_len * pp.seg_len;
+        }
         float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l: this thread's columns only
         float o[HD / 2];
 #pragma unroll
@@ -157,23 +194,43 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
             bar_arrive(k_empty + s);
             if (j + 1 == n_tiles) bar_arrive(q_empty);
 
-            // masks: key padding, ragged tail, causality (key index <= past + query index)
-            const bool need_mask = (k0 + kBN > p.Tkv) || (p.key_mask != nullptr) ||
-                                   (p.causal && k0 + kBN - 1 > p.past + q0 + wg * 64);
-            if (need_mask) {
+            if constexpr (PREFIX) {
+                // prefix tile: the prefix mask and its tail; own tile: the query's segment, up to the query, key_mask
+                const bool own = j >= pp.n_pre;
+                const int kb = own ? own0 + (j - pp.n_pre) * kBN : k0;
 #pragma unroll
                 for (int jj = 0; jj < kBN / 8; ++jj)
 #pragma unroll
                     for (int c = 0; c < 2; ++c) {
-                        const int key = k0 + jj * 8 + 2 * tq + c;
-                        bool vis = key < p.Tkv;
-                        if (vis && p.key_mask != nullptr) vis = p.key_mask[(long)b * p.Tkv + key] != 0;
+                        const int key = kb + jj * 8 + 2 * tq + c;
+                        bool vis;
+                        if (own) vis = key < p.Tkv && (p.key_mask == nullptr || p.key_mask[(long)b * p.Tkv + key] != 0);
+                        else vis = key < pp.Tp && (pp.prefix_mask == nullptr || pp.prefix_mask[(long)b * pp.Tp + key] != 0);
 #pragma unroll
                         for (int i = 0; i < 2; ++i) {
-                            const bool ok = vis && (!p.causal || key <= p.past + r0 + 8 * i);
+                            const bool ok = vis && (!own || (key >= seg0[i] && key <= r0 + 8 * i));
                             if (!ok) sc[jj * 4 + 2 * i + c] = -INFINITY;
                         }
                     }
+            } else {
+                // masks: key padding, ragged tail, causality (key index <= past + query index)
+                const bool need_mask = (k0 + kBN > p.Tkv) || (p.key_mask != nullptr) ||
+                                       (p.causal && k0 + kBN - 1 > p.past + q0 + wg * 64);
+                if (need_mask) {
+#pragma unroll
+                    for (int jj = 0; jj < kBN / 8; ++jj)
+#pragma unroll
+                        for (int c = 0; c < 2; ++c) {
+                            const int key = k0 + jj * 8 + 2 * tq + c;
+                            bool vis = key < p.Tkv;
+                            if (vis && p.key_mask != nullptr) vis = p.key_mask[(long)b * p.Tkv + key] != 0;
+#pragma unroll
+                            for (int i = 0; i < 2; ++i) {
+                                const bool ok = vis && (!p.causal || key <= p.past + r0 + 8 * i);
+                                if (!ok) sc[jj * 4 + 2 * i + c] = -INFINITY;
+                            }
+                        }
+                }
             }
             float alpha[2], neg_m[2];
 #pragma unroll
@@ -293,14 +350,16 @@ static int make_map_uncached(CUtensorMap *map, const void *ptr, int dtype, int B
     return MMFS_OK;
 }
 
-template <typename T, int HD, bool LSE>
+// PREFIX: mkp / mvp are the prefix maps and pp its parameters; the other instantiations pass mk / mv in their place
+template <typename T, int HD, bool LSE, bool PREFIX = false>
 static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const AttnParams &p,
-                       unsigned *work_counter, float *lse, cudaStream_t st) {
+                       unsigned *work_counter, float *lse, cudaStream_t st, const CUtensorMap *mkp = nullptr,
+                       const CUtensorMap *mvp = nullptr, const PrefixParams &pp = {}) {
     const int n_q = (p.Tq + kBM - 1) / kBM;
     const long n_work = (long)n_q * p.H * p.B;
     if (n_work >= (1L << 30)) { set_error("attn_forward: %ld work items", n_work); return MMFS_EUNSUPPORTED; }
     constexpr size_t smem = (size_t)(HD / 64) * (kBM * 128 + 4 * kBN * 128) + 14 * 8 + 2 * sizeof(int);
-    constexpr auto kern = attn_fwd_kernel<T, HD, LSE>;
+    constexpr auto kern = attn_fwd_kernel<T, HD, LSE, PREFIX>;
     const int rc = ensure_dynamic_smem<kern>(smem);
     if (rc != MMFS_OK) return rc;
     // more items than resident CTAs: persistent over the items the zeroed counter hands out, otherwise one item per CTA
@@ -308,7 +367,8 @@ static int launch_attn(const CUtensorMap &mq, const CUtensorMap &mk, const CUten
     const bool persistent = n_work > resident;
     if (persistent) MMFS_CUDA(cudaMemsetAsync(work_counter, 0, sizeof(unsigned), st));
     const int grid = persistent ? resident : (int)n_work;
-    kern<<<grid, kAttnThreads, smem, st>>>(mq, mk, mv, p, persistent ? work_counter : nullptr, (int)n_work, lse);
+    kern<<<grid, kAttnThreads, smem, st>>>(mq, mk, mv, p, persistent ? work_counter : nullptr, (int)n_work, lse,
+                                           PREFIX ? *mkp : mk, PREFIX ? *mvp : mv, pp);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -368,4 +428,60 @@ extern "C" int mmfs_attn_forward_lse(const void *q, const void *k, const void *v
     MMFS_CHECK_ARG(lse != nullptr, "attn_forward_lse: null pointer argument (lse)");
     return attn_forward(q, k, v, out, lse, key_mask, B, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts, o_bs, o_ts,
                         scale, causal, past, dtype, work_counter, stream);
+}
+
+namespace mmfs {
+// the generic-kernel branch of mmfs_attn_prefix_shared (attn_generic_sm100.cu)
+int attn_prefix_generic(const void *q, const void *k, const void *v, const void *k_prefix, const void *v_prefix, void *out,
+                        const uint8_t *prefix_mask, const uint8_t *key_mask, int B, int H, int Tq, int Tp, int seg_len,
+                        int hd, long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long kp_bs, long kp_ts,
+                        long vp_bs, long vp_ts, long o_bs, long o_ts, float scale, int dtype, cudaStream_t st);
+}  // namespace mmfs
+
+extern "C" int mmfs_attn_prefix_shared(const void *q, const void *k, const void *v, const void *k_prefix,
+                                       const void *v_prefix, void *out, const uint8_t *prefix_mask, const uint8_t *key_mask,
+                                       int P, int H, int Tq, int Tp, int seg_len, int hd, long q_bs, long q_ts, long k_bs,
+                                       long k_ts, long v_bs, long v_ts, long kp_bs, long kp_ts, long vp_bs, long vp_ts,
+                                       long o_bs, long o_ts, float scale, int dtype, unsigned *work_counter, void *stream) {
+    MMFS_CHECK_ARG(P >= 0 && H > 0 && Tq >= 0 && Tp > 0 && hd > 0 && hd <= 256, "attn_prefix_shared: bad shape (hd <= 256)");
+    MMFS_CHECK_ARG(seg_len >= 1, "attn_prefix_shared: seg_len = %d must be >= 1", seg_len);
+    MMFS_CHECK_ARG(Tq % seg_len == 0, "attn_prefix_shared: Tq = %d is not whole segments of seg_len = %d", Tq, seg_len);
+    if (P == 0 || Tq == 0) return MMFS_OK;
+    MMFS_CHECK_ARG(q && k && v && k_prefix && v_prefix && out && work_counter, "attn_prefix_shared: null pointer argument");
+    MMFS_CHECK_ARG((uintptr_t)work_counter % 4 == 0, "attn_prefix_shared: work_counter must be 4-byte aligned");
+    const size_t es = dtype_size(dtype);
+    if (dtype == MMFS_F64 || es == 0) {
+        set_error("attn_prefix_shared: needs f32/f16/bf16 (got dtype=%d)", dtype);
+        return MMFS_EUNSUPPORTED;
+    }
+    const uintptr_t ptrs = (uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)k_prefix | (uintptr_t)v_prefix | (uintptr_t)out;
+    if (ptrs % es != 0) {
+        set_error("attn_prefix_shared: pointers must be aligned to their element size");
+        return MMFS_EUNSUPPORTED;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    // the routing of ops.attention: the wgmma kernel for 16-bit hd 64 / 128 with at least 16 queries (attn_tc.supported)
+    // and 16-byte aligned rows, the generic kernel otherwise
+    const bool tc = (dtype == MMFS_BF16 || dtype == MMFS_F16) && (hd == 64 || hd == 128) && Tq >= 16 && ptrs % 16 == 0 &&
+                    (q_bs | q_ts | k_bs | k_ts | v_bs | v_ts | kp_bs | kp_ts | vp_bs | vp_ts | o_bs | o_ts) % 8 == 0 &&
+                    P <= 65535 && H <= 65535;
+    if (!tc)
+        return attn_prefix_generic(q, k, v, k_prefix, v_prefix, out, prefix_mask, key_mask, P, H, Tq, Tp, seg_len, hd, q_bs,
+                                   q_ts, k_bs, k_ts, v_bs, v_ts, kp_bs, kp_ts, vp_bs, vp_ts, o_bs, o_ts, scale, dtype, st);
+    CUtensorMap mq, mk, mv, mkp, mvp;
+    int rc;
+    if ((rc = make_map(&mq, q, dtype, P, Tq, H, hd, q_bs, q_ts, kBM)) != MMFS_OK) return rc;
+    if ((rc = make_map(&mk, k, dtype, P, Tq, H, hd, k_bs, k_ts, kBN)) != MMFS_OK) return rc;
+    if ((rc = make_map(&mv, v, dtype, P, Tq, H, hd, v_bs, v_ts, kBN)) != MMFS_OK) return rc;
+    if ((rc = make_map(&mkp, k_prefix, dtype, P, Tp, H, hd, kp_bs, kp_ts, kBN)) != MMFS_OK) return rc;
+    if ((rc = make_map(&mvp, v_prefix, dtype, P, Tp, H, hd, vp_bs, vp_ts, kBN)) != MMFS_OK) return rc;
+    AttnParams p;
+    p.out = out; p.key_mask = key_mask; p.B = P; p.H = H; p.Tq = Tq; p.Tkv = Tq; p.causal = 0; p.past = 0;
+    p.o_bs = o_bs; p.o_ts = o_ts; p.scale_log2e = scale * 1.4426950408889634f;
+    const PrefixParams pp{prefix_mask, Tp, seg_len, (Tp + kBN - 1) / kBN};
+    return dispatch_dtype<kF16Types>(dtype, "attn_prefix_shared", [&](auto tag) {
+        using T = typename decltype(tag)::type;
+        return hd == 64 ? launch_attn<T, 64, false, true>(mq, mk, mv, p, work_counter, nullptr, st, &mkp, &mvp, pp)
+                        : launch_attn<T, 128, false, true>(mq, mk, mv, p, work_counter, nullptr, st, &mkp, &mvp, pp);
+    });
 }

@@ -22,12 +22,23 @@ namespace mmfs {
 constexpr int kAttnChunk = 256;   // keys per chunk (8 per lane)
 constexpr int kAttnWarps = 4;
 
+// Prefix-shared segments (mmfs_attn_prefix_shared): k / v are the rows' own keys (Tkv = Tq), and row i walks the
+// virtual key range j = 0 .. Tp + i - s, s = i / seg_len * seg_len: prefix key j below Tp (under `mask`), then own key
+// s + j - Tp (under key_mask).  The other instantiations do not read `ps`, which comes last for that reason.
 template <typename T>
-__global__ void __launch_bounds__(32 * kAttnWarps)
+struct PrefixSeg {
+    const T *k, *v;                                   // (B, Tp, H, hd)
+    long k_bs, k_ts, v_bs, v_ts;
+    const uint8_t *mask;                              // (B, Tp) or null
+    int Tp, seg_len;
+};
+
+template <typename T, bool PREFIX = false>
+__global__ void __launch_bounds__(32 * kAttnWarps, PREFIX ? 8 : 0)   // PREFIX: 64 registers, no spills
 attn_generic_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *__restrict__ v, T *__restrict__ out,
                     const uint8_t *__restrict__ key_mask, long n_rows, int H, int Tq, int Tkv, int hd,
                     long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs, long o_ts,
-                    float scale, int causal, int past) {
+                    float scale, int causal, int past, PrefixSeg<T> ps) {
     extern __shared__ float s_dyn_f[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float *s_q = s_dyn_f + warp * (hd + kAttnChunk);
@@ -35,14 +46,20 @@ attn_generic_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *_
     const int cpl = (hd + 31) / 32;   // channels per lane (<= 8)
 
     for (long row = (long)blockIdx.x * kAttnWarps + warp; row < n_rows; row += (long)gridDim.x * kAttnWarps) {
-        const int i = (int)(row % Tq);
-        const int h = (int)((row / Tq) % H);
-        const int b = (int)(row / Tq / H);
+        // PREFIX: 32-bit row arithmetic (the host keeps n_rows below 2^31), which spares the 64-bit division call
+        const int i = PREFIX ? (int)row % Tq : (int)(row % Tq);
+        const int h = PREFIX ? (int)row / Tq % H : (int)((row / Tq) % H);
+        const int b = PREFIX ? (int)row / Tq / H : (int)(row / Tq / H);
         const T *qp = q + b * q_bs + i * q_ts + (long)h * hd;
         __syncwarp();
         for (int d = lane; d < hd; d += 32) s_q[d] = to_op(qp[d]) * scale;
         __syncwarp();
-        const int last_key = causal ? min(Tkv - 1, past + i) : Tkv - 1;
+        int last_key = causal ? min(Tkv - 1, past + i) : Tkv - 1;
+        int own0 = 0;                                 // PREFIX: own key of virtual key Tp
+        if constexpr (PREFIX) {
+            own0 = i / ps.seg_len * ps.seg_len - ps.Tp;
+            last_key = i - own0;
+        }
         float m_run = -INFINITY, l_run = 0.f;
         float acc[8];
 #pragma unroll
@@ -54,7 +71,16 @@ attn_generic_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *_
             for (int t = 0; t < kAttnChunk / 32; ++t) {
                 const int j = j0 + lane + 32 * t;
                 float s = -INFINITY;
-                if (j <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + j])) {
+                if constexpr (PREFIX) {
+                    const bool pre = j < ps.Tp;
+                    if (j <= last_key && (pre ? (ps.mask == nullptr || ps.mask[(long)b * ps.Tp + j])
+                                              : (key_mask == nullptr || key_mask[(long)b * Tkv + own0 + j]))) {
+                        const T *kp = (pre ? ps.k + b * ps.k_bs + j * ps.k_ts : k + b * k_bs + (own0 + j) * k_ts) + (long)h * hd;
+                        float dot = 0.f;
+                        for (int d = 0; d < hd; ++d) dot += s_q[d] * to_op(kp[d]);
+                        s = dot;
+                    }
+                } else if (j <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + j])) {
                     const T *kp = k + b * k_bs + j * k_ts + (long)h * hd;
                     float dot = 0.f;
                     for (int d = 0; d < hd; ++d) dot += s_q[d] * to_op(kp[d]);
@@ -87,6 +113,9 @@ attn_generic_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *_
                 const float p = s_p[jj];
                 if (p == 0.f) continue;                                // warp-uniform (same smem word)
                 const T *vp = v + b * v_bs + (long)(j0 + jj) * v_ts + (long)h * hd;
+                if constexpr (PREFIX)
+                    vp = j0 + jj < ps.Tp ? ps.v + b * ps.v_bs + (long)(j0 + jj) * ps.v_ts + (long)h * hd
+                                         : v + b * v_bs + (long)(own0 + j0 + jj) * v_ts + (long)h * hd;
 #pragma unroll
                 for (int c = 0; c < 8; ++c)
                     if (c < cpl && lane + 32 * c < hd) acc[c] += p * to_op(vp[lane + 32 * c]);
@@ -521,9 +550,29 @@ static int launch_attn_generic(const void *q, const void *k, const void *v, void
     const size_t smem = (size_t)kAttnWarps * (hd + kAttnChunk) * sizeof(float);
     attn_generic_kernel<T><<<grid, 32 * kAttnWarps, smem, st>>>((const T *)q, (const T *)k, (const T *)v, (T *)out, key_mask,
                                                               n_rows, H, Tq, Tkv, hd, q_bs, q_ts, k_bs, k_ts, v_bs, v_ts,
-                                                              o_bs, o_ts, scale, causal, past);
+                                                              o_bs, o_ts, scale, causal, past, PrefixSeg<T>{});
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
+}
+
+// mmfs_attn_prefix_shared's fallback (arguments checked there): the generic kernel's PREFIX instantiation
+int attn_prefix_generic(const void *q, const void *k, const void *v, const void *k_prefix, const void *v_prefix, void *out,
+                        const uint8_t *prefix_mask, const uint8_t *key_mask, int B, int H, int Tq, int Tp, int seg_len,
+                        int hd, long q_bs, long q_ts, long k_bs, long k_ts, long v_bs, long v_ts, long kp_bs, long kp_ts,
+                        long vp_bs, long vp_ts, long o_bs, long o_ts, float scale, int dtype, cudaStream_t st) {
+    const long n_rows = (long)B * H * Tq;
+    if (n_rows >= (1L << 31)) { set_error("attn_prefix_shared: %ld query rows", n_rows); return MMFS_EUNSUPPORTED; }
+    return dispatch_dtype<kF32Types>(dtype, "attn_prefix_shared", [&](auto tag) {
+        using T = typename decltype(tag)::type;
+        const int grid = capped_grid((n_rows + kAttnWarps - 1) / kAttnWarps, 16);
+        const size_t smem = (size_t)kAttnWarps * (hd + kAttnChunk) * sizeof(float);
+        const PrefixSeg<T> ps{(const T *)k_prefix, (const T *)v_prefix, kp_bs, kp_ts, vp_bs, vp_ts, prefix_mask, Tp, seg_len};
+        attn_generic_kernel<T, true><<<grid, 32 * kAttnWarps, smem, st>>>(
+            (const T *)q, (const T *)k, (const T *)v, (T *)out, key_mask, n_rows, H, Tq, Tq, hd, q_bs, q_ts, k_bs, k_ts, v_bs,
+            v_ts, o_bs, o_ts, scale, 0, 0, ps);
+        MMFS_CUDA(cudaGetLastError());
+        return MMFS_OK;
+    });
 }
 
 }  // namespace mmfs

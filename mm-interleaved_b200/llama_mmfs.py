@@ -256,6 +256,20 @@ class SharedPrefixKV:
         return self.k.shape[1] + self.k_gen.shape[1] - 1
 
 
+class PrefixKV:
+    """Read-only cache of one layer for scoring many short segments against one stored context
+    (``MMInterleaved.enable_shared_context_scores``): ``k``, ``v`` (P, T_p, H, hd) are views of an existing cache's first
+    T_p positions (e.g. ``StaticKV.k[:, :T_p]``), ``prefix_mask`` (P, T_p) marks the visible ones (or None), and the
+    forward's T = G · ``seg_len`` positions per row are G segments.  A layer given it rotates its q and k at the explicit
+    ``position_ids``, attends through ``ops.attention_prefix_shared`` (every visible prefix key, and causally the keys of
+    the query's own segment) and appends nothing, so one prefill serves every segment; ``use_cache`` must be False."""
+
+    __slots__ = ("k", "v", "prefix_mask", "seg_len")
+
+    def __init__(self, k, v, prefix_mask, seg_len):
+        self.k, self.v, self.prefix_mask, self.seg_len = k, v, prefix_mask, int(seg_len)
+
+
 class PreparedVision:
     """Image-side state of the MMFS cross-attention layers for ONE batch of images: per layer, ``value`` =
     value_proj(RMSNorm(vision)) (modeling_llama_mmfs.py:353, mmfs.py:165-172) -- everything those layers derive from
@@ -309,6 +323,9 @@ class LlamaAttention(nn.Module):
             return self._forward_training(hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual)
         qkv = decode_linear(hidden_states, self._qkv.get(), self._fp8, "qkv").view(B, T, 3, H, hd)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+        if isinstance(past_key_value, PrefixKV):
+            return self._forward_prefix(q, k, v, position_ids, past_key_value, attention_mask, use_cache, residual,
+                                        inplace)
         shared = isinstance(past_key_value, SharedPrefixKV)
         static = shared or isinstance(past_key_value, StaticKV)
         past = 0 if past_key_value is None else (past_key_value.length if static else past_key_value[0].shape[1])
@@ -358,6 +375,19 @@ class LlamaAttention(nn.Module):
             ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)   # (B, T, H*hd)
         out = decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace)
         return out, None, present
+
+    def _forward_prefix(self, q, k, v, position_ids, c, attention_mask, use_cache, residual, inplace):
+        """The layer over a ``PrefixKV``: RoPE on q and k at the explicit per-token ``position_ids`` (B, T), the
+        prefix-shared attention with ``attention_mask`` (B, T) as the segments' own-key mask, o_proj; nothing is cached."""
+        if use_cache:
+            raise RuntimeError("PrefixKV is read-only: run the segments with use_cache=False")
+        B, T = q.shape[:2]
+        if position_ids is None or position_ids.numel() != B * T:
+            raise RuntimeError("PrefixKV needs explicit position_ids of shape (B, T): the segments continue the prefix")
+        cos, sin = self.rope_tables(q.device, c.k.shape[1] + c.seg_len)   # positions < T_p + seg_len (LlamaModel checks)
+        ops.rope_qk_(q, k, cos, sin, position_ids)
+        ctx = ops.attention_prefix_shared(q, c.k, c.v, k, v, c.seg_len, prefix_mask=c.prefix_mask, key_mask=attention_mask)
+        return decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace), None, None
 
     def _forward_fp8(self, q, k, v, cos, sin, position_ids, c, past, attention_mask, residual, inplace):
         """The layer over an FP8 cache (``StaticKV`` / ``SharedPrefixKV`` with scales).  ``ops.rope_qk_append_fp8_``
@@ -608,7 +638,14 @@ class LlamaModel(nn.Module):
         if inputs_embeds is None:
             inputs_embeds = self.embed_tokens(input_ids)
         B, T, _ = inputs_embeds.shape
-        if past_key_values is None:
+        prefix = past_key_values is not None and isinstance(past_key_values[0], PrefixKV)
+        if prefix:                     # segments over a read-only prefix: explicit positions, (B, T) own-key mask
+            if use_cache:
+                raise RuntimeError("PrefixKV is read-only: pass use_cache=False")
+            if position_ids is None or position_ids.numel() != B * T:
+                raise ValueError(f"past_key_values of PrefixKV need explicit position_ids of shape {(B, T)}")
+            past = 0
+        elif past_key_values is None:
             past = 0
         else:
             past = (past_key_values[0].length if isinstance(past_key_values[0], (StaticKV, SharedPrefixKV))
@@ -617,6 +654,11 @@ class LlamaModel(nn.Module):
             position_ids = torch.arange(past, past + T, dtype=torch.long, device=inputs_embeds.device)
         else:
             position_ids = position_ids.view(-1, T).long()
+            if prefix:
+                position_ids = position_ids.expand(B, T)
+                limit = past_key_values[0].k.shape[1] + past_key_values[0].seg_len
+                if int(position_ids.min()) < 0 or int(position_ids.max()) >= limit:
+                    raise ValueError(f"PrefixKV segments sit at positions in [0, T_p + seg_len) = [0, {limit})")
         key_mask = None
         if attention_mask is not None:
             if tuple(attention_mask.shape) != (B, past + T):

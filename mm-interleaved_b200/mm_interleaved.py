@@ -9,6 +9,7 @@ of tensor ops whose shapes are known from the (static) maximum image count.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import List, Optional, Sequence
 
 import torch
@@ -17,7 +18,8 @@ from torch import nn
 
 from . import generation
 from ._cache import WeightCache
-from .llama_mmfs import LlamaAttention, LlamaMLP, LlamaMMFSConfig, LlamaModel, decode_linear
+from .llama_mmfs import (LlamaAttention, LlamaMLP, LlamaMMFSConfig, LlamaModel, PrefixKV, PreparedVision,
+                         decode_linear)
 from .msda import records
 
 # special-token convention of the reference (mm_interleaved.py:33-39; custom_datasets/wds_utils.py:186-215 appends
@@ -625,6 +627,7 @@ class MMInterleaved(InterleavedForward):
         self.dataset_to_ignore_noimage_cond_loss = list(dataset_to_ignore_noimage_cond_loss)
         self.mm_decoder.gradient_checkpointing = use_llama_gradient_checkpointing      # used under autograd only
         self._tok_graph = None
+        self._shared_context_scores = False                                           # enable_shared_context_scores()
 
     # ---------------------------------------------------------------------------------------------------------
     def enable_cuda_graphs(self, tokenizer: bool = True) -> "MMInterleaved":
@@ -815,12 +818,26 @@ class MMInterleaved(InterleavedForward):
                                        self._max_num_image(num_image_per_seq, kwargs.pop("max_num_image", None)),
                                        attention_mask=attention_mask, target_image_idxs=target_image_idxs, **kwargs)
 
+    def enable_shared_context_scores(self, enabled: bool = True) -> "MMInterleaved":
+        """``generate_scores`` on one prefill per context: every sample's context is prefilled once (all samples in one
+        right-padded batch, into a 16-bit cache), and each sample's options then run as one pass of G segments over that
+        cache (``llama_mmfs.PrefixKV``, ``ops.attention_prefix_shared``) instead of prefilling context + option once per
+        option.  Same inputs, positions, masks and output; the scores differ from the default path only by the order of
+        floating-point sums.  Off by default.  Options holding the bos, soi or image-token id raise ``ValueError`` (they
+        would change the image splice and visibility rules that the shared context fixes)."""
+        self._shared_context_scores = bool(enabled)
+        return self
+
     @torch.no_grad()
     def generate_scores(self, text_ids, image_tensors=None, num_image_per_seq=None, attention_mask=None, options_ids=None,
                         options_attn_masks=None, **kwargs):
         """mm_interleaved.py:666-743: for sample i, the log-likelihood of every answer option appended to its context,
         summed over the option's unmasked tokens; mini-batches of 4 options.  The image of a sample is tokenised ONCE and
-        its outputs are expanded over the options (the reference re-encodes the same image per option row)."""
+        its outputs are expanded over the options (the reference re-encodes the same image per option row).  Under
+        ``enable_shared_context_scores()`` the context is prefilled once per sample instead (``_shared_context_scores``)."""
+        if self._shared_context_scores:
+            return self._shared_context_scores_of(text_ids, image_tensors, num_image_per_seq, attention_mask, options_ids,
+                                                  options_attn_masks)
         import math
         scores = []
         for i in range(len(text_ids)):
@@ -848,6 +865,80 @@ class MMInterleaved(InterleavedForward):
             logp = F.log_softmax(logits.float(), dim=-1).gather(-1, options_ids[i][..., None]).squeeze(-1)
             scores.append((logp * options_attn_masks[i]).sum(dim=-1))
         return {"scores": torch.stack(scores, dim=0)[:, None, :]}
+
+    def _shared_context_scores_of(self, text_ids, image_tensors, num_image_per_seq, attention_mask, options_ids,
+                                  options_attn_masks):
+        """``generate_scores`` with one context prefill: (1) every image tokenised once; (2) all contexts prefilled in one
+        batch, right-padded, into a 16-bit static cache, keeping each sample's hidden state at its last context position;
+        (3) per sample one pass over ``options_ids[i][:, :-1]`` as G segments of L - 1 tokens (the last option token is
+        never an input to a scored logit), option token t at position ``len(text_ids[i]) + t`` (the default path's
+        position), attending to the sample's cache row under its context mask; (4) the logit of option token 0 from the
+        context's last hidden state, of token t >= 1 from option position t - 1, then the default path's arithmetic.
+        Runs the 16-bit weights whatever ``enable_fp8_decode`` says, as the default path does."""
+        st = self.special_token_dict
+        n = len(text_ids)
+        dev = text_ids[0].device
+        for i in range(n):
+            bad = torch.isin(options_ids[i], torch.tensor([st["bos_token_id"], st["soi_token_id"], st["image_token_id"]],
+                                                          device=options_ids[i].device))
+            if bool(bad.any()):
+                raise ValueError("generate_scores: an option holds the bos, soi or image-token id, which would change the "
+                                 "image splice and visibility rules of the shared context; score it with "
+                                 "enable_shared_context_scores(False)")
+        nimg = num_image_per_seq.reshape(-1).to(dev)
+        if nimg.numel() != n or image_tensors.shape[0] != n:
+            raise RuntimeError("generate_scores expects one image per sample (mm_interleaved.py:684-689)")
+        lens = [len(t) for t in text_ids]
+        C = max(lens)
+        ids = torch.full((n, C), st["pad_token_id"], dtype=torch.long, device=dev)
+        ctx_mask = torch.zeros((n, C), dtype=torch.long, device=dev)
+        for i in range(n):
+            ids[i, :lens[i]] = text_ids[i]
+            ctx_mask[i, :lens[i]] = attention_mask[i]
+        last = torch.tensor([c - 1 for c in lens], device=dev)
+        with self._sixteen_bit_weights():
+            mm_embeds, cross, feats = self.prepare(ids, self._tokenize(image_tensors), nimg, 1)
+            pv = self.mm_decoder.prepare_vision(feats)
+            cache = self.mm_decoder.static_cache(n, C, dtype=mm_embeds.dtype, device=dev, kv_fp8=False)
+            hid = self.mm_decoder(inputs_embeds=mm_embeds, attention_mask=ctx_mask, vision_hidden_states=pv,
+                                  cross_attention_mask=cross, past_key_values=cache, use_cache=True,
+                                  return_dict=True).last_hidden_state
+            h_last = hid[torch.arange(n, device=dev), last]                              # (n, C_hidden)
+            cross_last = cross[torch.arange(n, device=dev), last][:, None]                # (n, 1, n_img)
+            scores = []
+            for i in range(n):
+                opts, omask = options_ids[i].to(dev), options_attn_masks[i].to(dev)
+                G, L = opts.shape
+                h = h_last[i].view(1, 1, -1).expand(G, 1, -1)
+                if L > 1:
+                    x = opts[:, :-1].reshape(1, G * (L - 1))
+                    pos = (lens[i] + torch.arange(L - 1, device=dev)).repeat(G)[None]
+                    pre = [PrefixKV(c.k[i:i + 1], c.v[i:i + 1], ctx_mask[i:i + 1], L - 1) for c in cache]
+                    pv_i = PreparedVision((1,) + pv.raw_shape[1:])
+                    pv_i.values = {l: v[i:i + 1] for l, v in pv.values.items()}
+                    out = self.mm_decoder(inputs_embeds=self.mm_decoder.embed_tokens(x),
+                                          attention_mask=omask[:, :-1].reshape(1, -1), position_ids=pos,
+                                          past_key_values=pre, vision_hidden_states=pv_i,
+                                          cross_attention_mask=cross_last[i:i + 1], use_cache=False, return_dict=True)
+                    h = torch.cat((h, out.last_hidden_state.view(G, L - 1, -1)), dim=1)
+                logits = self.text_decoder.logits(h)                                      # (G, L, V)
+                logp = F.log_softmax(logits.float(), dim=-1).gather(-1, opts[..., None]).squeeze(-1)
+                scores.append((logp * omask).sum(dim=-1))
+        return {"scores": torch.stack(scores, dim=0)[:, None, :]}
+
+    @contextlib.contextmanager
+    def _sixteen_bit_weights(self):
+        """Drop the FP8 decode copies for the block (restored after): ``decode_linear`` would otherwise route a
+        one-position call of at most ``FP8_DECODE_MAX_ROWS`` rows -- a single-option pass -- to them."""
+        mods = [m for m in [*self.mm_decoder.modules(), self.text_decoder] if isinstance(m, (LlamaAttention, LlamaMLP, TextDecoder))]
+        saved = [m._fp8 for m in mods]
+        for m in mods:
+            m._fp8 = None
+        try:
+            yield
+        finally:
+            for m, f in zip(mods, saved):
+                m._fp8 = f
 
     @torch.no_grad()
     def generate_interleaved(self, text_ids, image_tensors, num_image_per_seq, attention_mask=None,

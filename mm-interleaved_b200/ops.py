@@ -435,6 +435,45 @@ def attention_decode_shared(q, k_prefix, v_prefix, k_gen, v_gen, prefix_len, key
     return out.view(R, 1, H * hd)
 
 
+def attention_prefix_shared(q, k_prefix, v_prefix, k, v, seg_len, prefix_mask=None, key_mask=None, scale=None):
+    """Answer options scored against one stored context (``mmfs_attn_prefix_shared``): q, k, v (P, Tq, H, hd), where
+    batch entry p holds Tq = G * ``seg_len`` queries in G segments and k / v are the segments' own (rotated) keys and
+    values; k_prefix / v_prefix (P, T_p, H, hd) the stored context.  Query i sees every prefix key j with
+    ``prefix_mask[p, j]`` (P, T_p) and the own keys j of its segment with j <= i and ``key_mask[p, j]`` (P, Tq); either
+    mask may be None (all visible).  A row that sees no key gives 0.  Returns (P, Tq, H*hd).  Routed as ``attention``:
+    the wgmma kernel for 16-bit hd 64 / 128 prefill shapes, the generic kernel otherwise."""
+    P, Tq, H, hd = q.shape
+    Tp = k_prefix.shape[1]
+    inference_only("attention_prefix_shared", q, k_prefix, v_prefix, k, v)
+    for t in (q, k, v, k_prefix, v_prefix):
+        _require(t.is_cuda and t.dim() == 4 and t.dtype == q.dtype and t.device == q.device and t.shape[0] == P
+                 and tuple(t.shape[2:]) == (H, hd) and t.stride(3) == 1 and t.stride(2) == hd,
+                 "attention_prefix_shared: q / k / v / prefix must be (P, T, H, hd) CUDA tensors of q's dtype, heads dense")
+    _require(tuple(k.shape) == (P, Tq, H, hd) and v.shape == k.shape, "attention_prefix_shared: k / v must be (P, Tq, H, hd)")
+    _require(v_prefix.shape == k_prefix.shape and Tp > 0, "attention_prefix_shared: k_prefix / v_prefix must be (P, T_p, H, hd), T_p > 0")
+    seg_len = int(seg_len)
+    _require(seg_len >= 1 and Tq % seg_len == 0, "attention_prefix_shared: Tq must be whole segments of seg_len >= 1")
+    masks = []
+    for m, n, what in ((prefix_mask, Tp, "prefix_mask"), (key_mask, Tq, "key_mask")):
+        if m is not None:
+            m = m.to(device=q.device, dtype=torch.uint8).contiguous()
+            _require(tuple(m.shape) == (P, n), f"attention_prefix_shared: {what} must be ({P}, {n})")
+        masks.append(m)
+    scale = float(scale if scale is not None else hd ** -0.5)
+    out = torch.empty((P, Tq, H, hd), dtype=q.dtype, device=q.device)
+    counter = torch.empty((1,), dtype=torch.int32, device=q.device)
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    with torch.cuda.device(q.device):
+        rc = _lib.lib().mmfs_attn_prefix_shared(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), k_prefix.data_ptr(), v_prefix.data_ptr(), out.data_ptr(),
+            ptr(masks[0]), ptr(masks[1]), P, H, Tq, Tp, seg_len, hd, q.stride(0), q.stride(1), k.stride(0), k.stride(1),
+            v.stride(0), v.stride(1), k_prefix.stride(0), k_prefix.stride(1), v_prefix.stride(0), v_prefix.stride(1),
+            out.stride(0), out.stride(1), scale, _DTYPE_CODE[q.dtype], counter.data_ptr(), _stream())
+    _lib.check(rc, "attention_prefix_shared")
+    launch_counter[0] += 1
+    return out.view(P, Tq, H * hd)
+
+
 # ---- training path: backward kernels (csrc/attn_bwd_sm100.cu, csrc/llama_ops_sm100.cu).  autograd_ops.py wraps them in
 # autograd Functions; like the forward wrappers they refuse to run where autograd would record them.
 
