@@ -14,7 +14,7 @@
 // One warp per (b, h, query row).  Keys are processed in chunks of 32*KPL: phase 1 gives every
 // lane whole keys (row-contiguous 16-byte loads, q broadcast from shared memory), phase 2 gives
 // every lane channels (coalesced V rows), online softmax across chunks.
-#include "common.cuh"
+#include "decode_common.cuh"
 #include "sampler_common.cuh"   // MixFma (mixed-precision FMA)
 
 namespace mmfs {
@@ -131,55 +131,34 @@ attn_generic_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *_
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Decode (q_len = 1 over a KV cache): split-KV ("flash decoding").  The row-per-warp kernel above gives a decode step
-// B*H = 160 warps for the whole GPU, each walking 2k keys serially with scalar loads.  Here grid = (ceil(Tkv / 256), H, B): every CTA reduces 256 keys of one (b, h) -- lane = key for the
-// scores (16-byte loads along the key row, q broadcast from shared memory), lane = channels for P V (coalesced V
-// rows) -- and writes an (m, l, acc[hd]) partial; a second kernel merges the partials.  HBM-bound: K and V are read
-// exactly once.
+// Decode (q_len = 1 over a KV cache): split-KV ("flash decoding") on the skeleton of decode_common.cuh.  The
+// row-per-warp kernel above gives a decode step B*H = 160 warps for the whole GPU, each walking 2k keys serially with
+// scalar loads.  Here every CTA reduces 256 keys of one (b, h) -- lane = key for the scores (16-byte loads along the
+// key row, q broadcast from shared memory), lane = channels for P V (coalesced V rows) -- and the last CTA of the
+// (b, h) merges the partials.  HBM-bound: K and V are read exactly once.  The SHARED instantiations
+// (mmfs_attn_decode_shared, the graphed beam search) read k / v as the (P, Tp, H, hd) prefix and `gen` as the
+// (R, max_new, H, hd) generated rows.
 // ------------------------------------------------------------------------------------------------------------
-constexpr int kDecKeys = 256;     // keys per CTA
-constexpr int kDecWarps = 4;      // 64 keys per warp, two passes of 32
-
-// Shared-prefix layout (mmfs_attn_decode_shared, the graphed beam search): the R query rows come in groups of G, one
-// group per prompt; the kernels' k / v (with k_bs, k_ts, v_bs, v_ts) are then the (P, Tp, H, hd) prefix, one row per
-// prompt, and row r's key / value at position j is prefix[r / G][j] below *prefix_len (clamped to [0, Tp]) and
-// gen[r][min(j - prefix_len, max_new - 1)] from there on.  A SHARED instantiation launches grid (n_split * G, H, P) with
-// blockIdx.x = split * G + g, so the G rows that read the same prefix tile are adjacent in launch order and share it
-// through L2.  Only the addressing differs: the arithmetic, the splits and the merge order are the replicated
-// kernels', so the output is bit-identical to mmfs_attn_decode over the replicated cache.
 template <typename T>
-struct SharedPrefix {
-    const T *k_gen, *v_gen;                           // (R, max_new, H, hd)
-    long kg_bs, kg_ts, vg_bs, vg_ts;
-    const long long *prefix_len;                      // (1,) device
-    int G, Tp, max_new;
+struct Kv16 {                                         // a (rows, T, H, hd) K / V pair
+    const T *k, *v;
+    long k_bs, k_ts, v_bs, v_ts;
 };
 
-template <typename T>
-__device__ __forceinline__ int shared_prefix_len(const SharedPrefix<T> &sp) {
-    return (int)min(max(*sp.prefix_len, 0ll), (long long)sp.Tp);
-}
-
-// position j of row b: prefix row `pre` (already offset to the prompt, head and lane) or generated row `gen`
-template <typename T>
-__device__ __forceinline__ const T *shared_kv_row(const T *pre, long pre_ts, const T *gen, long gen_ts, int j, int plen,
-                                                  int max_new) {
-    return j < plen ? pre + (long)j * pre_ts : gen + (long)min(j - plen, max_new - 1) * gen_ts;
-}
-
+// A warp's 64 keys in two passes of 32; the CTA writes its (acc[hd], m, l) partial and attn_decode_merge_kernel merges
+// them.  (Merging in the last CTA, as the other decode kernels do, costs this kernel registers and occupancy.)
 template <typename T, bool SHARED = false>
 __global__ void __launch_bounds__(32 * kDecWarps)
 attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *__restrict__ v,
                          const uint8_t *__restrict__ key_mask, float *__restrict__ part, int H, int Tkv, int hd,
-                         long q_bs, long k_bs, long k_ts, long v_bs, long v_ts, float scale, int last_key,
-                         SharedPrefix<T> sp) {
+                         long q_bs, long k_bs, long k_ts, long v_bs, long v_ts, float scale, int last_key, Kv16<T> gen,
+                         SharedLayout sl) {
     constexpr int VEC = 16 / (int)sizeof(T);
     extern __shared__ float s_dec[];                  // q[hd] | per-warp partials [kDecWarps][hd + 2]
     float *s_q = s_dec, *s_red = s_dec + hd;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int split = SHARED ? blockIdx.x / sp.G : blockIdx.x, h = blockIdx.y,
-              b = SHARED ? blockIdx.z * sp.G + blockIdx.x % sp.G : blockIdx.z, n_split = SHARED ? gridDim.x / sp.G : gridDim.x;
-    const int plen = SHARED ? shared_prefix_len(sp) : 0;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, h = blockIdx.y;
+    const DecodeCta<SHARED> cta(sl);
+    const int b = cta.b;
     const int cpl = hd / 32;                          // channels per lane in the P V phase (host: hd % 32 == 0, <= 8)
     const T *qp = q + b * q_bs + (long)h * hd;
     for (int d = threadIdx.x; d < hd; d += blockDim.x) s_q[d] = to_op(qp[d]) * scale;
@@ -189,20 +168,15 @@ attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const
     float acc[8];
 #pragma unroll
     for (int c = 0; c < 8; ++c) acc[c] = 0.f;
-    const int kbase = split * kDecKeys + warp * (kDecKeys / kDecWarps);
+    const int kbase = cta.split * kDecKeys + warp * kDecKPW;
 #pragma unroll 1
-    for (int it = 0; it < kDecKeys / kDecWarps / 32; ++it) {
+    for (int it = 0; it < kDecKPW / 32; ++it) {
         const int j0 = kbase + it * 32;
         if (j0 > last_key) break;                     // warp-uniform
         const int j = j0 + lane;
         float sc = -INFINITY;
         if (j <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + j])) {
-            const T *kp;
-            if constexpr (SHARED)
-                kp = shared_kv_row(k + blockIdx.z * k_bs + (long)h * hd, k_ts, sp.k_gen + b * sp.kg_bs + (long)h * hd, sp.kg_ts,
-                                   j, plen, sp.max_new);
-            else
-                kp = k + b * k_bs + (long)j * k_ts + (long)h * hd;
+            const T *kp = cta.at(k + (long)h * hd, k_bs, k_ts, gen.k + (long)h * hd, gen.k_bs, gen.k_ts, j);
             float dot = 0.f;
             for (int d0 = 0; d0 < hd; d0 += VEC) {
                 float f[VEC];
@@ -230,16 +204,11 @@ attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const
         m_run = m_new;
 #pragma unroll
         for (int c = 0; c < 8; ++c) acc[c] *= corr;
-        const T *vb = v + b * v_bs + (long)h * hd + lane * cpl;
         for (int jj = 0; jj < 32; ++jj) {
             const float pw = __shfl_sync(0xffffffffu, pj, jj);
             if (pw == 0.f) continue;                  // warp-uniform
-            const T *vp;
-            if constexpr (SHARED)
-                vp = shared_kv_row(v + blockIdx.z * v_bs + (long)h * hd + lane * cpl, v_ts,
-                                   sp.v_gen + b * sp.vg_bs + (long)h * hd + lane * cpl, sp.vg_ts, j0 + jj, plen, sp.max_new);
-            else
-                vp = vb + (long)(j0 + jj) * v_ts;
+            const T *vp = cta.at(v + (long)h * hd + lane * cpl, v_bs, v_ts, gen.v + (long)h * hd + lane * cpl, gen.v_bs,
+                                 gen.v_ts, j0 + jj);
             bool done = false;
             if constexpr (sizeof(T) == 2) {
                 if (cpl == 4) {                        // hd = 128, 16-bit: one 8-byte load per lane, 256 B per warp
@@ -274,7 +243,7 @@ attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const
     float m_all = -INFINITY;
 #pragma unroll
     for (int w = 0; w < kDecWarps; ++w) m_all = fmaxf(m_all, s_red[w * (hd + 2) + hd]);
-    float *dst = part + (((long)b * H + h) * n_split + split) * (hd + 2);
+    float *dst = part + (((long)b * H + h) * cta.n_split + cta.split) * (hd + 2);
     for (int d = threadIdx.x; d < hd + 2; d += blockDim.x) {
         float r = 0.f;
         if (d == hd) r = m_all;
@@ -298,9 +267,7 @@ attn_decode_split_kernel(const T *__restrict__ q, const T *__restrict__ k, const
 // branched and loaded key by key, which left two loads in flight per warp (SASS: LDG.U8 -> BRA -> 2 x LDG.128 -> SHFL per
 // key).  A masked key inside the range is still loaded (clamped address)
 // and discarded.
-// A warp reduces 64 keys in one pass (no running rescale); the CTA's four warps are combined in shared memory into one
-// (m, l, acc[128]) partial, and the LAST CTA of a (b, h) to arrive (a ticket per (b, h) in the scratch buffer, zeroed by
-// the launcher) merges the n_split partials and writes the output row -- no second kernel.
+// A warp reduces 64 keys in one pass (no running rescale).
 template <typename T>
 __device__ __forceinline__ float dot16_mixed(const uint4 &ka, const uint4 &kb, const uint4 &qa, const uint4 &qb) {
     float d0 = 0.f, d1 = 0.f;
@@ -320,19 +287,15 @@ __global__ void __launch_bounds__(32 * kDecWarps, SHARED ? 4 : 5)
 attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, const T *__restrict__ v,
                             const uint8_t *__restrict__ key_mask, float *__restrict__ part, unsigned *__restrict__ tickets,
                             T *__restrict__ out, int H, int Tkv, long q_bs, long k_bs, long k_ts, long v_bs, long v_ts,
-                            long o_bs, float scale, int last_key, SharedPrefix<T> sp) {
-    constexpr int WARPS = kDecWarps, HD = 128, KPW = kDecKeys / WARPS;
+                            long o_bs, float scale, int last_key, Kv16<T> gen, SharedLayout sl) {
+    constexpr int WARPS = kDecWarps, HD = 128, KPW = kDecKPW;
     static_assert(KPW == 64, "the pipeline below walks a warp's keys in four batches of 16");
-    static_assert(32 * WARPS >= HD, "one thread per channel in the combine / merge steps");
     __shared__ float s_p[WARPS][KPW];
     __shared__ __align__(16) float s_acc[WARPS][HD];
-    __shared__ float s_m[WARPS], s_l[WARPS];
-    __shared__ int s_is_last;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int split = SHARED ? blockIdx.x / sp.G : blockIdx.x, h = blockIdx.y,
-              b = SHARED ? blockIdx.z * sp.G + blockIdx.x % sp.G : blockIdx.z, n_split = SHARED ? gridDim.x / sp.G : gridDim.x;
-    const int plen = SHARED ? shared_prefix_len(sp) : 0;
-    const int k0 = split * kDecKeys + warp * KPW;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, h = blockIdx.y;
+    const DecodeCta<SHARED> cta(sl);
+    const int b = cta.b;
+    const int k0 = cta.split * kDecKeys + warp * KPW;
     const int half = lane >> 4, ch = (lane & 15) * 8;
     float m = -INFINITY, l = 0.f;
     float acc[8];
@@ -351,36 +314,24 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
         const int sub = lane & 7, grp = lane >> 3;
         const T *qp = q + b * q_bs + (long)h * HD + sub * 16;    // this lane's 16 channels of q, kept packed
         const uint4 qa = ldg_nc_v4(qp), qb = ldg_nc_v4(qp + 8);
-        const T *kb = k + b * k_bs + (long)h * HD + sub * 16;
         // Software pipeline over eight batches (K0..K3, V0..V3) with two register buffers: the loads of batch i+1 are
         // issued BEFORE the arithmetic of batch i, and V0 is requested before the softmax reductions (V does not depend
         // on P), so every warp keeps one 4 KB batch in flight from its first instruction to its last.  (Without this
         // a warp has nothing in flight while it computes.)
-        const T *vb = v + b * v_bs + (long)h * HD + ch;
         auto load_k = [&](uint4 (&r)[8], int bt) {
 #pragma unroll
             for (int s = 0; s < 4; ++s) {
-                const T *kp;
-                if constexpr (SHARED)
-                    kp = shared_kv_row(k + blockIdx.z * k_bs + (long)h * HD + sub * 16, k_ts,
-                                       sp.k_gen + b * sp.kg_bs + (long)h * HD + sub * 16, sp.kg_ts,
-                                       min(k0 + bt * 16 + s * 4 + grp, last_key), plen, sp.max_new);
-                else
-                    kp = kb + (long)min(k0 + bt * 16 + s * 4 + grp, last_key) * k_ts;
+                const T *kp = cta.at(k + cta.pb * k_bs + (long)h * HD + sub * 16, k_ts, gen.k + b * gen.k_bs + (long)h * HD + sub * 16,
+                                     gen.k_ts, min(k0 + bt * 16 + s * 4 + grp, last_key));
                 r[2 * s] = ldg_nc_v4(kp);
                 r[2 * s + 1] = ldg_nc_v4(kp + 8);
             }
         };
         auto load_v = [&](uint4 (&r)[8], int bt) {
 #pragma unroll
-            for (int s = 0; s < 8; ++s) {
-                if constexpr (SHARED)
-                    r[s] = ldg_nc_v4(shared_kv_row(v + blockIdx.z * v_bs + (long)h * HD + ch, v_ts,
-                                                   sp.v_gen + b * sp.vg_bs + (long)h * HD + ch, sp.vg_ts,
-                                                   min(k0 + bt * 16 + s * 2 + half, last_key), plen, sp.max_new));
-                else
-                    r[s] = ldg_nc_v4(vb + (long)min(k0 + bt * 16 + s * 2 + half, last_key) * v_ts);
-            }
+            for (int s = 0; s < 8; ++s)
+                r[s] = ldg_nc_v4(cta.at(v + cta.pb * v_bs + (long)h * HD + ch, v_ts, gen.v + b * gen.v_bs + (long)h * HD + ch,
+                                        gen.v_ts, min(k0 + bt * 16 + s * 2 + half, last_key)));
         };
         auto scores = [&](const uint4 (&r)[8], int bt) {          // 4 steps of 4 keys
             const unsigned okw = (bt < 2 ? ok_lo : ok_hi) >> ((bt & 1) * 16);
@@ -438,53 +389,8 @@ attn_decode_split128_kernel(const T *__restrict__ q, const T *__restrict__ k, co
         *reinterpret_cast<float4 *>(&s_acc[warp][ch]) = make_float4(acc[0], acc[1], acc[2], acc[3]);
         *reinterpret_cast<float4 *>(&s_acc[warp][ch + 4]) = make_float4(acc[4], acc[5], acc[6], acc[7]);
     }
-    if (lane == 0) { s_m[warp] = m; s_l[warp] = l; }
-    __syncthreads();
-    // ---- the CTA's partial: thread = channel (threads past HD only take part in the barriers) ----------------------
-    const int d = threadIdx.x;
-    const bool chan = d < HD;
-    float M = s_m[0];
-#pragma unroll
-    for (int w = 1; w < WARPS; ++w) M = fmaxf(M, s_m[w]);
-    float num = 0.f, den = 0.f;
-    if (M != -INFINITY && chan) {
-#pragma unroll
-        for (int w = 0; w < WARPS; ++w) {
-            if (s_m[w] == -INFINITY) continue;
-            const float e = __expf(s_m[w] - M);
-            num = fmaf(e, s_acc[w][d], num);
-            den = fmaf(e, s_l[w], den);
-        }
-    }
-    T *orow = out + b * o_bs + (long)h * HD;
-    if (n_split == 1) {                                           // nothing to merge with
-        if (chan) orow[d] = from_op<T>(den > 0.f ? num / den : 0.f);
-        return;
-    }
-    float *dst = part + (((long)b * H + h) * n_split + split) * (HD + 2);
-    if (chan) dst[d] = num;
-    if (d == 0) { dst[HD] = M; dst[HD + 1] = den; }
-    __threadfence();                                              // this thread's partial is visible device-wide ...
-    __syncthreads();
-    if (d == 0) s_is_last = atomicAdd(&tickets[b * H + h], 1u) == (unsigned)(n_split - 1);   // ... before the ticket
-    __syncthreads();
-    if (!s_is_last || !chan) return;
-    __threadfence();
-    // ---- last CTA of this (b, h): merge (L2 loads: the partials were written by other SMs) ---------------------
-    const float *p0 = part + ((long)b * H + h) * n_split * (HD + 2);
-    float MM = -INFINITY;
-    for (int s = 0; s < n_split; ++s) MM = fmaxf(MM, __ldcg(p0 + s * (HD + 2) + HD));
-    num = 0.f, den = 0.f;
-    if (MM != -INFINITY) {
-#pragma unroll 4
-        for (int s = 0; s < n_split; ++s) {
-            const float ms = __ldcg(p0 + s * (HD + 2) + HD);
-            const float e = ms == -INFINITY ? 0.f : __expf(ms - MM);
-            num = fmaf(e, __ldcg(p0 + s * (HD + 2) + d), num);
-            den = fmaf(e, __ldcg(p0 + s * (HD + 2) + HD + 1), den);
-        }
-    }
-    orow[d] = from_op<T>(den > 0.f ? num / den : 0.f);           // fully masked row -> zeros
+    decode_epilogue<T>(m, l, &s_acc[0][0], HD, HD, part, tickets, (long)b * H + h, out + b * o_bs + (long)h * HD,
+                       cta.split, cta.n_split);
 }
 
 // (Alternative not taken: staging a warp's whole 64-key K and V tiles in shared memory with cp.async -- 32 KB per warp
@@ -511,23 +417,20 @@ __global__ void attn_decode_merge_kernel(const float *__restrict__ part, T *__re
     }
 }
 
-static inline long decode_ticket_floats(int B, int H) { return ((long)B * H + 3) / 4 * 4; }   // keeps the partials 16-byte aligned
-
-// B query rows; SHARED: B = P * sp.G rows over the shared-prefix layout (k / v = the prefix)
+// B query rows; SHARED: B = P * sl.G rows, k / v the prefix and gen the generated rows
 template <typename T, bool SHARED = false>
 static int launch_attn_decode(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask, float *scratch,
                               int B, int H, int Tkv, int hd, long q_bs, long k_bs, long k_ts, long v_bs, long v_ts, long o_bs,
-                              float scale, int last_key, cudaStream_t st, SharedPrefix<T> sp = {}) {
-    const int n_split = (last_key + kDecKeys) / kDecKeys;           // keys 0 .. last_key
-    dim3 grid = SHARED ? dim3(n_split * sp.G, H, B / sp.G) : dim3(n_split, H, B);
+                              float scale, int last_key, cudaStream_t st, const Kv16<T> &gen = {},
+                              const SharedLayout &sl = {}) {
+    const dim3 grid = decode_grid(last_key, B, H, sl);
     if constexpr (sizeof(T) == 2) {
         if (hd == 128 && ((uintptr_t)q % 16 == 0) && (q_bs % 8 == 0) && ((uintptr_t)scratch % 16 == 0)) {
-            unsigned *tickets = reinterpret_cast<unsigned *>(scratch);          // [B * H], then the partials
-            float *part = scratch + decode_ticket_floats(B, H);
-            if (n_split > 1) MMFS_CUDA(cudaMemsetAsync(tickets, 0, sizeof(unsigned) * (size_t)B * H, st));
+            unsigned *tickets = reinterpret_cast<unsigned *>(scratch);
+            if (decode_splits(last_key) > 1) MMFS_CUDA(cudaMemsetAsync(tickets, 0, sizeof(unsigned) * (size_t)B * H, st));
             attn_decode_split128_kernel<T, SHARED><<<grid, 32 * kDecWarps, 0, st>>>(
-                (const T *)q, (const T *)k, (const T *)v, key_mask, part, tickets, (T *)out, H, Tkv, q_bs, k_bs, k_ts, v_bs, v_ts,
-                o_bs, scale, last_key, sp);
+                (const T *)q, (const T *)k, (const T *)v, key_mask, scratch + decode_ticket_floats(B, H), tickets, (T *)out, H,
+                Tkv, q_bs, k_bs, k_ts, v_bs, v_ts, o_bs, scale, last_key, gen, sl);
             MMFS_CUDA(cudaGetLastError());
             return MMFS_OK;
         }
@@ -535,8 +438,9 @@ static int launch_attn_decode(const void *q, const void *k, const void *v, void 
     const size_t smem = (size_t)(hd + kDecWarps * (hd + 2)) * sizeof(float);
     attn_decode_split_kernel<T, SHARED><<<grid, 32 * kDecWarps, smem, st>>>((const T *)q, (const T *)k, (const T *)v, key_mask,
                                                                            scratch, H, Tkv, hd, q_bs, k_bs, k_ts, v_bs, v_ts,
-                                                                           scale, last_key, sp);
-    attn_decode_merge_kernel<T><<<dim3(H, B), hd < 128 ? 64 : 128, 0, st>>>(scratch, (T *)out, H, hd, n_split, o_bs);
+                                                                           scale, last_key, gen, sl);
+    attn_decode_merge_kernel<T><<<dim3(H, B), hd < 128 ? 64 : 128, 0, st>>>(scratch, (T *)out, H, hd, decode_splits(last_key),
+                                                                            o_bs);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -594,8 +498,7 @@ extern "C" int mmfs_attn_generic(const void *q, const void *k, const void *v, vo
 }
 
 extern "C" long mmfs_attn_decode_scratch_floats(int B, int H, int Tkv, int hd) {
-    // tickets [B * H] (hd-128 16-bit path) + one partial per (b, h, split)
-    return decode_ticket_floats(B, H) + (long)B * H * ((Tkv + kDecKeys - 1) / kDecKeys) * (hd + 2);
+    return decode_ticket_floats(B, H) + (long)B * H * decode_splits(Tkv - 1) * (hd + 2);
 }
 
 extern "C" int mmfs_attn_decode(const void *q, const void *k, const void *v, void *out, const uint8_t *key_mask, float *scratch,
@@ -611,7 +514,7 @@ extern "C" int mmfs_attn_decode(const void *q, const void *k, const void *v, voi
         set_error("attn_decode: needs f32/f16/bf16, hd %% 32 == 0 (<= 256), 16-byte aligned K / V rows");
         return MMFS_EUNSUPPORTED;
     }
-    const int last_key = causal ? (past < Tkv - 1 ? past : Tkv - 1) : Tkv - 1;     // the single query row sits at position `past`
+    const int last_key = decode_last_key(causal, past, Tkv);
     MMFS_CHECK_ARG(last_key >= 0, "attn_decode: negative past");
     cudaStream_t st = (cudaStream_t)stream;
     return dispatch_dtype<kF32Types>(dtype, "attn_decode", [&](auto tag) {
@@ -640,13 +543,14 @@ extern "C" int mmfs_attn_decode_shared(const void *q, const void *k_prefix, cons
         set_error("attn_decode_shared: needs f32/f16/bf16, hd %% 32 == 0 (<= 256), 16-byte aligned prefix / gen rows, R / G <= 65535");
         return MMFS_EUNSUPPORTED;
     }
-    const int last_key = causal ? (past < Tkv - 1 ? past : Tkv - 1) : Tkv - 1;
+    const int last_key = decode_last_key(causal, past, Tkv);
     MMFS_CHECK_ARG(last_key >= 0, "attn_decode_shared: negative past");
     cudaStream_t st = (cudaStream_t)stream;
     return dispatch_dtype<kF32Types>(dtype, "attn_decode_shared", [&](auto tag) {
         using T = typename decltype(tag)::type;
-        const SharedPrefix<T> sp{(const T *)k_gen, (const T *)v_gen, kg_bs, kg_ts, vg_bs, vg_ts, prefix_len, G, Tp, max_new};
         return launch_attn_decode<T, true>(q, k_prefix, v_prefix, out, key_mask, scratch, R, H, Tkv, hd, q_bs, kp_bs, kp_ts,
-                                           vp_bs, vp_ts, o_bs, scale, last_key, st, sp);
+                                           vp_bs, vp_ts, o_bs, scale, last_key, st,
+                                           Kv16<T>{(const T *)k_gen, (const T *)v_gen, kg_bs, kg_ts, vg_bs, vg_ts},
+                                           SharedLayout{prefix_len, G, Tp, max_new});
     });
 }

@@ -7,21 +7,17 @@
 // whose keys and values happen to be those numbers.  The append kernel also writes x8 * s back over its k / v inputs
 // (the QKV GEMM's output), so a prefill's attention over its own positions sees exactly what later steps read.
 //
-// Decode attention (one query row over the cache) follows attn_decode_split128_kernel (attn_generic_sm100.cu): grid
-// (ceil(keys / 256), H, rows), four warps of 64 keys per CTA, one (m, l, acc) partial per CTA and the last CTA of a
-// (row, head) merging them in split order (a ticket per (row, head) in the scratch buffer).  Scales are folded into
+// Decode attention (one query row over the cache) is a split-KV kernel on the skeleton of decode_common.cuh, whose
+// splits, cache addressing and split merge it shares with the 16-bit decode kernels.  Scales are folded into
 // scalars: score_j = (q . k8_j) * (scale_k[j] * softmax_scale), and P V accumulates (p_j * scale_v[j]) * v8_j.  The
 // e4m3 -> f16 conversion (cvt.rn.f16x2.e4m3x2) is exact and every sum is fp32.
 #include <cuda_fp8.h>
 
-#include "common.cuh"
+#include "decode_common.cuh"
 
 namespace mmfs {
 namespace {
 
-constexpr int kFp8Keys = 256;     // keys per CTA (the split size of mmfs_attn_decode: the scratch sizes agree)
-constexpr int kFp8Warps = 4;
-constexpr int kFp8KPW = kFp8Keys / kFp8Warps;
 constexpr int kFp8MaxHd = 256;
 
 template <typename T> __device__ __forceinline__ float rnd_t(float x) { return to_op(from_op<T>(x)); }
@@ -124,43 +120,21 @@ struct Fp8KV {                    // an e4m3 (rows, T, H, hd) K / V pair and its
     long bs, ts, sbs, sts;        // strides in elements: K / V rows and positions, scale rows and positions
 };
 
-struct Fp8Gen {                   // shared-prefix layout: the rows' generated positions after *prefix_len
-    Fp8KV c;
-    const long long *prefix_len;
-    int G, Tp, max_new;
-};
-
-// position j of query row b (prompt pb): SHARED reads the prompt's prefix row below plen and row b of gen after it
-template <bool SHARED, typename P>
-__device__ __forceinline__ const P *kv_at(const P *pre, long pre_bs, long pre_ts, const P *gen, long gen_bs, long gen_ts,
-                                          int b, int pb, int j, int plen, int max_new) {
-    if constexpr (SHARED)
-        return j < plen ? pre + pb * pre_bs + (long)j * pre_ts : gen + b * gen_bs + (long)min(j - plen, max_new - 1) * gen_ts;
-    else
-        return pre + b * pre_bs + (long)j * pre_ts;
-}
-
 // HD128: a key is 128 bytes, 8 lanes x one 16-byte load, 4 keys per warp step; K and V come in batches of 32 keys
 // (eight 16-byte loads per lane, 4 KB per warp) double-buffered in registers.  Otherwise (hd % 32 == 0, <= 256): lane =
-// key for the scores (q from shared memory), lane = hd / 32 channels for P V.
+// key for the scores (q from shared memory), lane = hd / 32 channels for P V.  `g` is the SHARED layout's generated rows.
 template <typename T, bool SHARED, bool HD128>
-__global__ void __launch_bounds__(32 * kFp8Warps, 4)
-attn_decode_fp8_kernel(const T *__restrict__ q, Fp8KV c, Fp8Gen sp, const uint8_t *__restrict__ key_mask,
+__global__ void __launch_bounds__(32 * kDecWarps, 4)
+attn_decode_fp8_kernel(const T *__restrict__ q, Fp8KV c, Fp8KV g, SharedLayout sl, const uint8_t *__restrict__ key_mask,
                        float *__restrict__ part, unsigned *__restrict__ tickets, T *__restrict__ out, int H, int Tkv, int hd,
                        long q_bs, long o_bs, float scale, int last_key) {
-    __shared__ float s_p[kFp8Warps][kFp8KPW];
-    __shared__ __align__(16) float s_acc[kFp8Warps][HD128 ? 128 : kFp8MaxHd];
+    __shared__ float s_p[kDecWarps][kDecKPW];
+    __shared__ __align__(16) float s_acc[kDecWarps][HD128 ? 128 : kFp8MaxHd];
     __shared__ __align__(16) float s_q[HD128 ? 4 : kFp8MaxHd];
-    __shared__ float s_m[kFp8Warps], s_l[kFp8Warps];
-    __shared__ int s_is_last;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int split = SHARED ? blockIdx.x / sp.G : blockIdx.x, h = blockIdx.y,
-              b = SHARED ? blockIdx.z * sp.G + blockIdx.x % sp.G : blockIdx.z, n_split = SHARED ? gridDim.x / sp.G : gridDim.x;
-    const int pb = SHARED ? blockIdx.z : b;
-    const int plen = SHARED ? (int)min(max(*sp.prefix_len, 0ll), (long long)sp.Tp) : 0;
-    const int max_new = sp.max_new;
-    const int k0 = split * kFp8Keys + warp * kFp8KPW;
-    const Fp8KV &g = sp.c;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, h = blockIdx.y;
+    const DecodeCta<SHARED> cta(sl);
+    const int b = cta.b;
+    const int k0 = cta.split * kDecKeys + warp * kDecKPW;
 
     unsigned ok_lo = 0u, ok_hi = 0u;                 // validity of keys k0 + 0..31 / k0 + 32..63
     float ks_lo = 0.f, ks_hi = 0.f, vs_lo = 0.f, vs_hi = 0.f;   // their scales (lane = key); masked keys' are never used
@@ -169,10 +143,10 @@ attn_decode_fp8_kernel(const T *__restrict__ q, Fp8KV c, Fp8Gen sp, const uint8_
         ok_lo = __ballot_sync(0xffffffffu, ja <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + ja]));
         ok_hi = __ballot_sync(0xffffffffu, jb <= last_key && (key_mask == nullptr || key_mask[(long)b * Tkv + jb]));
         const int ca = min(ja, last_key), cb = min(jb, last_key);
-        ks_lo = *kv_at<SHARED>(c.ks + h, c.sbs, c.sts, g.ks + h, g.sbs, g.sts, b, pb, ca, plen, max_new);
-        ks_hi = *kv_at<SHARED>(c.ks + h, c.sbs, c.sts, g.ks + h, g.sbs, g.sts, b, pb, cb, plen, max_new);
-        vs_lo = *kv_at<SHARED>(c.vs + h, c.sbs, c.sts, g.vs + h, g.sbs, g.sts, b, pb, ca, plen, max_new);
-        vs_hi = *kv_at<SHARED>(c.vs + h, c.sbs, c.sts, g.vs + h, g.sbs, g.sts, b, pb, cb, plen, max_new);
+        ks_lo = *cta.at(c.ks + h, c.sbs, c.sts, g.ks + h, g.sbs, g.sts, ca);
+        ks_hi = *cta.at(c.ks + h, c.sbs, c.sts, g.ks + h, g.sbs, g.sts, cb);
+        vs_lo = *cta.at(c.vs + h, c.sbs, c.sts, g.vs + h, g.sbs, g.sts, ca);
+        vs_hi = *cta.at(c.vs + h, c.sbs, c.sts, g.vs + h, g.sbs, g.sts, cb);
     }
     float m = -INFINITY, l = 0.f;
     auto softmax = [&]() {                           // over the warp's 64 scores in s_p, in place
@@ -211,8 +185,8 @@ attn_decode_fp8_kernel(const T *__restrict__ q, Fp8KV c, Fp8Gen sp, const uint8_
             auto load = [&](uint4 (&r)[8], const uint8_t *pre, const uint8_t *gen, int bt) {
 #pragma unroll
                 for (int s = 0; s < 8; ++s)
-                    r[s] = ldg_nc_v4(kv_at<SHARED>(pre + (long)h * 128 + sub * 16, c.bs, c.ts, gen + (long)h * 128 + sub * 16,
-                                                   g.bs, g.ts, b, pb, min(k0 + bt * 32 + s * 4 + grp, last_key), plen, max_new));
+                    r[s] = ldg_nc_v4(cta.at(pre + (long)h * 128 + sub * 16, c.bs, c.ts, gen + (long)h * 128 + sub * 16, g.bs,
+                                            g.ts, min(k0 + bt * 32 + s * 4 + grp, last_key)));
             };
             auto scores = [&](const uint4 (&r)[8], int bt) {
                 const unsigned okw = bt ? ok_hi : ok_lo;
@@ -278,8 +252,7 @@ attn_decode_fp8_kernel(const T *__restrict__ q, Fp8KV c, Fp8Gen sp, const uint8_
 #pragma unroll 1
             for (int hf = 0; hf < 2; ++hf) {
                 const int j = min(k0 + hf * 32 + lane, last_key);
-                const uint8_t *kp = kv_at<SHARED>(c.k + (long)h * hd, c.bs, c.ts, g.k + (long)h * hd, g.bs, g.ts, b, pb, j, plen,
-                                                  max_new);
+                const uint8_t *kp = cta.at(c.k + (long)h * hd, c.bs, c.ts, g.k + (long)h * hd, g.bs, g.ts, j);
                 float dot = 0.f;
                 for (int d0 = 0; d0 < hd; d0 += 16) {
                     float f[16];
@@ -291,12 +264,12 @@ attn_decode_fp8_kernel(const T *__restrict__ q, Fp8KV c, Fp8Gen sp, const uint8_
                 s_p[warp][hf * 32 + lane] = ok ? dot * ((hf ? ks_hi : ks_lo) * scale) : -INFINITY;
             }
             softmax();
-            for (int jj = 0; jj < kFp8KPW; ++jj) {
+            for (int jj = 0; jj < kDecKPW; ++jj) {
                 const float p = s_p[warp][jj];
                 const float sv = __shfl_sync(0xffffffffu, jj < 32 ? vs_lo : vs_hi, jj & 31);
                 if (p == 0.f) continue;              // warp-uniform; a masked slot is never read into the sums
-                const uint8_t *vp = kv_at<SHARED>(c.v + (long)h * hd + lane * cpl, c.bs, c.ts, g.v + (long)h * hd + lane * cpl,
-                                                  g.bs, g.ts, b, pb, k0 + jj, plen, max_new);
+                const uint8_t *vp = cta.at(c.v + (long)h * hd + lane * cpl, c.bs, c.ts, g.v + (long)h * hd + lane * cpl, g.bs,
+                                           g.ts, k0 + jj);
                 const float pw = p * sv;
 #pragma unroll
                 for (int i = 0; i < 8; ++i)
@@ -307,80 +280,30 @@ attn_decode_fp8_kernel(const T *__restrict__ q, Fp8KV c, Fp8Gen sp, const uint8_
         for (int i = 0; i < 8; ++i)
             if (i < cpl) s_acc[warp][lane * cpl + i] = acc[i];
     }
-    if (lane == 0) { s_m[warp] = m; s_l[warp] = l; }
-    __syncthreads();
-    // ---- the CTA's partial (thread = channel) --------------------------------------------------------------------
-    float M = s_m[0];
-#pragma unroll
-    for (int w = 1; w < kFp8Warps; ++w) M = fmaxf(M, s_m[w]);
-    float den = 0.f;
-    if (M != -INFINITY) {
-#pragma unroll
-        for (int w = 0; w < kFp8Warps; ++w)
-            if (s_m[w] != -INFINITY) den = fmaf(__expf(s_m[w] - M), s_l[w], den);
-    }
-    T *orow = out + b * o_bs + (long)h * hd;
-    float *dst = part + (((long)b * H + h) * n_split + split) * (hd + 2);
-    for (int d = threadIdx.x; d < hd; d += blockDim.x) {
-        float num = 0.f;
-        if (M != -INFINITY) {
-#pragma unroll
-            for (int w = 0; w < kFp8Warps; ++w)
-                if (s_m[w] != -INFINITY) num = fmaf(__expf(s_m[w] - M), s_acc[w][d], num);
-        }
-        if (n_split == 1) orow[d] = from_op<T>(den > 0.f ? num / den : 0.f);
-        else dst[d] = num;
-    }
-    if (n_split == 1) return;
-    if (threadIdx.x == 0) { dst[hd] = M; dst[hd + 1] = den; }
-    __threadfence();                                 // this thread's partial is visible device-wide ...
-    __syncthreads();
-    if (threadIdx.x == 0) s_is_last = atomicAdd(&tickets[b * H + h], 1u) == (unsigned)(n_split - 1);   // ... before the ticket
-    __syncthreads();
-    if (!s_is_last) return;
-    __threadfence();
-    // ---- last CTA of this (row, head): merge the partials in split order ------------------------------------------
-    const float *p0 = part + ((long)b * H + h) * n_split * (hd + 2);
-    float MM = -INFINITY;
-    for (int s = 0; s < n_split; ++s) MM = fmaxf(MM, __ldcg(p0 + s * (hd + 2) + hd));
-    float dd = 0.f;
-    if (MM != -INFINITY)
-        for (int s = 0; s < n_split; ++s) {
-            const float ms = __ldcg(p0 + s * (hd + 2) + hd);
-            if (ms != -INFINITY) dd = fmaf(__expf(ms - MM), __ldcg(p0 + s * (hd + 2) + hd + 1), dd);
-        }
-    for (int d = threadIdx.x; d < hd; d += blockDim.x) {
-        float num = 0.f;
-        if (MM != -INFINITY)
-            for (int s = 0; s < n_split; ++s) {
-                const float ms = __ldcg(p0 + s * (hd + 2) + hd);
-                if (ms != -INFINITY) num = fmaf(__expf(ms - MM), __ldcg(p0 + s * (hd + 2) + d), num);
-            }
-        orow[d] = from_op<T>(dd > 0.f ? num / dd : 0.f);   // fully masked row -> zeros
-    }
+    decode_epilogue<T>(m, l, &s_acc[0][0], HD128 ? 128 : kFp8MaxHd, hd, part, tickets, (long)b * H + h,
+                       out + b * o_bs + (long)h * hd, cta.split, cta.n_split);
 }
 
-inline long ticket_floats(int B, int H) { return ((long)B * H + 3) / 4 * 4; }   // as mmfs_attn_decode_scratch_floats
-
+// B query rows; SHARED: B = P * sl.G rows, c the prefix and g the generated rows
 template <typename T, bool SHARED>
-int launch_decode_fp8(const void *q, const Fp8KV &c, const Fp8Gen &sp, void *out, const uint8_t *key_mask, float *scratch,
-                      int B, int H, int Tkv, int hd, long q_bs, long o_bs, float scale, int last_key, cudaStream_t st) {
-    const int n_split = (last_key + kFp8Keys) / kFp8Keys;
-    const dim3 grid = SHARED ? dim3(n_split * sp.G, H, B / sp.G) : dim3(n_split, H, B);
+int launch_decode_fp8(const void *q, const Fp8KV &c, const Fp8KV &g, const SharedLayout &sl, void *out,
+                      const uint8_t *key_mask, float *scratch, int B, int H, int Tkv, int hd, long q_bs, long o_bs, float scale,
+                      int last_key, cudaStream_t st) {
+    const dim3 grid = decode_grid(last_key, B, H, sl);
     unsigned *tickets = reinterpret_cast<unsigned *>(scratch);
-    float *part = scratch + ticket_floats(B, H);
-    if (n_split > 1) MMFS_CUDA(cudaMemsetAsync(tickets, 0, sizeof(unsigned) * (size_t)B * H, st));
+    float *part = scratch + decode_ticket_floats(B, H);
+    if (decode_splits(last_key) > 1) MMFS_CUDA(cudaMemsetAsync(tickets, 0, sizeof(unsigned) * (size_t)B * H, st));
     bool done = false;
     if constexpr (sizeof(T) == 2) {
         if (hd == 128) {
-            attn_decode_fp8_kernel<T, SHARED, true><<<grid, 32 * kFp8Warps, 0, st>>>(
-                (const T *)q, c, sp, key_mask, part, tickets, (T *)out, H, Tkv, hd, q_bs, o_bs, scale, last_key);
+            attn_decode_fp8_kernel<T, SHARED, true><<<grid, 32 * kDecWarps, 0, st>>>(
+                (const T *)q, c, g, sl, key_mask, part, tickets, (T *)out, H, Tkv, hd, q_bs, o_bs, scale, last_key);
             done = true;
         }
     }
     if (!done)
-        attn_decode_fp8_kernel<T, SHARED, false><<<grid, 32 * kFp8Warps, 0, st>>>(
-            (const T *)q, c, sp, key_mask, part, tickets, (T *)out, H, Tkv, hd, q_bs, o_bs, scale, last_key);
+        attn_decode_fp8_kernel<T, SHARED, false><<<grid, 32 * kDecWarps, 0, st>>>(
+            (const T *)q, c, g, sl, key_mask, part, tickets, (T *)out, H, Tkv, hd, q_bs, o_bs, scale, last_key);
     MMFS_CUDA(cudaGetLastError());
     return MMFS_OK;
 }
@@ -458,12 +381,11 @@ extern "C" int mmfs_attn_decode_fp8(const void *q, const uint8_t *k, const uint8
         set_error("attn_decode_fp8: needs hd %% 32 == 0 (<= 256), 16-byte aligned q and K / V rows, scale rows of >= H");
         return MMFS_EUNSUPPORTED;
     }
-    const int last_key = causal ? (past < Tkv - 1 ? past : Tkv - 1) : Tkv - 1;
+    const int last_key = decode_last_key(causal, past, Tkv);
     MMFS_CHECK_ARG(last_key >= 0, "attn_decode_fp8: negative past");
     return dispatch_dtype<kF32Types, MMFS_EUNSUPPORTED>(dtype, "attn_decode_fp8", [&](auto tag) {
-        return launch_decode_fp8<typename decltype(tag)::type, false>(q, c, Fp8Gen{c, nullptr, 1, 0, 1}, out, key_mask, scratch,
-                                                                      B, H, Tkv, hd, q_bs, o_bs, scale, last_key,
-                                                                      (cudaStream_t)stream);
+        return launch_decode_fp8<typename decltype(tag)::type, false>(q, c, c, SharedLayout{}, out, key_mask, scratch, B, H,
+                                                                      Tkv, hd, q_bs, o_bs, scale, last_key, (cudaStream_t)stream);
     });
 }
 
@@ -489,11 +411,11 @@ extern "C" int mmfs_attn_decode_shared_fp8(const void *q, const uint8_t *k_prefi
                   "rows of >= H, R / G <= 65535");
         return MMFS_EUNSUPPORTED;
     }
-    const int last_key = causal ? (past < Tkv - 1 ? past : Tkv - 1) : Tkv - 1;
+    const int last_key = decode_last_key(causal, past, Tkv);
     MMFS_CHECK_ARG(last_key >= 0, "attn_decode_shared_fp8: negative past");
     return dispatch_dtype<kF32Types, MMFS_EUNSUPPORTED>(dtype, "attn_decode_shared_fp8", [&](auto tag) {
-        return launch_decode_fp8<typename decltype(tag)::type, true>(q, pre, Fp8Gen{gen, prefix_len, G, Tp, max_new}, out,
-                                                                     key_mask, scratch, R, H, Tkv, hd, q_bs, o_bs, scale,
+        return launch_decode_fp8<typename decltype(tag)::type, true>(q, pre, gen, SharedLayout{prefix_len, G, Tp, max_new},
+                                                                     out, key_mask, scratch, R, H, Tkv, hd, q_bs, o_bs, scale,
                                                                      last_key, (cudaStream_t)stream);
     });
 }

@@ -285,6 +285,14 @@ class PreparedVision:
         self.values = {}                          # layer index -> (B, n_img*hw, M, D)
 
 
+def _key_mask(attention_mask):
+    """The (B, T_kv) key mask of a layer's ``attention_mask``: the mask itself, or of a reference-style additive
+    (B, 1, T, T_kv) mask, the keys visible to the last query."""
+    if attention_mask is None or attention_mask.dim() != 4:
+        return attention_mask
+    return attention_mask[:, 0, -1, :] > (torch.finfo(attention_mask.dtype).min / 2)
+
+
 class LlamaAttention(nn.Module):
     def __init__(self, config: LlamaMMFSConfig):
         super().__init__()
@@ -332,46 +340,53 @@ class LlamaAttention(nn.Module):
         if position_ids is None:
             position_ids = torch.arange(past, past + T, device=hidden_states.device)
         cos, sin = self.rope_tables(hidden_states.device, past + T)
-        if static and past_key_value.k_scale is not None:
-            return self._forward_fp8(q, k, v, cos, sin, position_ids, past_key_value, past, attention_mask, residual,
-                                     inplace)
-        if shared:                                              # graph decode over a shared prompt: append to the row's gen
-            if T != 1:
-                raise RuntimeError("SharedPrefixKV is a graph-decode cache (one token per step): prefill into its prefix "
-                                   "through StaticKV.over, and decode eagerly over a StaticKV")
-            ops.rope_qk_append_(q, k, v, cos, sin, position_ids, past_key_value.k_gen, past_key_value.v_gen,
-                                past_key_value.slot)
-            present = past_key_value
-        elif static and past_key_value.slot is not None:          # graph decode: device-side slot, whole buffer visible
-            if T != 1:
-                raise RuntimeError("StaticKV.slot (graph decode) takes one token per step")
-            ops.rope_qk_append_(q, k, v, cos, sin, position_ids, past_key_value.k, past_key_value.v, past_key_value.slot)
-            k, v = past_key_value.k, past_key_value.v
-            past = k.shape[1] - 1
-            present = past_key_value
-        elif static:
-            if past + T > past_key_value.k.shape[1]:
-                raise RuntimeError(f"StaticKV of {past_key_value.k.shape[1]} positions cannot take {past} + {T}")
-            ops.rope_qk_append_(q, k, v, cos, sin, position_ids, past_key_value.k, past_key_value.v, past)   # one kernel:
-            past_key_value.length = past + T                                   # RoPE + both cache writes
-            k, v = past_key_value.k[:, :past + T], past_key_value.v[:, :past + T]
-            present = past_key_value
+        key_mask = _key_mask(attention_mask)
+        if static:
+            # An FP8 cache (scales set): ops.rope_qk_append_fp8_ appends the rotated keys and the values as E4M3 and
+            # rewrites the k / v views with x8 * scale, so every path below sees the keys and values x8 * scale.
+            c, present = past_key_value, past_key_value
+            fp8 = c.k_scale is not None
+            if shared or c.slot is not None:                    # graph decode: device-side slot, whole buffer visible
+                if T != 1:
+                    raise RuntimeError("a graph-decode cache (SharedPrefixKV, StaticKV.slot) takes one token per step: "
+                                       "prefill into a SharedPrefixKV's prefix through StaticKV.over")
+                slot, n = c.slot, c.k.shape[1]
+                if not shared:
+                    past = n - 1
+            else:
+                if past + T > c.k.shape[1]:
+                    raise RuntimeError(f"StaticKV of {c.k.shape[1]} positions cannot take {past} + {T}")
+                slot, n = past, past + T
+                c.length = n
+            kc, vc, ksc, vsc = (c.k_gen, c.v_gen, c.ks_gen, c.vs_gen) if shared else (c.k, c.v, c.k_scale, c.v_scale)
+            if fp8:
+                ops.rope_qk_append_fp8_(q, k, v, cos, sin, position_ids, kc, vc, ksc, vsc, slot)
+            else:
+                ops.rope_qk_append_(q, k, v, cos, sin, position_ids, kc, vc, slot)    # one kernel: RoPE + both cache writes
+            if shared and fp8:
+                ctx = ops.attention_decode_shared_fp8(q, c.k, c.v, c.k_scale, c.v_scale, c.k_gen, c.v_gen, c.ks_gen,
+                                                      c.vs_gen, c.prefix_len, key_mask=key_mask, past=past)
+            elif shared:
+                ctx = ops.attention_decode_shared(q, c.k, c.v, c.k_gen, c.v_gen, c.prefix_len, key_mask=key_mask,
+                                                  past=past)
+            elif fp8 and T == 1:
+                ctx = ops.attention_decode_fp8(q, c.k[:, :n], c.v[:, :n], c.k_scale[:, :n], c.v_scale[:, :n],
+                                               key_mask=key_mask, past=past)
+            else:
+                # 16-bit: the cache itself; an FP8 prefill from position 0: the rewritten k / v; after cached
+                # positions: the cache's first n positions dequantised into a workspace
+                if not fp8:
+                    k, v = c.k[:, :n], c.v[:, :n]
+                elif past > 0:
+                    k = ops.kv_dequantize_fp8(c.k[:, :n], c.k_scale[:, :n], q.dtype)
+                    v = ops.kv_dequantize_fp8(c.v[:, :n], c.v_scale[:, :n], q.dtype)
+                ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)
         else:
             ops.rope_qk_(q, k, cos, sin, position_ids)
             if past_key_value is not None:
                 k = torch.cat([past_key_value[0], k], dim=1)
                 v = torch.cat([past_key_value[1], v], dim=1)
             present = (k, v) if use_cache else None
-        key_mask = None
-        if attention_mask is not None:
-            if attention_mask.dim() == 4:   # reference-style additive (B,1,T,T_kv): keys visible to the last query
-                key_mask = attention_mask[:, 0, -1, :] > (torch.finfo(attention_mask.dtype).min / 2)
-            else:
-                key_mask = attention_mask
-        if shared:
-            c = past_key_value
-            ctx = ops.attention_decode_shared(q, c.k, c.v, c.k_gen, c.v_gen, c.prefix_len, key_mask=key_mask, past=past)
-        else:
             ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)   # (B, T, H*hd)
         out = decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace)
         return out, None, present
@@ -389,43 +404,6 @@ class LlamaAttention(nn.Module):
         ctx = ops.attention_prefix_shared(q, c.k, c.v, k, v, c.seg_len, prefix_mask=c.prefix_mask, key_mask=attention_mask)
         return decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace), None, None
 
-    def _forward_fp8(self, q, k, v, cos, sin, position_ids, c, past, attention_mask, residual, inplace):
-        """The layer over an FP8 cache (``StaticKV`` / ``SharedPrefixKV`` with scales).  ``ops.rope_qk_append_fp8_``
-        appends the rotated keys and the values as E4M3 and rewrites the k / v views with ``x8 * scale``; then a decode
-        step (T == 1) attends over the FP8 cache directly, a prefill from position 0 runs the 16-bit attention on the
-        rewritten views, and a prefill after cached positions runs it on the cache's first ``past + T`` positions
-        dequantised into a workspace.  Every path sees the keys and values ``x8 * scale``."""
-        B, T = q.shape[:2]
-        shared = isinstance(c, SharedPrefixKV)
-        if (shared or c.slot is not None) and T != 1:
-            raise RuntimeError("a graph-decode cache (SharedPrefixKV, StaticKV.slot) takes one token per step")
-        key_mask = attention_mask
-        if attention_mask is not None and attention_mask.dim() == 4:
-            key_mask = attention_mask[:, 0, -1, :] > (torch.finfo(attention_mask.dtype).min / 2)
-        if shared:
-            ops.rope_qk_append_fp8_(q, k, v, cos, sin, position_ids, c.k_gen, c.v_gen, c.ks_gen, c.vs_gen, c.slot)
-            ctx = ops.attention_decode_shared_fp8(q, c.k, c.v, c.k_scale, c.v_scale, c.k_gen, c.v_gen, c.ks_gen, c.vs_gen,
-                                                  c.prefix_len, key_mask=key_mask, past=past)
-        else:
-            if c.slot is not None:                              # graph decode: device-side slot, whole buffer visible
-                slot, n, past = c.slot, c.k.shape[1], c.k.shape[1] - 1
-            else:
-                if past + T > c.k.shape[1]:
-                    raise RuntimeError(f"StaticKV of {c.k.shape[1]} positions cannot take {past} + {T}")
-                slot, n = past, past + T
-                c.length = n
-            ops.rope_qk_append_fp8_(q, k, v, cos, sin, position_ids, c.k, c.v, c.k_scale, c.v_scale, slot)
-            if T == 1:
-                ctx = ops.attention_decode_fp8(q, c.k[:, :n], c.v[:, :n], c.k_scale[:, :n], c.v_scale[:, :n],
-                                               key_mask=key_mask, past=past)
-            else:
-                if past > 0:
-                    k = ops.kv_dequantize_fp8(c.k[:, :n], c.k_scale[:, :n], q.dtype)
-                    v = ops.kv_dequantize_fp8(c.v[:, :n], c.v_scale[:, :n], q.dtype)
-                ctx = ops.attention(q, k, v, key_mask=key_mask, causal=True, past=past)
-        out = decode_linear(ctx, self.o_proj.weight, self._fp8, "o", residual=residual, inplace=inplace)
-        return out, None, c
-
     def _forward_training(self, hidden_states, attention_mask, position_ids, past_key_value, use_cache, residual):
         """The prefill under autograd: QKV GEMM -> RoPE -> causal attention (saving O and the row log-sum-exp) -> o_proj,
         each step with its backward (autograd_ops)."""
@@ -442,10 +420,7 @@ class LlamaAttention(nn.Module):
             position_ids = torch.arange(T, device=hidden_states.device)
         cos, sin = self.rope_tables(hidden_states.device, T)
         qkv = autograd_ops.rope_qkv(qkv, cos, sin, position_ids)
-        key_mask = attention_mask
-        if attention_mask is not None and attention_mask.dim() == 4:
-            key_mask = attention_mask[:, 0, -1, :] > (torch.finfo(attention_mask.dtype).min / 2)
-        ctx = autograd_ops.attention(qkv, key_mask)
+        ctx = autograd_ops.attention(qkv, _key_mask(attention_mask))
         out = self.o_proj(ctx) if residual is None else _addmm_residual(residual, ctx, self.o_proj.weight, False)
         return out, None, None
 

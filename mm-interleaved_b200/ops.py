@@ -415,16 +415,9 @@ def attention_decode_shared(q, k_prefix, v_prefix, k_gen, v_gen, prefix_len, key
     _require(P > 0 and R % P == 0, "attention_decode_shared: the rows must be whole groups, one per prefix row")
     _require(prefix_len.device == q.device and prefix_len.dtype == torch.int64 and prefix_len.numel() == 1,
              "attention_decode_shared: prefix_len must be a (1,) int64 device tensor")
-    scale = float(scale if scale is not None else hd ** -0.5)
-    out = torch.empty((R, 1, H, hd), dtype=q.dtype, device=q.device)
-    km = None
-    if key_mask is not None:
-        km = key_mask.to(torch.uint8).contiguous()
-        _require(tuple(km.shape) == (R, Tkv), "attention_decode_shared: key_mask must be (R, T_p + max_new)")
-    lib = _lib.lib()
-    scratch = torch.empty((lib.mmfs_attn_decode_scratch_floats(R, H, Tkv, hd),), dtype=torch.float32, device=q.device)
+    scale, km, out, scratch = _decode_setup("attention_decode_shared", q, R, Tkv, key_mask, scale)
     with torch.cuda.device(q.device):
-        rc = lib.mmfs_attn_decode_shared(q.data_ptr(), k_prefix.data_ptr(), v_prefix.data_ptr(), k_gen.data_ptr(),
+        rc = _lib.lib().mmfs_attn_decode_shared(q.data_ptr(), k_prefix.data_ptr(), v_prefix.data_ptr(), k_gen.data_ptr(),
                                          v_gen.data_ptr(), out.data_ptr(), km.data_ptr() if km is not None else None,
                                          prefix_len.data_ptr(), scratch.data_ptr(), R, R // P, H, Tkv, Tp, max_new, hd,
                                          q.stride(0), k_prefix.stride(0), k_prefix.stride(1), v_prefix.stride(0),
@@ -1062,15 +1055,24 @@ def rope_qk_append_fp8_(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cos: 
     launch_counter[0] += 1
 
 
-def _check_decode_q(what, q, rows, key_mask, Tkv):
+def _check_decode_q(what, q, rows):
     _require(q.is_cuda and q.dtype in _KV_FP8_DTYPES and q.dim() == 4 and q.shape[0] == rows
              and q.shape[1] == 1 and q.stride(3) == 1 and q.stride(2) == q.shape[3],
              f"{what}: q must be an fp32 / bf16 / fp16 CUDA (rows, 1, H, hd) tensor with dense heads")
-    if key_mask is None:
-        return None
-    km = key_mask.to(torch.uint8).contiguous()
-    _require(tuple(km.shape) == (rows, Tkv), f"{what}: key_mask must be ({rows}, {Tkv})")
-    return km
+
+
+def _decode_setup(what, q, rows, Tkv, key_mask, scale):
+    """What the decode wrappers share: the softmax scale (hd ** -0.5 by default), the key mask as a contiguous
+    (rows, Tkv) uint8 tensor or None, the (rows, 1, H, hd) output and the ``mmfs_attn_decode_scratch_floats`` scratch."""
+    H, hd = q.shape[2], q.shape[3]
+    km = None
+    if key_mask is not None:
+        km = key_mask.to(torch.uint8).contiguous()
+        _require(tuple(km.shape) == (rows, Tkv), f"{what}: key_mask must be ({rows}, {Tkv})")
+    out = torch.empty((rows, 1, H, hd), dtype=q.dtype, device=q.device)
+    scratch = torch.empty((_lib.lib().mmfs_attn_decode_scratch_floats(rows, H, Tkv, hd),), dtype=torch.float32,
+                          device=q.device)
+    return float(scale if scale is not None else hd ** -0.5), km, out, scratch
 
 
 def attention_decode_fp8(q, k8, v8, k_scale, v_scale, key_mask=None, causal=True, past=0, scale=None) -> torch.Tensor:
@@ -1081,14 +1083,11 @@ def attention_decode_fp8(q, k8, v8, k_scale, v_scale, key_mask=None, causal=True
     B, _, H, hd = q.shape
     Tkv = k8.shape[1] if k8.dim() == 4 else 0
     inference_only("attention_decode_fp8", q)
-    km = _check_decode_q("attention_decode_fp8", q, B, key_mask, Tkv)
+    _check_decode_q("attention_decode_fp8", q, B)
     _check_fp8_cache("attention_decode_fp8", k8, v8, k_scale, v_scale, B, H, hd, q.device)
-    scale = float(scale if scale is not None else hd ** -0.5)
-    out = torch.empty((B, 1, H, hd), dtype=q.dtype, device=q.device)
-    lib = _lib.lib()
-    scratch = torch.empty((lib.mmfs_attn_decode_scratch_floats(B, H, Tkv, hd),), dtype=torch.float32, device=q.device)
+    scale, km, out, scratch = _decode_setup("attention_decode_fp8", q, B, Tkv, key_mask, scale)
     with torch.cuda.device(q.device):
-        rc = lib.mmfs_attn_decode_fp8(q.data_ptr(), k8.data_ptr(), v8.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
+        rc = _lib.lib().mmfs_attn_decode_fp8(q.data_ptr(), k8.data_ptr(), v8.data_ptr(), k_scale.data_ptr(), v_scale.data_ptr(),
                                       out.data_ptr(), km.data_ptr() if km is not None else None, scratch.data_ptr(), B, H,
                                       Tkv, hd, q.stride(0), k8.stride(0), k8.stride(1), k_scale.stride(0), k_scale.stride(1),
                                       out.stride(0), scale, 1 if causal else 0, int(past), _DTYPE_CODE[q.dtype], _stream())
@@ -1108,18 +1107,15 @@ def attention_decode_shared_fp8(q, k_prefix, v_prefix, ks_prefix, vs_prefix, k_g
     max_new = k_gen.shape[1] if k_gen.dim() == 4 else 0
     Tkv = Tp + max_new
     inference_only("attention_decode_shared_fp8", q)
-    km = _check_decode_q("attention_decode_shared_fp8", q, R, key_mask, Tkv)
+    _check_decode_q("attention_decode_shared_fp8", q, R)
     _require(P > 0 and R % P == 0, "attention_decode_shared_fp8: the rows must be whole groups, one per prefix row")
     _check_fp8_cache("attention_decode_shared_fp8", k_prefix, v_prefix, ks_prefix, vs_prefix, P, H, hd, q.device)
     _check_fp8_cache("attention_decode_shared_fp8", k_gen, v_gen, ks_gen, vs_gen, R, H, hd, q.device)
     _require(prefix_len.device == q.device and prefix_len.dtype == torch.int64 and prefix_len.numel() == 1,
              "attention_decode_shared_fp8: prefix_len must be a (1,) int64 device tensor")
-    scale = float(scale if scale is not None else hd ** -0.5)
-    out = torch.empty((R, 1, H, hd), dtype=q.dtype, device=q.device)
-    lib = _lib.lib()
-    scratch = torch.empty((lib.mmfs_attn_decode_scratch_floats(R, H, Tkv, hd),), dtype=torch.float32, device=q.device)
+    scale, km, out, scratch = _decode_setup("attention_decode_shared_fp8", q, R, Tkv, key_mask, scale)
     with torch.cuda.device(q.device):
-        rc = lib.mmfs_attn_decode_shared_fp8(
+        rc = _lib.lib().mmfs_attn_decode_shared_fp8(
             q.data_ptr(), k_prefix.data_ptr(), v_prefix.data_ptr(), ks_prefix.data_ptr(), vs_prefix.data_ptr(),
             k_gen.data_ptr(), v_gen.data_ptr(), ks_gen.data_ptr(), vs_gen.data_ptr(), out.data_ptr(),
             km.data_ptr() if km is not None else None, prefix_len.data_ptr(), scratch.data_ptr(), R, R // P, H, Tkv, Tp,
